@@ -6,7 +6,9 @@
 #include "hb_lowrank.cuh"
 #include <cstdlib>
 
-int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc);
+int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
+                 const double* fuse_rx = nullptr, double* tdot = nullptr);
+bool hb_syrk_extra_row_is_free(int M);
 int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
                        const double* dot_x, double* dot_out);
 
@@ -538,7 +540,9 @@ int do_condense(hb_lowrank* k)
 
 // fuse_rx (optional): the x-block of the right-hand side the caller is about to solve for. The int8-slice condensation has to sweep all
 // rows for their maxima anyway; the same sweep then leaves tdot = [J; S; Y] (DhInv .* rx), from which step 2 of solveCompressed follows
-// without reading J again (see solve_compressed).
+// without reading J again (see solve_compressed). The FP64 kernel computes the same dots as one more row of its SYRK, which is free
+// when it fits in the padding of the last 128-row tile (otherwise a whole tile row would cost more than the sweep it saves); rx must be
+// 16-byte aligned to keep the fast kernel.
 int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
 {
   hb_ctx* c = k->ctx;
@@ -546,8 +550,11 @@ int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
   k->tdot_valid = false;
   if(Ma > 0) {
     k->condense_used = mode;
-    if(mode == 0) HB_CHECK(hb_syrk_rows(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma));
-    else {
+    if(mode == 0) {
+      const bool fuse = fuse_rx && m > 0 && hb_syrk_extra_row_is_free(Ma) && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
+      HB_CHECK(hb_syrk_rows(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, fuse ? fuse_rx : nullptr, fuse ? k->tdot : nullptr));
+      k->tdot_valid = fuse;
+    } else {
       const bool fuse = fuse_rx && m > 0;
       if(fuse && k->n == 0) HB_CUDA(cudaMemsetAsync(k->tdot, 0, sizeof(double) * Ma, c->stream));
       HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot : nullptr));
@@ -955,9 +962,9 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   }
   if(have_J) HB_CHECK(hb_lowrank_set_jacobian(k, k->hJ, k->hJ + (size_t)meq * n));
   HB_CHECK(hb_lowrank_update(k, k->hbuf[0], k->hbuf[1], k->hbuf[2], k->hbuf[3], k->hbuf[4], k->hbuf[5], k->hbuf[6], k->hbuf[7]));
-  if(!chunked) {
-    HB_CHECK(do_condense(k));
-  } else {
+  // Not chunked: the condensation stays pending so that solve_compressed below runs it with rx fused, exactly as a device-side
+  // update + solveCompressed does; breakdowns are reported after the solve.
+  if(chunked) {
     constexpr int NCH = 16;
     if(!k->copy_stream) {
       HB_CUDA(cudaStreamCreateWithFlags(&k->copy_stream, cudaStreamNonBlocking));
@@ -1010,6 +1017,7 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
     HB_CHECK(condense_check(k));
   }
   HB_CHECK(hb_lowrank_solve_compressed(k, k->hbuf[8], k->hbuf[9], k->hbuf[10], k->hbuf[11], k->hbuf[12], k->hbuf[13]));
+  HB_CHECK(condense_check(k));
   if(n) HB_CUDA(cudaMemcpyAsync(dx, k->hbuf[11], sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
   if(meq) HB_CUDA(cudaMemcpyAsync(dyc, k->hbuf[12], sizeof(double) * meq, cudaMemcpyDeviceToHost, c->stream));
   if(mi) HB_CUDA(cudaMemcpyAsync(dyd, k->hbuf[13], sizeof(double) * mi, cudaMemcpyDeviceToHost, c->stream));

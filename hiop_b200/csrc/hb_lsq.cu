@@ -12,7 +12,8 @@
 #include "hb_dense.cuh"
 #include "../../include/hiopb200.h"
 
-int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc);
+int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
+                 const double* fuse_rx = nullptr, double* tdot = nullptr);
 int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
                        const double* dot_x, double* dot_out);
 

@@ -12,8 +12,9 @@
 // Work decomposition: 128x128 output tiles (upper triangle of the tile grid only), K swept in BK=16 chunks through a
 // 4-stage cp.async pipeline into padded shared memory (row stride 20 doubles = 160 B -> the m8n8k4 fragment reads
 // of a half-warp, 4 rows x 32 B, fall into 4 distinct 32 B bank groups: conflict-free LDS.64).
-// The (tile, K-range) space is cut into one contiguous range per CTA by a host-side schedule (stream-K): every SM
-// gets the same number of MMA iterations whatever M is. Each CTA writes its partial 128x128 tile to a workspace
+// The (tile, K-range) space is cut into one (tile, K window) per CTA in K lanes, plus stream-K ranges for the CTAs left
+// over (see build_schedule): every SM gets the same number of MMA iterations whatever M is, and the tiles of a lane
+// read the same columns at the same time. Each CTA writes its partial 128x128 tile to a workspace
 // slot; a second kernel sums the slots of each tile in a FIXED order and mirrors the result, so the output is
 // bit-reproducible run to run (no atomics).
 #include "hb_common.cuh"
@@ -129,8 +130,8 @@ __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_
 
 template <bool ALIGN16>
 __global__ void __launch_bounds__(THREADS, 1)
-k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const Seg* __restrict__ segs,
-            const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
+k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const double* __restrict__ extra_row,
+            const Seg* __restrict__ segs, const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
 {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Stage* stages = reinterpret_cast<Stage*>(smem_raw);
@@ -149,10 +150,10 @@ k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const 
     __syncthreads(); // previous segment fully consumed before the row tables / stages are reused
     if(tid < BM) {
       const int ra = sg.ti * BM + tid;
-      srow_a[tid] = ra < M ? rowptr[ra] : nullptr;
+      srow_a[tid] = ra < M ? rowptr[ra] : (ra == M ? extra_row : nullptr);
     } else {
       const int rb = sg.tj * BM + (tid - BM);
-      srow_b[tid - BM] = rb < M ? rowptr[rb] : nullptr;
+      srow_b[tid - BM] = rb < M ? rowptr[rb] : (rb == M ? extra_row : nullptr);
     }
     __syncthreads();
 
@@ -261,8 +262,8 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
 }
 
 __global__ void __launch_bounds__(WTHREADS, 1)
-k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const Seg* __restrict__ segs,
-          const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
+k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const double* __restrict__ extra_row,
+          const Seg* __restrict__ segs, const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
 {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   WStage* stages = reinterpret_cast<WStage*>(smem_raw);
@@ -297,7 +298,7 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
       asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory"); // all producers done with the previous segment's row table
       for(int r = p; r < 2 * BM; r += WPROD) {
         const int grow = (r < BM ? sg.ti * BM + r : sg.tj * BM + (r - BM));
-        srow[r] = grow < M ? rowptr[grow] : nullptr;
+        srow[r] = grow < M ? rowptr[grow] : (grow == M ? extra_row : nullptr);
       }
       asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory");
       for(int it = 0; it < sg.k_count; it++) {
@@ -372,10 +373,11 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
   }
 }
 
-// Sums the partial slots of each tile in schedule order and writes C (both triangles).
+// Sums the partial slots of each tile in schedule order and writes C (both triangles); with an extra row (tdot != NULL) its products
+// with rows 0..M-1 (column M of the result) go to tdot.
 __global__ void __launch_bounds__(256)
 k_syrk_fixup(int M, const int2* __restrict__ tile_ij, const int* __restrict__ tile_slot_begin, const int* __restrict__ tile_slots,
-             const double* __restrict__ ws, double* __restrict__ C, int ldc)
+             const double* __restrict__ ws, double* __restrict__ C, int ldc, double* __restrict__ tdot)
 {
   const int t = blockIdx.x;
   const int2 ij = tile_ij[t];
@@ -384,10 +386,14 @@ k_syrk_fixup(int M, const int2* __restrict__ tile_ij, const int* __restrict__ ti
   for(int e = threadIdx.x; e < 16 * BM; e += 256) {
     const int r = r0 + e / BM, c = e % BM;
     const int gi = ij.x * BM + r, gj = ij.y * BM + c;
-    if(gi >= M || gj >= M) continue;
+    if(gi >= M || gj > M || (gj == M && !tdot)) continue;
     if(ij.x == ij.y && c < r) continue; // diagonal tile: use the upper part and mirror it (exact symmetry)
     double v = 0.0;
     for(int s = s0; s < s1; s++) v += ws[(size_t)tile_slots[s] * (BM * BM) + r * BM + c];
+    if(gj == M) {
+      tdot[gi] = v;
+      continue;
+    }
     C[(size_t)gi * ldc + gj] = v;
     C[(size_t)gj * ldc + gi] = v;
   }
@@ -442,20 +448,45 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   std::vector<Seg> segs;
   std::vector<int> cta_begin(G + 1, 0);
   std::vector<std::vector<int>> per_tile(ntiles);
-  for(int cta = 0; cta < G; cta++) {
-    cta_begin[cta] = (int)segs.size();
-    long long it = hb_part_begin(total, G, cta), end = hb_part_begin(total, G, cta + 1);
-    while(it < end) {
-      const int tile = (int)(it / kiters);
-      const long long kk0 = it % kiters;
-      long long cnt = kiters - kk0;
-      if(cnt > end - it) cnt = end - it;
-      Seg s;
-      s.ti = tij[tile].x; s.tj = tij[tile].y; s.k_begin = (int)kk0; s.k_count = (int)cnt; s.slot = (int)segs.size();
-      per_tile[tile].push_back(s.slot);
-      segs.push_back(s);
-      it += cnt;
+  auto push = [&](int tile, long long k0, long long cnt) {
+    Seg s;
+    s.ti = tij[tile].x; s.tj = tij[tile].y; s.k_begin = (int)k0; s.k_count = (int)cnt; s.slot = (int)segs.size();
+    per_tile[tile].push_back(s.slot);
+    segs.push_back(s);
+  };
+  // stream-K: CTAs cta0 .. cta0+nct-1 take equal contiguous ranges of the tile-major space (tile, k in [kfirst, kiters))
+  auto stream_k = [&](int cta0, int nct, long long kfirst) {
+    const long long w = kiters - kfirst, tot = (long long)ntiles * w;
+    for(int cta = 0; cta < nct; cta++) {
+      cta_begin[cta0 + cta] = (int)segs.size();
+      long long it = hb_part_begin(tot, nct, cta), end = hb_part_begin(tot, nct, cta + 1);
+      while(it < end) {
+        const int tile = (int)(it / w);
+        const long long kk0 = it % w;
+        long long cnt = w - kk0;
+        if(cnt > end - it) cnt = end - it;
+        push(tile, kfirst + kk0, cnt);
+        it += cnt;
+      }
     }
+  };
+  // K lanes: when every tile can have a CTA of its own (G >= ntiles), CTA lane*ntiles + t runs tile t over the K window of its lane, so
+  // all tiles of a lane read the same columns of [J; S; Y] at the same time and each panel chunk comes from DRAM about once per lane
+  // (with stream-K alone the CTAs of the 8 tiles that share a panel sit at unrelated K offsets, and J is re-read from DRAM). The
+  // R = G - L*ntiles CTAs left over take the columns after the lanes stream-K style. A lane CTA runs floor(total / G) iterations, the
+  // others at most ceil((total mod G) / R) more.
+  const int L = G / ntiles, R = G - L * ntiles;
+  const long long w = L < 1 ? 0 : (R ? total / G : kiters / L);
+  if(L >= 1 && w >= 1) {
+    for(int lane = 0; lane < L; lane++)
+      for(int t = 0; t < ntiles; t++) {
+        cta_begin[lane * ntiles + t] = (int)segs.size();
+        const long long k0 = R ? lane * w : hb_part_begin(kiters, L, lane), k1 = R ? k0 + w : hb_part_begin(kiters, L, lane + 1);
+        push(t, k0, k1 - k0);
+      }
+    if(R) stream_k(L * ntiles, R, L * w);
+  } else {
+    stream_k(0, G, 0);
   }
   cta_begin[G] = (int)segs.size();
   std::vector<int> tsb(ntiles + 1, 0), tsl;
@@ -484,22 +515,29 @@ bool g_attr_set = false;
 
 } // namespace
 
+// true when an (M+1)-th row adds no tile row to the SYRK of M rows (hb_syrk_rows' fuse_rx costs no extra MMA)
+bool hb_syrk_extra_row_is_free(int M) { return (M + BM) / BM == (M + BM - 1) / BM; }
+
 // rowptr: DEVICE table of M row pointers (each row K doubles, K-contiguous). d: length K (device) or NULL (= ones).
 // C: M x M (ldc), both triangles written. `aligned16`: every row pointer and d are 16-byte aligned.
-int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc)
+// fuse_rx (optional, device, length K): swept as row M of the same pass; tdot[i] = sum_k row_i[k] d[k] fuse_rx[k] for i < M. It costs
+// no extra MMA when M + 1 rows need no more 128-row tiles than M.
+int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
+                 const double* fuse_rx, double* tdot)
 {
-  HB_REQUIRE(c && M >= 0 && K >= 0 && ldc >= M, "hb_syrk_rows: bad arguments");
+  HB_REQUIRE(c && M >= 0 && K >= 0 && ldc >= M && (fuse_rx == nullptr) == (tdot == nullptr), "hb_syrk_rows: bad arguments");
   if(M == 0) return HB_OK;
   if(K == 0) {
     HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
+    if(tdot) HB_CUDA(cudaMemsetAsync(tdot, 0, sizeof(double) * M, c->stream));
     return HB_OK;
   }
   HB_REQUIRE(c->device < 16, "device ordinal too large");
-  const bool d_aligned = (reinterpret_cast<uintptr_t>(d) & 15u) == 0;
+  const bool d_aligned = (reinterpret_cast<uintptr_t>(d) & 15u) == 0 && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
   const char* force_generic = getenv("HB_SYRK_GENERIC");
   const bool use_ws = aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0) && !(force_generic && force_generic[0] == '1');
   Schedule* Sp = nullptr;
-  HB_CHECK(build_schedule(c, Sp, M, K, use_ws ? WBK : BK));
+  HB_CHECK(build_schedule(c, Sp, M + (fuse_rx ? 1 : 0), K, use_ws ? WBK : BK));
   Schedule& S = *Sp;
   HB_CHECK(hb_ws_reserve(c, (size_t)S.nslots * BM * BM * sizeof(double)));
   if(!g_attr_set) {
@@ -511,17 +549,17 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
   const int G = S.Gl;
   if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
   if(use_ws)
-    k_syrk_ws<<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    k_syrk_ws<<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
   else if(aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0))
-    k_syrk_diag<true><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    k_syrk_diag<true><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
   else
-    k_syrk_diag<false><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    k_syrk_diag<false><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
   HB_LAUNCHED();
   if(c->timing) {
     HB_CUDA(cudaEventRecord(c->ev_syrk1, c->stream));
     c->syrk_timed = true;
   }
-  k_syrk_fixup<<<dim3(S.ntiles, BM / 16), 256, 0, c->stream>>>(M, S.d_tile_ij, S.d_tile_slot_begin, S.d_tile_slots, (const double*)c->ws, C, ldc);
+  k_syrk_fixup<<<dim3(S.ntiles, BM / 16), 256, 0, c->stream>>>(M, S.d_tile_ij, S.d_tile_slot_begin, S.d_tile_slots, (const double*)c->ws, C, ldc, tdot);
   HB_LAUNCHED();
   return HB_OK;
 }
