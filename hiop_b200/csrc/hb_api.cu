@@ -35,6 +35,10 @@ extern "C" int hb_ctx_create(int device, hb_ctx** out)
   HB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   HB_CUDA(cudaMalloc(&c->red_dev, sizeof(double) * HB_RED_SLOTS));
   HB_CUDA(cudaMallocHost(&c->red_host, sizeof(double) * 64));
+  HB_CHECK(hb_syrk_init_attrs(c));
+  HB_CHECK(hb_ozaki_init_attrs(c));
+  HB_CHECK(hb_microbench_init_attrs(c));
+  HB_CHECK(hb_dense_init(c));
   *out = c;
   return HB_OK;
 }
@@ -45,6 +49,8 @@ extern "C" int hb_ctx_destroy(hb_ctx* c)
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   if(c->oz_state && c->oz_free) c->oz_free(c->oz_state);
+  if(c->syrk_sched && c->syrk_free) c->syrk_free(c->syrk_sched);
+  cudaFree(c->bkc_prof);
   for(cudaEvent_t e : c->ev_phase) if(e) cudaEventDestroy(e);
   if(c->ws) cudaFree(c->ws);
   if(c->ev_syrk0) { cudaEventDestroy(c->ev_syrk0); cudaEventDestroy(c->ev_syrk1); }

@@ -6,7 +6,7 @@
 // DSYTF2 / DLASYF ('L'), same inertia. oracle/bk_model.py is the numpy statement of exactly this organisation (tested against DSYTRF).
 //
 // Why a cluster: the pivot search needs the maximum of the whole current column once per column -- N global reductions per
-// factorization. A grid-wide barrier per column adds up over thousands of columns, the one-CTA panel of hb_bk.cu streams the panel through
+// factorization. A grid-wide barrier per column adds up over thousands of columns, the one-CTA DLASYF panel of hb_dense.cu streams the panel through
 // one SM. A cluster barrier is far cheaper (tools/cluster_probe.cu) and 16 SMs hold a 32-column panel of 13000 rows in shared memory.
 //
 //   * CTA r owns a contiguous slab of rows; slab[c][row] is kept RIGHT-LOOKING inside the panel (after each pivot the remaining
@@ -29,48 +29,10 @@ namespace cg = cooperative_groups;
 
 namespace {
 
-#define LC(A, lda, i, j) (A)[(size_t)(j) * (lda) + (i)]
-
 constexpr int CS = 16;     // CTAs per cluster
 constexpr int PT = 1024;   // threads per CTA
 constexpr int NBMAX = 64;  // widest panel (used when the slab of 64 columns fits in the cluster's shared memory)
-#define BK_ALPHA 0.6403882032022076
 
-struct ArgMax
-{
-  double v;
-  int i;
-};
-__device__ __forceinline__ ArgMax am_comb(ArgMax a, ArgMax b)
-{
-  if(b.v > a.v || (b.v == a.v && b.i < a.i)) return b; // IDAMAX: first index of the maximum
-  return a;
-}
-__device__ ArgMax cta_argmax(ArgMax a, ArgMax* sm)
-{
-#pragma unroll
-  for(int o = 16; o > 0; o >>= 1) {
-    ArgMax b;
-    b.v = __shfl_xor_sync(0xffffffffu, a.v, o);
-    b.i = __shfl_xor_sync(0xffffffffu, a.i, o);
-    a = am_comb(a, b);
-  }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  __syncthreads();
-  if(lane == 0) sm[warp] = a;
-  __syncthreads();
-  // second stage by shuffles in every warp (a loop over the 32 partials in all 1024 threads cost ~2500 cycles of LDS traffic per column)
-  ArgMax r{-1.0, 0x7fffffff};
-  if(lane < (int)(blockDim.x >> 5)) r = sm[lane];
-#pragma unroll
-  for(int o = 16; o > 0; o >>= 1) {
-    ArgMax b;
-    b.v = __shfl_xor_sync(0xffffffffu, r.v, o);
-    b.i = __shfl_xor_sync(0xffffffffu, r.i, o);
-    r = am_comb(r, b);
-  }
-  return r;
-}
 // the 16 per-CTA candidates of a mailbox -> the cluster-wide maximum (every warp by shuffles)
 template <typename IT>
 __device__ __forceinline__ ArgMax mailbox_argmax(const double* v, const IT* idx)
@@ -83,7 +45,7 @@ __device__ __forceinline__ ArgMax mailbox_argmax(const double* v, const IT* idx)
     ArgMax b;
     b.v = __shfl_xor_sync(0xffffffffu, r.v, o);
     b.i = __shfl_xor_sync(0xffffffffu, r.i, o);
-    r = am_comb(r, b);
+    r = argmax_comb(r, b);
   }
   r.v = __shfl_sync(0xffffffffu, r.v, 0);
   r.i = __shfl_sync(0xffffffffu, r.i, 0);
@@ -200,7 +162,7 @@ k_bk_panel(double* __restrict__ A, long long lda, int N, double* __restrict__ W,
       ArgMax a{-1.0, big};
       for(int rl = tid; rl < S; rl += nthr) {
         const int i = lo + rl;
-        if(i < N && i > k) a = am_comb(a, ArgMax{fabs(slab[(size_t)kl * S + rl]), i});
+        if(i < N && i > k) a = argmax_comb(a, ArgMax{fabs(slab[(size_t)kl * S + rl]), i});
       }
       a = cta_argmax(a, sh.am);
       // this step's mail: 16 candidates (value + index) from the 16 CTAs and the top of column k from CTA 0
@@ -280,7 +242,7 @@ k_bk_panel(double* __restrict__ A, long long lda, int N, double* __restrict__ W,
             for(int c = 0; c < kl; c++) acc += slab[(size_t)c * S + rl] * sh.vld[c];
             cv = raw - acc;
           }
-          if(i != imax) a2 = am_comb(a2, ArgMax{fabs(cv), i});
+          if(i != imax) a2 = argmax_comb(a2, ArgMax{fabs(cv), i});
         }
         ccol[rl] = cv;
       }
@@ -630,13 +592,19 @@ k_inertia_par(const double* __restrict__ F, long long ldf, int N, const int* __r
   if(threadIdx.x < 3) out[threadIdx.x] = cnt[threadIdx.x];
 }
 
-bool g_bkc_attr[16] = {false};
-long long* g_bkc_prof = nullptr; // diagnostics: device array of 8 cycle counters when profiling is on
-
 } // namespace
 
 // geometry of one cluster panel with `rows` active rows: rows per CTA (S), panel width (NB: the widest of 64/32/16/8 whose slab fits),
 // dynamic shared memory
+int hb_bkc_init_attrs(hb_ctx* c)
+{
+  HB_CUDA(cudaFuncSetAttribute(k_bk_panel<false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  HB_CUDA(cudaFuncSetAttribute(k_bk_panel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  HB_CUDA(cudaFuncSetAttribute(k_bk_panel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  HB_CUDA(cudaFuncSetAttribute(k_bk_panel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  return HB_OK;
+}
+
 static void bkc_geometry(int rows, int* S, int* NB, size_t* smem)
 {
   int s = (rows + CS - 1) / CS;
@@ -651,7 +619,7 @@ static void bkc_geometry(int rows, int* S, int* NB, size_t* smem)
   *smem = ((size_t)nb * s + s) * sizeof(double) + 2 * sizeof(BkStep);
 }
 
-bool hb_bkc_supported(hb_ctx* c, int N)
+bool hb_bkc_supported(int N)
 {
   int S, NB;
   size_t smem;
@@ -668,13 +636,6 @@ int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ip
   double* swap_scratch = Wp + (size_t)NBMAX * ldw; // Wp holds NBMAX columns of W followed by 2*NBMAX rows of staging for the interchanges
   HB_REQUIRE((lda & 1) == 0, "hb_bkc_factor: needs an even leading dimension");
   HB_CHECK(hb_big_init(c, b));
-  if(c->device < 16 && !g_bkc_attr[c->device]) {
-    HB_CUDA(cudaFuncSetAttribute(k_bk_panel<false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    HB_CUDA(cudaFuncSetAttribute(k_bk_panel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    HB_CUDA(cudaFuncSetAttribute(k_bk_panel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-    HB_CUDA(cudaFuncSetAttribute(k_bk_panel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    g_bkc_attr[c->device] = true;
-  }
   cudaStream_t st = c->stream, side = b->panel_stream;
   HB_CUDA(cudaMemsetAsync(state_dev, 0, sizeof(int) * 4, st));
   k_iota<<<(N + 255) / 256, 256, 0, st>>>(N, perm_dev, dsub_dev);
@@ -688,7 +649,7 @@ int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ip
     bkc_geometry(N - k0_min, &S, &NB, &smem);
     int threads = S < PT ? S : PT; // one row per thread where possible: fewer idle warps in every barrier / shuffle stage
     if(threads < 128) threads = 128;
-    if(g_bkc_prof) k_bk_panel<true><<<CS, threads, smem, st>>>(A, lda, N, Wp, ldw, NB, S, ipiv_dev, dsub_dev, state_dev, swaplog_dev, p, g_bkc_prof);
+    if(c->bkc_prof) k_bk_panel<true><<<CS, threads, smem, st>>>(A, lda, N, Wp, ldw, NB, S, ipiv_dev, dsub_dev, state_dev, swaplog_dev, p, c->bkc_prof);
     else k_bk_panel<false><<<CS, threads, smem, st>>>(A, lda, N, Wp, ldw, NB, S, ipiv_dev, dsub_dev, state_dev, swaplog_dev, p, nullptr);
     HB_LAUNCHED();
     // the interchanges on the previous columns and on the permutation run beside the trailing update (disjoint data)
@@ -712,11 +673,16 @@ int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ip
   return HB_OK;
 }
 
-int hb_bkc_inertia(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, int* out3_dev)
+int hb_dense_inertia_blockdiag(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, int* out3_dev)
 {
   k_inertia_par<<<1, 1024, 0, c->stream>>>(F, ldf, N, ipiv_dev, dsub_dev, out3_dev);
   HB_LAUNCHED();
   return HB_OK;
+}
+
+int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev)
+{
+  return hb_dense_inertia_blockdiag(c, N, F, ldf, nullptr, nullptr, out3_dev);
 }
 
 int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, double* x)
@@ -730,15 +696,15 @@ int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* i
 int hb_bkc_profile(hb_ctx* c, int on, long long* prof_host8)
 {
   if(on) {
-    if(!g_bkc_prof) HB_CUDA(cudaMalloc(&g_bkc_prof, sizeof(long long) * 8));
-    HB_CUDA(cudaMemsetAsync(g_bkc_prof, 0, sizeof(long long) * 8, c->stream));
-  } else if(g_bkc_prof) {
+    if(!c->bkc_prof) HB_CUDA(cudaMalloc(&c->bkc_prof, sizeof(long long) * 8));
+    HB_CUDA(cudaMemsetAsync(c->bkc_prof, 0, sizeof(long long) * 8, c->stream));
+  } else if(c->bkc_prof) {
     if(prof_host8) {
-      HB_CUDA(cudaMemcpyAsync(prof_host8, g_bkc_prof, sizeof(long long) * 8, cudaMemcpyDeviceToHost, c->stream));
+      HB_CUDA(cudaMemcpyAsync(prof_host8, c->bkc_prof, sizeof(long long) * 8, cudaMemcpyDeviceToHost, c->stream));
       HB_CUDA(cudaStreamSynchronize(c->stream));
     }
-    cudaFree(g_bkc_prof);
-    g_bkc_prof = nullptr;
+    cudaFree(c->bkc_prof);
+    c->bkc_prof = nullptr;
   }
   return HB_OK;
 }

@@ -9,14 +9,12 @@
 // Reference semantics: DPOTRF('L') on the column-major-lower view (hiopKKTLinSys.cpp:1228-1290 via DPOSVX; hiopDualsUpdater.cpp
 // :717); info = first non-positive pivot (1-based), 0 if none.
 #include "hb_common.cuh"
+#include "hb_dense.cuh"
 #include <cooperative_groups.h>
-#include <cstdlib>
 
 namespace cg = cooperative_groups;
 
 namespace {
-
-#define LC(A, lda, i, j) (A)[(size_t)(j) * (lda) + (i)]
 
 constexpr int CB = 64;   // panel width
 constexpr int CT = 256;  // threads per CTA
@@ -525,47 +523,34 @@ k_diag_inverses(const double* __restrict__ F, int ldf, int N, double* __restrict
   for(int r = 0; r < 16; r++) inv[r * 17 + c] = x[r];
 }
 
-bool g_coop_checked = false, g_coop_ok = false;
-int g_coop_max_ctas = 0;
-
 } // namespace
 
-// returns HB_OK and sets *used = true when the cooperative kernel ran; *used = false -> caller uses the multi-launch path
-int hb_dense_chol_coop(hb_ctx* c, int N, double* A, int lda, int* info_dev, double* invd, bool* used)
+int hb_chol_coop_init(hb_ctx* c)
 {
-  *used = false;
-  if(!g_coop_checked) {
-    g_coop_checked = true;
-    const char* e = getenv("HB_CHOL_COOP");
-    int coop = 0;
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, c->device);
-    if(coop && !(e && e[0] == '0')) {
-      if(cudaFuncSetAttribute(k_chol_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSmem)) == cudaSuccess) {
-        int occ = 0;
-        if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_chol_coop, CT, sizeof(CoopSmem)) == cudaSuccess && occ >= 1) {
-          g_coop_ok = true;
-          g_coop_max_ctas = c->num_sms * occ < c->num_sms ? c->num_sms * occ : c->num_sms;
-        }
-      }
-      cudaGetLastError();
-    }
-  }
-  if(!g_coop_ok || N <= CB || N > 2048) return HB_OK;
-  // one CTA per trailing tile of the first panel (the widest step), never more than fit on the device at once
-  const int nt0 = (N - CB + CB - 1) / CB;
-  int G = nt0 * (nt0 + 1) / 2;
-  if(G > g_coop_max_ctas) G = g_coop_max_ctas;
-  if(G < 1) G = 1;
-  HB_CUDA(cudaMemsetAsync(info_dev, 0, sizeof(int), c->stream));
-  long long* prof = nullptr;
-  void* args[] = {&A, &lda, &N, &info_dev, &invd, &prof};
-  HB_CUDA(cudaLaunchCooperativeKernel((const void*)k_chol_coop, dim3(G), dim3(CT), args, sizeof(CoopSmem), c->stream));
-  HB_LAUNCHED();
-  *used = true;
+  HB_CUDA(cudaFuncSetAttribute(k_chol_coop, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(CoopSmem)));
+  int coop = 0, occ = 0, occ_solve = 0;
+  HB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, c->device));
+  HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_chol_coop, CT, sizeof(CoopSmem)));
+  HB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_solve, k_spd_solve_coop, CT, 0));
+  // every CTA of a cooperative launch must be resident at once; one per SM (the solve never launches more than one per SM either)
+  c->coop_ctas = (coop && occ >= 1 && occ_solve >= 1) ? c->num_sms : 0;
   return HB_OK;
 }
 
-// fills invd for a factor produced by any Cholesky path
+int hb_dense_chol_coop(hb_ctx* c, int N, double* A, int lda, int* info_dev, double* invd, long long* prof)
+{
+  // one CTA per trailing tile of the first panel (the widest step), never more than fit on the device at once
+  const int nt0 = (N - CB + CB - 1) / CB;
+  int G = nt0 * (nt0 + 1) / 2;
+  if(G > c->coop_ctas) G = c->coop_ctas;
+  if(G < 1) G = 1;
+  HB_CUDA(cudaMemsetAsync(info_dev, 0, sizeof(int), c->stream));
+  void* args[] = {&A, &lda, &N, &info_dev, &invd, &prof};
+  HB_CUDA(cudaLaunchCooperativeKernel((const void*)k_chol_coop, dim3(G), dim3(CT), args, sizeof(CoopSmem), c->stream));
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
 int hb_dense_chol_diag_inverses(hb_ctx* c, int N, const double* F, int ldf, double* invd)
 {
   if(N <= 0) return HB_OK;
@@ -573,35 +558,14 @@ int hb_dense_chol_diag_inverses(hb_ctx* c, int N, const double* F, int ldf, doub
   HB_LAUNCHED();
   return HB_OK;
 }
-bool hb_dense_coop_available(hb_ctx* c)
-{
-  bool used = false;
-  hb_dense_chol_coop(c, 0, nullptr, 0, nullptr, nullptr, &used); // runs the one-time capability check
-  return g_coop_ok;
-}
 
-// cooperative solve + refinement; invd must come from hb_dense_chol_coop of the same factor. work: 2N+2 doubles.
 int hb_dense_spd_solve_coop(hb_ctx* c, int N, const double* F, int ldf, const double* invd, const double* s, const double* Nref, int ldn,
-                            const double* rhs, double* x, double* work, double tol, int max_refine, double* stats_dev, bool* used)
+                            const double* rhs, double* x, double* work, double tol, int max_refine, double* stats_dev)
 {
-  *used = false;
-  if(!g_coop_ok || !invd || N <= CB || N > 16384) return HB_OK;
-  static bool attr = false;
-  static int max_ctas = 0;
-  if(!attr) {
-    int occ = 0;
-    if(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_spd_solve_coop, CT, 0) != cudaSuccess || occ < 1) {
-      cudaGetLastError();
-      return HB_OK;
-    }
-    max_ctas = c->num_sms;
-    attr = true;
-  }
   int G = (N + 7) / 8; // ~8 rows / columns per CTA in the widest sweep step, one row of the residual per warp
-  if(G > max_ctas) G = max_ctas;
+  if(G > c->coop_ctas) G = c->coop_ctas;
   void* args[] = {&F, &ldf, &N, &invd, &s, &Nref, &ldn, &rhs, &x, &work, &tol, &max_refine, &stats_dev};
   HB_CUDA(cudaLaunchCooperativeKernel((const void*)k_spd_solve_coop, dim3(G), dim3(CT), args, 0, c->stream));
   HB_LAUNCHED();
-  *used = true;
   return HB_OK;
 }

@@ -76,6 +76,14 @@ struct hb_ctx
   // per-context state of the int8-slice condensation (hb_ozaki.cu): slice buffer, exponents, tensor maps, work list
   void* oz_state = nullptr;
   void (*oz_free)(void*) = nullptr;
+  // schedule cache of the FP64 condensation (hb_syrk.cu)
+  void* syrk_sched = nullptr;
+  void (*syrk_free)(void*) = nullptr;
+  // dense symmetric solvers: size thresholds (with their environment overrides, set by hb_dense_init in hb_symdense.cu) and the
+  // number of CTAs of the cooperative Cholesky resident at once (0: no cooperative kernels -- unsupported, or HB_CHOL_COOP=0)
+  int bk_cluster_min = 0, big_min_chol = 0, big_min_ldl = 0, pair_min = 0;
+  int coop_ctas = 0;
+  long long* bkc_prof = nullptr; // diagnostics: 8 cycle counters of the cluster Bunch-Kaufman panel while profiling is on
   // NCCL
   void* nccl_comm = nullptr;
   int nranks = 1, rank = 0;
@@ -84,6 +92,13 @@ struct hb_ctx
 static constexpr int HB_RED_SLOTS = 4096;
 
 int hb_ws_reserve(hb_ctx* ctx, size_t bytes);
+
+// set once by hb_ctx_create: the dynamic-shared-memory / cluster attributes of each kernel file's kernels (function attributes are
+// per device) and the dense solvers' thresholds
+int hb_syrk_init_attrs(hb_ctx* c);
+int hb_ozaki_init_attrs(hb_ctx* c);
+int hb_microbench_init_attrs(hb_ctx* c);
+int hb_dense_init(hb_ctx* c);
 
 // phase marks of the quasi-Newton step (ids are the HB_PH_* below); a no-op unless hb_ctx_phase_timeline switched them on
 enum { HB_PH_START = 0, HB_PH_UPDATE, HB_PH_OZ_ROWMAX, HB_PH_OZ_SLICE, HB_PH_CAUG, HB_PH_ALLREDUCE, HB_PH_VN, HB_PH_CHOL, HB_PH_HSOLVE1, HB_PH_JX, HB_PH_SPDSOLVE, HB_PH_JTY, HB_PH_HSOLVE2, HB_PH_COUNT };
@@ -107,6 +122,11 @@ __device__ __forceinline__ double hb_warp_max(double v)
 #pragma unroll
   for(int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+// c[0..1] += a * b on the FP64 tensor path (SASS DMMA): one m8n8k4 fragment per thread
+__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
+{
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 __device__ __forceinline__ double hb_warp_min(double v)
 {

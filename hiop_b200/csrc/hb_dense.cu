@@ -15,15 +15,8 @@
 
 namespace {
 
-#define LC(A, lda, i, j) (A)[(size_t)(j) * (lda) + (i)]
-
 constexpr int NB = 64;             // panel width of the blocked factorizations
 constexpr int PANEL_THREADS = 256; // one row of the slab per thread
-
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
 
 // ---------------------------------------------------------------------------------------------------------
 // Panel kernel: every CTA factors the nb x nb diagonal block in shared memory (redundantly -- it is 64^3/3 flops),
@@ -178,23 +171,34 @@ k_panel(double* __restrict__ A, int lda, int N, int k0, int nb, double* __restri
 // ---------------------------------------------------------------------------------------------------------
 // Trailing update on the DMMA pipe: for i >= j >= r0:  Lc(i,j) -= sum_p P[p][i] * Q[p][j],  p < kb.
 // P, Q are kb "row-contiguous" panels: P[p][i] = Pbase[p*ldp + i] (for Cholesky P = Q = the factor panel rows,
-// for LDL^T P = W = L*D, Q = L). 64x64 output tiles, 4 warps (2x2), warp tile 32x32.
+// for LDL^T P = W = L*D, Q = L). 64x64 output tiles, 4 warps (2x2), warp tile 32x32. P feeds the A fragments, Q the B fragments:
+// swapping the two would change the rounding of every product.
+// FROM_STATE (blocked Bunch-Kaufman): the panel's origin k0 and width kb are read from the device state word (state[0], state[1]),
+// r0 = k0 + kb, P = L21 (the panel's columns of A) and Q = W21; the grid covers the widest remainder the panel can leave.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int TT = 64;
 constexpr int TLD = TT + 4; // padded: fragment reads (p = lane%4, i = lane/4) are bank-conflict free
+template <bool FROM_STATE>
 __global__ void __launch_bounds__(128)
 k_trailing(double* __restrict__ A, int lda, int N, int r0, const double* __restrict__ P, long long ldp, const double* __restrict__ Q,
-           long long ldq, int kb)
+           long long ldq, int kb, const int* __restrict__ state)
 {
   extern __shared__ __align__(16) unsigned char trailing_smem[];
   double (*sP)[TLD] = reinterpret_cast<double (*)[TLD]>(trailing_smem);
   double (*sQ)[TLD] = sP + NB;
-  const int nt = (N - r0 + TT - 1) / TT;
+  if(FROM_STATE) {
+    const int k0 = state[0];
+    kb = state[1];
+    r0 = k0 + kb;
+    if(kb == 0 || r0 >= N) return;
+    P = A + (size_t)k0 * lda;
+    ldp = lda;
+  }
   // linear tile id -> (ti >= tj)
   int t = blockIdx.x, ti = 0;
   while(t >= ti + 1) { t -= ti + 1; ti++; }
   const int tj = t;
-  (void)nt;
+  if(FROM_STATE && ti >= (N - r0 + TT - 1) / TT) return;
   const int i0 = r0 + ti * TT, j0 = r0 + tj * TT;
   const int tid = threadIdx.x;
   {
@@ -417,38 +421,6 @@ __global__ void k_equilibrate(const double* __restrict__ Nfull, int ldn, int N, 
 // large N is k_lasyf_panel + k_trailing below.
 // ---------------------------------------------------------------------------------------------------------
 constexpr int BK_THREADS = 1024;
-#define BK_ALPHA 0.6403882032022076 /* (1+sqrt(17))/8 */
-
-struct ArgMax
-{
-  double v;
-  int i;
-};
-__device__ __forceinline__ ArgMax argmax_comb(ArgMax a, ArgMax b)
-{
-  // IDAMAX semantics: first index of the maximum absolute value
-  if(b.v > a.v || (b.v == a.v && b.i < a.i)) return b;
-  return a;
-}
-__device__ ArgMax block_argmax(ArgMax a, ArgMax* sm /* 32 */)
-{
-#pragma unroll
-  for(int o = 16; o > 0; o >>= 1) {
-    ArgMax b;
-    b.v = __shfl_xor_sync(0xffffffffu, a.v, o);
-    b.i = __shfl_xor_sync(0xffffffffu, a.i, o);
-    a = argmax_comb(a, b);
-  }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  __syncthreads();
-  if(lane == 0) sm[warp] = a;
-  __syncthreads();
-  ArgMax r = sm[0];
-  const int nw = blockDim.x >> 5;
-  for(int w = 1; w < nw; w++) r = argmax_comb(r, sm[w]);
-  return r; // every thread gets the same answer
-}
-
 __global__ void __launch_bounds__(BK_THREADS)
 k_sytf2(double* __restrict__ A, int lda, int N, int* __restrict__ ipiv, int* __restrict__ info)
 {
@@ -465,7 +437,7 @@ k_sytf2(double* __restrict__ A, int lda, int N, int* __restrict__ ipiv, int* __r
     if(k < N - 1) {
       ArgMax a{-1.0, big};
       for(int i = k + 1 + tid; i < N; i += BK_THREADS) a = argmax_comb(a, ArgMax{fabs(LC(A, lda, i, k)), i});
-      a = block_argmax(a, sm);
+      a = cta_argmax(a, sm);
       imax = a.i;
       colmax = a.v;
     }
@@ -479,7 +451,7 @@ k_sytf2(double* __restrict__ A, int lda, int N, int* __restrict__ ipiv, int* __r
         ArgMax a{-1.0, big};
         for(int j = k + tid; j < imax; j += BK_THREADS) a = argmax_comb(a, ArgMax{fabs(LC(A, lda, imax, j)), j});
         for(int i = imax + 1 + tid; i < N; i += BK_THREADS) a = argmax_comb(a, ArgMax{fabs(LC(A, lda, i, imax)), i});
-        a = block_argmax(a, sm);
+        a = cta_argmax(a, sm);
         const double rowmax = a.v;
         if(absakk >= BK_ALPHA * colmax * (colmax / rowmax)) kp = k;
         else if(fabs(LC(A, lda, imax, imax)) >= BK_ALPHA * rowmax) kp = imax;
@@ -557,6 +529,195 @@ k_sytf2(double* __restrict__ A, int lda, int N, int* __restrict__ ipiv, int* __r
     __syncthreads();
   }
   if(tid == 0) *info = linfo;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Blocked Bunch-Kaufman (DSYTRF 'L' structure: DLASYF panels + rank-kb trailing updates). The panel (<= 64 columns) is factorized by
+// ONE CTA with LAPACK's pivot rule (same pivots as DSYTF2), keeping W = L*D of the panel in a scratch buffer; the trailing matrix is
+// then updated A22 -= L21 * W21^T by k_trailing<true>. No host synchronisation inside the loop: the number of columns a panel managed
+// to factorize (63 or 64, a 2x2 pivot may not straddle the panel edge) lives in a device-side state word that the next kernels read.
+// ---------------------------------------------------------------------------------------------------------
+#define WC(W, ldw, i, c) (W)[(size_t)(c) * (ldw) + (i)]
+
+// state[0] = k0 of the current panel, state[1] = kb factorized by the last panel, state[2] = info (first zero pivot, 1-based)
+__global__ void __launch_bounds__(BK_THREADS)
+k_lasyf_panel(double* __restrict__ A, int lda, int N, double* __restrict__ W, int ldw, int* __restrict__ ipiv, int* __restrict__ state)
+{
+  __shared__ ArgMax sm[32];
+  __shared__ double wrow[NB];
+  const int tid = threadIdx.x;
+  const int big = 0x7fffffff;
+  const int k0 = state[0];
+  if(k0 >= N) {
+    if(tid == 0) state[1] = 0;
+    return;
+  }
+  const int ns = N - k0;
+  const bool last = ns <= NB;
+  int linfo = 0;
+  int k = k0;
+  while(true) {
+    const int kl = k - k0;
+    if(k >= N) break;
+    if(!last && kl >= NB - 1) break;
+    // --- W(k:N,kl) = A(k:N,k) - A(k:N,k0:k-1) * W(k,0:kl-1)^T
+    __syncthreads();
+    for(int c = tid; c < kl; c += BK_THREADS) wrow[c] = WC(W, ldw, k, c);
+    __syncthreads();
+    for(int i = k + tid; i < N; i += BK_THREADS) {
+      double v = LC(A, lda, i, k), v1 = 0.0, v2 = 0.0, v3 = 0.0;
+      int c = 0;
+#pragma unroll 2
+      for(; c + 4 <= kl; c += 4) { // four independent accumulators: the loads of a batch are in flight together
+        v -= LC(A, lda, i, k0 + c) * wrow[c];
+        v1 -= LC(A, lda, i, k0 + c + 1) * wrow[c + 1];
+        v2 -= LC(A, lda, i, k0 + c + 2) * wrow[c + 2];
+        v3 -= LC(A, lda, i, k0 + c + 3) * wrow[c + 3];
+      }
+      for(; c < kl; c++) v -= LC(A, lda, i, k0 + c) * wrow[c];
+      WC(W, ldw, i, kl) = (v + v1) + (v2 + v3);
+    }
+    __syncthreads();
+    int kstep = 1, kp = k;
+    const double absakk = fabs(WC(W, ldw, k, kl));
+    int imax = k;
+    double colmax = 0.0;
+    if(k < N - 1) {
+      ArgMax a{-1.0, big};
+      for(int i = k + 1 + tid; i < N; i += BK_THREADS) a = argmax_comb(a, ArgMax{fabs(WC(W, ldw, i, kl)), i});
+      a = cta_argmax(a, sm);
+      imax = a.i;
+      colmax = a.v;
+    }
+    if(fmax(absakk, colmax) == 0.0 || absakk != absakk) {
+      if(linfo == 0) linfo = k + 1;
+      kp = k;
+    } else {
+      if(absakk >= BK_ALPHA * colmax) {
+        kp = k;
+      } else {
+        // column imax (updated) into W(:,kl+1)
+        __syncthreads();
+        for(int c = tid; c < kl; c += BK_THREADS) wrow[c] = WC(W, ldw, imax, c);
+        __syncthreads();
+        for(int i = k + tid; i < N; i += BK_THREADS) {
+          double v = i < imax ? LC(A, lda, imax, i) : LC(A, lda, i, imax), v1 = 0.0, v2 = 0.0, v3 = 0.0;
+          int c = 0;
+#pragma unroll 2
+          for(; c + 4 <= kl; c += 4) {
+            v -= LC(A, lda, i, k0 + c) * wrow[c];
+            v1 -= LC(A, lda, i, k0 + c + 1) * wrow[c + 1];
+            v2 -= LC(A, lda, i, k0 + c + 2) * wrow[c + 2];
+            v3 -= LC(A, lda, i, k0 + c + 3) * wrow[c + 3];
+          }
+          for(; c < kl; c++) v -= LC(A, lda, i, k0 + c) * wrow[c];
+          WC(W, ldw, i, kl + 1) = (v + v1) + (v2 + v3);
+        }
+        __syncthreads();
+        ArgMax a{-1.0, big};
+        for(int i = k + tid; i < N; i += BK_THREADS)
+          if(i != imax) a = argmax_comb(a, ArgMax{fabs(WC(W, ldw, i, kl + 1)), i});
+        a = cta_argmax(a, sm);
+        const double rowmax = a.v;
+        if(absakk >= BK_ALPHA * colmax * (colmax / rowmax)) {
+          kp = k;
+        } else if(fabs(WC(W, ldw, imax, kl + 1)) >= BK_ALPHA * rowmax) {
+          kp = imax;
+          __syncthreads();
+          for(int i = k + tid; i < N; i += BK_THREADS) WC(W, ldw, i, kl) = WC(W, ldw, i, kl + 1);
+          __syncthreads();
+        } else {
+          kp = imax;
+          kstep = 2;
+        }
+      }
+      const int kk = k + kstep - 1, kkl = kk - k0;
+      __syncthreads();
+      if(kp != kk) {
+        // copy the non-updated column kk into position kp of the trailing submatrix
+        if(tid == 0) LC(A, lda, kp, kp) = LC(A, lda, kk, kk);
+        for(int i = kk + 1 + tid; i < kp; i += BK_THREADS) LC(A, lda, kp, i) = LC(A, lda, i, kk);
+        for(int i = kp + 1 + tid; i < N; i += BK_THREADS) LC(A, lda, i, kp) = LC(A, lda, i, kk);
+        // swap rows kk and kp in the panel's finished columns of A and in W(.,0:kkl)
+        for(int c = tid; c < kl; c += BK_THREADS) {
+          const double t = LC(A, lda, kk, k0 + c);
+          LC(A, lda, kk, k0 + c) = LC(A, lda, kp, k0 + c);
+          LC(A, lda, kp, k0 + c) = t;
+        }
+        for(int c = tid; c <= kkl; c += BK_THREADS) {
+          const double t = WC(W, ldw, kk, c);
+          WC(W, ldw, kk, c) = WC(W, ldw, kp, c);
+          WC(W, ldw, kp, c) = t;
+        }
+        __syncthreads();
+      }
+      if(kstep == 1) {
+        const double akk = WC(W, ldw, k, kl);
+        const double r1 = 1.0 / akk;
+        for(int i = k + tid; i < N; i += BK_THREADS) {
+          const double w = WC(W, ldw, i, kl);
+          LC(A, lda, i, k) = (i == k) ? w : w * r1;
+        }
+      } else {
+        if(k < N - 2) {
+          double d21 = WC(W, ldw, k + 1, kl);
+          const double d11 = WC(W, ldw, k + 1, kl + 1) / d21;
+          const double d22 = WC(W, ldw, k, kl) / d21;
+          const double t = 1.0 / (d11 * d22 - 1.0);
+          d21 = t / d21;
+          for(int j = k + 2 + tid; j < N; j += BK_THREADS) {
+            const double wj0 = WC(W, ldw, j, kl), wj1 = WC(W, ldw, j, kl + 1);
+            LC(A, lda, j, k) = d21 * (d11 * wj0 - wj1);
+            LC(A, lda, j, k + 1) = d21 * (d22 * wj1 - wj0);
+          }
+        }
+        if(tid == 0) {
+          LC(A, lda, k, k) = WC(W, ldw, k, kl);
+          LC(A, lda, k + 1, k) = WC(W, ldw, k + 1, kl);
+          LC(A, lda, k + 1, k + 1) = WC(W, ldw, k + 1, kl + 1);
+        }
+      }
+    }
+    if(tid == 0) {
+      if(kstep == 1) ipiv[k] = kp + 1;
+      else { ipiv[k] = -(kp + 1); ipiv[k + 1] = -(kp + 1); }
+    }
+    k += kstep;
+    __syncthreads();
+  }
+  if(tid == 0) {
+    state[1] = k - k0;
+    if(linfo != 0 && state[2] == 0) state[2] = linfo;
+  }
+}
+
+// Puts L21 of the finished panel in LAPACK's standard form (partial undo of the row interchanges, DLASYF label 120)
+// and advances the state to the next panel.
+__global__ void k_lasyf_finish(double* __restrict__ A, int lda, int N, const int* __restrict__ ipiv, int* __restrict__ state)
+{
+  const int k0 = state[0], kb = state[1];
+  if(kb == 0) return;
+  const int kend = k0 + kb;
+  int j = kend - 1;
+  while(j >= k0) {
+    const int jj = j;
+    int jp = ipiv[j];
+    if(jp < 0) { jp = -jp; j -= 1; }
+    jp -= 1;
+    j -= 1;
+    const int ncols = j - k0 + 1;
+    if(jp != jj && ncols >= 1) {
+      for(int c = threadIdx.x; c < ncols; c += blockDim.x) {
+        const double t = LC(A, lda, jp, k0 + c);
+        LC(A, lda, jp, k0 + c) = LC(A, lda, jj, k0 + c);
+        LC(A, lda, jj, k0 + c) = t;
+      }
+    }
+    __syncthreads();
+    if(j <= k0) break;
+  }
+  __syncthreads();
+  if(threadIdx.x == 0) state[0] = kend;
 }
 
 // DSYTRS 'L': one thread per right-hand side (rhs r = B + r*ldb, contiguous N doubles). Used for V^{-1}[S1^T;Y1^T]
@@ -740,28 +901,19 @@ k_chol_solve(const double* __restrict__ F, int ldf, int N, double* __restrict__ 
 } // namespace
 
 // ---------------------------------------------------------------------------------------------------------
-// internal API
+// internal API (hb_dense.cuh): each entry point runs one path; hb_symdense.cu decides which
 // ---------------------------------------------------------------------------------------------------------
 constexpr size_t TRAILING_SMEM = sizeof(double) * 2 * NB * TLD;
-static bool g_trailing_attr = false;
 
-int hb_dense_chol_coop(hb_ctx* c, int N, double* A, int lda, int* info_dev, double* invd, bool* used);
-int hb_dense_chol_diag_inverses(hb_ctx* c, int N, const double* F, int ldf, double* invd);
-bool hb_dense_coop_available(hb_ctx* c);
-int hb_dense_spd_solve_coop(hb_ctx* c, int N, const double* F, int ldf, const double* invd, const double* s, const double* Nref, int ldn,
-                            const double* rhs, double* x, double* work, double tol, int max_refine, double* stats_dev, bool* used);
-
-int hb_dense_factor_blocked(hb_ctx* c, int N, double* A, int lda, bool ldl, double* Wpanel /* NB*N doubles if ldl */, int* info_dev)
+int hb_dense_init_attrs(hb_ctx* c)
 {
-  if(!ldl) { // small SPD systems: one cooperative launch instead of two launches per panel (hb_chol_coop.cu)
-    bool used = false;
-    HB_CHECK(hb_dense_chol_coop(c, N, A, lda, info_dev, nullptr, &used));
-    if(used) return HB_OK;
-  }
-  if(!g_trailing_attr) {
-    HB_CUDA(cudaFuncSetAttribute(k_trailing, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TRAILING_SMEM));
-    g_trailing_attr = true;
-  }
+  HB_CUDA(cudaFuncSetAttribute(k_trailing<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TRAILING_SMEM));
+  HB_CUDA(cudaFuncSetAttribute(k_trailing<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TRAILING_SMEM));
+  return HB_OK;
+}
+
+int hb_dense_factor_panel(hb_ctx* c, int N, double* A, int lda, bool ldl, double* Wpanel /* NB*N doubles if ldl */, int* info_dev)
+{
   HB_CUDA(cudaMemsetAsync(info_dev, 0, sizeof(int), c->stream));
   for(int k0 = 0; k0 < N; k0 += NB) {
     const int nb = N - k0 < NB ? N - k0 : NB;
@@ -776,7 +928,8 @@ int hb_dense_factor_blocked(hb_ctx* c, int N, double* A, int lda, bool ldl, doub
       const int ntiles = nt * (nt + 1) / 2;
       const double* Q = A + (size_t)k0 * lda; // factor panel rows: Q[p][i] = Lc(i, k0+p)
       const double* P = ldl ? Wpanel : Q;
-      k_trailing<<<ntiles, 128, TRAILING_SMEM, c->stream>>>(A, lda, N, k0 + nb, P, ldl ? (long long)N : (long long)lda, Q, lda, nb);
+      k_trailing<false><<<ntiles, 128, TRAILING_SMEM, c->stream>>>(A, lda, N, k0 + nb, P, ldl ? (long long)N : (long long)lda, Q, lda, nb,
+                                                                     nullptr);
       HB_LAUNCHED();
     }
   }
@@ -791,10 +944,36 @@ int hb_dense_sytf2(hb_ctx* c, int N, double* A, int lda, int* ipiv_dev, int* inf
   return HB_OK;
 }
 
-int hb_dense_sytrs(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, double* B, int ldb, int nrhs)
+int hb_dense_sytrf_blocked(hb_ctx* c, int N, double* A, int lda, int* ipiv_dev, double* Wpanel, int* info_dev)
+{
+  if(N == 0) return HB_OK;
+  // device state word (k0, kb, info) in the workspace
+  HB_CHECK(hb_ws_reserve(c, 64));
+  int* state = reinterpret_cast<int*>(c->ws);
+  HB_CUDA(cudaMemsetAsync(state, 0, sizeof(int) * 4, c->stream));
+  const int max_panels = (N + (NB - 1) - 1) / (NB - 1) + 1;
+  for(int p = 0; p < max_panels; p++) {
+    const int k0_min = p * (NB - 1); // a panel advances by at least NB-1 columns
+    if(k0_min >= N) break;
+    k_lasyf_panel<<<1, BK_THREADS, 0, c->stream>>>(A, lda, N, Wpanel, N, ipiv_dev, state);
+    HB_LAUNCHED();
+    const int rest_max = N - k0_min - (NB - 1);
+    if(rest_max > 0) {
+      const int nt = (rest_max + TT - 1) / TT;
+      k_trailing<true><<<nt * (nt + 1) / 2, 128, TRAILING_SMEM, c->stream>>>(A, lda, N, 0, nullptr, 0, Wpanel, N, 0, state);
+      HB_LAUNCHED();
+    }
+    k_lasyf_finish<<<1, 64, 0, c->stream>>>(A, lda, N, ipiv_dev, state);
+    HB_LAUNCHED();
+  }
+  HB_CUDA(cudaMemcpyAsync(info_dev, state + 2, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+  return HB_OK;
+}
+
+int hb_dense_sytrs(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, double* B, int ldb, int nrhs, bool cta_per_rhs)
 {
   if(N == 0 || nrhs == 0) return HB_OK;
-  if(nrhs >= 8 || N <= 64) {
+  if(!cta_per_rhs) {
     k_sytrs_per_rhs<<<(nrhs + 63) / 64, 64, 0, c->stream>>>(A, lda, N, ipiv_dev, B, ldb, nrhs);
     HB_LAUNCHED();
   } else {
@@ -806,10 +985,11 @@ int hb_dense_sytrs(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_d
   return HB_OK;
 }
 
-int hb_dense_inertia(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, int mode, int* out3_dev)
+int hb_dense_inertia_ipiv(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, int* out3_dev)
 {
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * 2 * (size_t)(N > 0 ? N : 1) + 256));
-  k_inertia<<<1, 1024, 0, c->stream>>>(A, lda, N, ipiv_dev, mode, out3_dev, reinterpret_cast<double*>(reinterpret_cast<char*>(c->ws) + 256));
+  k_inertia<<<1, 1024, 0, c->stream>>>(A, lda, N, ipiv_dev, HB_FACT_BUNCH_KAUFMAN, out3_dev,
+                                       reinterpret_cast<double*>(reinterpret_cast<char*>(c->ws) + 256));
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -831,39 +1011,6 @@ int hb_dense_equilibrate(hb_ctx* c, int N, const double* Nfull, int ldn, double*
   k_equilibrate<<<g, 256, 0, c->stream>>>(Nfull, ldn, N, F, ldf, s);
   HB_LAUNCHED();
   return HB_OK;
-}
-
-// SPD factorization that also keeps the 16 x 16 diagonal inverses for the cooperative solve (invd: HB_CHOL_INV_DOUBLES(N) doubles);
-// *have_inv tells whether they were produced (small / large N use the multi-launch path and the one-CTA solve)
-static hb_big g_chol_big[16]; // look-ahead state (panel stream, scratch) of the large condensed systems, one per device
-
-int hb_dense_chol_with_inverses(hb_ctx* c, int N, double* A, int lda, int* info_dev, double* invd, bool* have_inv)
-{
-  *have_inv = false;
-  HB_CHECK(hb_dense_chol_coop(c, N, A, lda, info_dev, invd, have_inv));
-  if(*have_inv) return HB_OK;
-  // beyond the single-launch cooperative kernel: the look-ahead Cholesky of hb_dense_big.cu (config 4: m = 4000 per condensed system)
-  if(N > 2048 && (lda & 1) == 0 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0 && c->device < 16) {
-    HB_CHECK(hb_big_factor(c, &g_chol_big[c->device], N, A, lda, false, info_dev));
-  } else
-  HB_CHECK(hb_dense_factor_blocked(c, N, A, lda, false, nullptr, info_dev));
-  if(N > 64 && invd && hb_dense_coop_available(c)) { // large N: multi-launch factor, but the solve can still be cooperative
-    HB_CHECK(hb_dense_chol_diag_inverses(c, N, A, lda, invd));
-    *have_inv = true;
-  }
-  return HB_OK;
-}
-
-int hb_dense_spd_solve_refine2(hb_ctx* c, int N, const double* F, int ldf, const double* invd, const double* s, const double* Nref, int ldn,
-                               const double* rhs, double* x, double* work2N2, double tol, int max_refine, double* stats_dev)
-{
-  if(N == 0) return HB_OK;
-  if(invd) {
-    bool used = false;
-    HB_CHECK(hb_dense_spd_solve_coop(c, N, F, ldf, invd, s, Nref, ldn, rhs, x, work2N2, tol, max_refine, stats_dev, &used));
-    if(used) return HB_OK;
-  }
-  return hb_dense_spd_solve_refine(c, N, F, ldf, s, Nref, ldn, rhs, x, work2N2, tol, max_refine, stats_dev);
 }
 
 int hb_dense_spd_solve_refine(hb_ctx* c, int N, const double* F, int ldf, const double* s, const double* Nref, int ldn, const double* rhs,

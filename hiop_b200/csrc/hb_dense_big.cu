@@ -21,11 +21,8 @@
 // rows below. N = 8192: 2 x 32 launches.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
-#include <cstdlib>
 
 namespace {
-
-#define LC(A, lda, i, j) (A)[(size_t)(j) * (lda) + (i)]
 
 constexpr int BB = 128;  // factorization block = size of the stored diagonal-block inverses
 constexpr int KC = 16;   // operand rows per pipeline stage
@@ -34,10 +31,6 @@ constexpr int TM = 128;  // tile rows (i)
 constexpr int PLD = TM + 4;
 constexpr int CLD = TM + 2;
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes)
 {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
@@ -854,11 +847,13 @@ __global__ void k_scatter(int N, const int* __restrict__ perm, const double* __r
   if(i < N) out[perm[i]] = in[i];
 }
 
-bool g_big_attr[16] = {false};
+} // namespace
 
-int ensure_attrs(hb_ctx* c)
+// ---------------------------------------------------------------------------------------------------------------------
+// internal API (hb_dense.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+int hb_big_init_attrs(hb_ctx* c)
 {
-  if(c->device < 16 && g_big_attr[c->device]) return HB_OK;
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<64, EPI_SUB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<64>::SMEM));
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<128, EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<128>::SMEM));
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<128, EPI_STORE_LDL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<128>::SMEM));
@@ -867,18 +862,11 @@ int ensure_attrs(hb_ctx* c)
   HB_CUDA(cudaFuncSetAttribute(k_block_inverses, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DiagSmem)));
   HB_CUDA(cudaFuncSetAttribute(k_trsm_panel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TrsmSmem)));
   HB_CUDA(cudaFuncSetAttribute(k_trsm_panel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TrsmSmem)));
-  if(c->device < 16) g_big_attr[c->device] = true;
   return HB_OK;
 }
 
-} // namespace
-
-// ---------------------------------------------------------------------------------------------------------------------
-// internal API (hb_dense.cuh)
-// ---------------------------------------------------------------------------------------------------------------------
 int hb_big_init(hb_ctx* c, hb_big* b)
 {
-  HB_CHECK(ensure_attrs(c));
   if(!b->panel_stream) {
     int lo = 0, hi = 0;
     HB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
@@ -946,7 +934,7 @@ int hb_big_reserve(hb_ctx* c, hb_big* b, int N, bool need_w)
 //   diag(2a) trsm(2a) U1(2a -> block 2a+1) diag(2a+1) trsm(2a+1)
 // while the update stream still applies pair a-1 to the columns beyond; the update stream applies pair a first to the two column
 // blocks the next pair needs (events E_UA, E_UBa release the panel stream one block at a time), then to everything else.
-int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ldl, int* info_dev)
+int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ldl, bool pairs, int* info_dev)
 {
   HB_REQUIRE((lda & 1) == 0 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0, "hb_big_factor: needs an even leading dimension and a 16-byte aligned matrix");
   HB_CHECK(hb_big_reserve(c, b, N, ldl));
@@ -983,9 +971,7 @@ int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ld
     HB_LAUNCHED();
     return HB_OK;
   };
-  // pairing pays once the update dominates the panel chain (threshold not re-measured on H100; HB_DENSE_PAIR_MIN overrides it)
-  static const int pair_min = getenv("HB_DENSE_PAIR_MIN") ? atoi(getenv("HB_DENSE_PAIR_MIN")) : 6144;
-  const int GW = N >= pair_min ? 2 : 1; // blocks per group
+  const int GW = pairs ? 2 : 1; // blocks per group
   for(int a = 0; GW * a < nblk; a++) {
     const int b0 = GW * a, b1 = GW == 2 ? 2 * a + 1 : nblk; // b1 >= nblk: no second block
     const int k0 = b0 * BB;                                   // first column of the group
@@ -1048,7 +1034,6 @@ int hb_big_diag_profile(hb_ctx* c, hb_big* b, int N, double* A, long long lda, i
 // trailing update of a pivoted panel whose origin / width live in device memory (state[0] = k0, state[1] = kb): A22 -= W21 L21^T
 int hb_big_trailing_from_state(hb_ctx* c, int N, double* A, long long lda, const double* W, long long ldw, const int* state_dev, int r0_min, cudaStream_t st)
 {
-  HB_CHECK(ensure_attrs(c));
   if(r0_min >= N) return HB_OK;
   GemmArgs g{};
   g.P = W; g.ldp = ldw; g.Q = nullptr; g.ldq = lda; g.qsub = 0; g.kb = 0;
@@ -1076,7 +1061,6 @@ int hb_big_block_inverses(hb_ctx* c, hb_big* b, int N, const double* F, long lon
 
 // x <- solution of (L [D] L^T) x = x with the factor F (+ b->InvAll). dmode: 0 = Cholesky (no D), 1 = D from the diagonal (LDL^T),
 // 2 = Bunch-Kaufman block diagonal (ipiv_dev, dsub_dev), perm_dev (may be NULL): x is gathered through it first and scattered back at the end.
-int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, double* x);
 int hb_big_solve(hb_ctx* c, hb_big* b, int N, const double* F, long long ldf, int dmode, const int* ipiv_dev, const double* dsub_dev, const int* perm_dev,
                  double* x)
 {

@@ -485,7 +485,7 @@ int hess_solve(hb_lowrank* k, const double* rhs, double* x)
   if(k->n == 0) return HB_OK;
   if(k->l > 0) {
     HB_CHECK(multidot(k, k->DhInv, rhs, k->sigma)); // [sigma*S*(DhInv rhs); Y*(DhInv rhs)]
-    HB_CHECK(hb_dense_sytrs(c, 2 * k->l, k->V, 2 * k->l, k->ipivV, k->p2l, 2 * k->l, 1));
+    HB_CHECK(hb_dense_bk_small_solve(c, 2 * k->l, k->V, 2 * k->l, k->ipivV, k->p2l, 2 * k->l, 1));
   }
   k_lowrank_apply<<<stream_grid(c, k->n), ET, sizeof(double) * 2 * (k->l > 0 ? k->l : 1), c->stream>>>(
       k->n, k->l, k->sigma, k->St, k->Yt, k->n, k->p2l, k->DhInv, rhs, 0.0, nullptr, 0.0, 1.0, x);
@@ -589,11 +589,11 @@ int condense_finish(hb_lowrank* k)
   if(l > 0) {
     k_build_V<<<(4 * l * l + 127) / 128, 128, 0, c->stream>>>(m, l, k->sigma, k->Caug, Ma, k->SSt, k->Ld, k->Dd_sec, k->V);
     HB_LAUNCHED();
-    HB_CHECK(hb_dense_sytf2(c, 2 * l, k->V, 2 * l, k->ipivV, k->info + 0));
+    HB_CHECK(hb_dense_bk_small_factor(c, 2 * l, k->V, 2 * l, k->ipivV, k->info + 0));
     if(m > 0) {
       k_build_U<<<(m * 2 * l + 127) / 128, 128, 0, c->stream>>>(m, l, k->sigma, k->Caug, Ma, k->U, k->Z);
       HB_LAUNCHED();
-      HB_CHECK(hb_dense_sytrs(c, 2 * l, k->V, 2 * l, k->ipivV, k->Z, 2 * l, m));
+      HB_CHECK(hb_dense_bk_small_solve(c, 2 * l, k->V, 2 * l, k->ipivV, k->Z, 2 * l, m));
     }
   }
   if(m > 0) {
@@ -603,7 +603,7 @@ int condense_finish(hb_lowrank* k)
     HB_LAUNCHED();
     HB_CHECK(hb_dense_equilibrate(c, m, k->Nmat, m, k->F, m, k->svec));
     hb_phase_mark(c, HB_PH_VN);
-    HB_CHECK(hb_dense_chol_with_inverses(c, m, k->F, m, k->info + 1, k->Finv, &k->have_finv));
+    HB_CHECK(hb_dense_condensed_factor(c, &k->big, m, k->F, m, k->Finv, k->info + 1));
     hb_phase_mark(c, HB_PH_CHOL);
   }
   HB_CUDA(cudaMemcpyAsync(k->info_host, k->info, sizeof(int) * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -670,6 +670,7 @@ extern "C" int hb_lowrank_destroy(hb_lowrank* k)
   for(double* b : bufs) if(b) cudaFree(b);
   for(double* b : k->hbuf) if(b) cudaFree(b);
   cudaFree(k->ipivV); cudaFree(k->ipivM); cudaFree(k->info); cudaFree(k->rowptr_dev);
+  hb_big_release(&k->big);
   cudaFreeHost(k->rowptr_host); cudaFreeHost(k->info_host); cudaFreeHost(k->stats_host);
   if(k->copy_stream) {
     cudaStreamDestroy(k->copy_stream);
@@ -832,8 +833,7 @@ extern "C" int hb_lowrank_solve_compressed(hb_lowrank* k, double* rx, const doub
   }
   if(m > 0) {
     // 3. N dy = rhs with residual-driven refinement               :1169, 1192-1350
-    HB_CHECK(hb_dense_spd_solve_refine2(c, m, k->F, m, k->have_finv ? k->Finv : nullptr, k->svec, k->Nmat, m, k->rhs, k->dy, k->work, 1e-8, 3,
-                                        k->stats));
+    HB_CHECK(hb_dense_condensed_solve(c, m, k->F, m, k->Finv, k->svec, k->Nmat, m, k->rhs, k->dy, k->work, 1e-8, 3, k->stats));
     hb_phase_mark(c, HB_PH_SPDSOLVE);
     if(k->meq) HB_CUDA(cudaMemcpyAsync(dyc, k->dy, sizeof(double) * k->meq, cudaMemcpyDeviceToDevice, c->stream));
     if(k->mineq) HB_CUDA(cudaMemcpyAsync(dyd, k->dy + k->meq, sizeof(double) * k->mineq, cudaMemcpyDeviceToDevice, c->stream));
@@ -910,11 +910,11 @@ extern "C" int hb_lowrank_hess_times_vec(hb_lowrank* k, double beta, double* y, 
       HB_CUDA(cudaMemsetAsync(k->info + 2, 0, sizeof(int), c->stream));
       k_build_Mdirect<<<(4 * l * l + 127) / 128, 128, 0, c->stream>>>(l, k->sigma, k->SSt, k->Ld, k->Dd_sec, k->Mdir);
       HB_LAUNCHED();
-      HB_CHECK(hb_dense_sytf2(c, 2 * l, k->Mdir, 2 * l, k->ipivM, k->info + 2));
+      HB_CHECK(hb_dense_bk_small_factor(c, 2 * l, k->Mdir, 2 * l, k->ipivM, k->info + 2));
       k->mdir_valid = true;
     }
     HB_CHECK(multidot(k, nullptr, x, k->sigma)); // [sigma S x; Y x]
-    HB_CHECK(hb_dense_sytrs(c, 2 * l, k->Mdir, 2 * l, k->ipivM, k->p2l, 2 * l, 1));
+    HB_CHECK(hb_dense_bk_small_solve(c, 2 * l, k->Mdir, 2 * l, k->ipivM, k->p2l, 2 * l, 1));
   }
   k_lowrank_apply<<<stream_grid(c, k->n), ET, sizeof(double) * 2 * (l > 0 ? l : 1), c->stream>>>(
       k->n, l, k->sigma, k->St, k->Yt, k->n, k->p2l, nullptr, x, k->sigma, add_log_term ? k->Dx : nullptr, beta, alpha, y);

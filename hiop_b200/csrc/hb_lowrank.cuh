@@ -1,6 +1,7 @@
 // Shared between hb_lowrank.cu and hb_krylov.cu: the quasi-Newton KKT handle and the two Jacobian gemv helpers.
 #pragma once
 #include "hb_common.cuh"
+#include "hb_dense.cuh"
 
 struct hb_lowrank
 {
@@ -52,7 +53,7 @@ struct hb_lowrank
   const double** chunk_rowptr_dev = nullptr;
   const double** chunk_rowptr_host = nullptr; // pinned, 32 x (m + 2 lmax)
   double* Finv = nullptr;  // 16 x 16 inverses of the diagonal of F (cooperative Cholesky / solve)
-  bool have_finv = false;
+  hb_big big;              // look-ahead Cholesky of large condensed systems: panel stream, events, scratch
   double* lsq_M = nullptr; // m x m LSQ matrix / Cholesky factor + 2 m-vectors (hb_lsq.cu)
   int sec_lcurr = -1, sec_strategy = 1;
   double sec_sigma0 = 1.0;

@@ -75,8 +75,8 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
     HB_LAUNCHED();
   }
   HB_CUDA(cudaMemsetAsync(k->info + 3, 0, sizeof(int), c->stream));
-  HB_CHECK(hb_dense_factor_blocked(c, m, M, m, false, nullptr, k->info + 3));
-  HB_CHECK(hb_dense_tri_solve(c, m, M, m, false, rhs));
+  HB_CHECK(hb_dense_lsq_factor(c, m, M, m, k->info + 3));
+  HB_CHECK(hb_dense_lsq_solve(c, m, M, m, rhs));
   HB_CUDA(cudaMemcpyAsync(k->info_host + 3, k->info + 3, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if(me) HB_CUDA(cudaMemcpyAsync(yc, rhs, sizeof(double) * me, cudaMemcpyDeviceToDevice, c->stream));
   if(mi) HB_CUDA(cudaMemcpyAsync(yd, rhs + me, sizeof(double) * mi, cudaMemcpyDeviceToDevice, c->stream));

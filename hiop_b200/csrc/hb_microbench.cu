@@ -57,7 +57,15 @@ k_peak_i8(int iters, int* __restrict__ sink)
   if(tid == 0) sink[blockIdx.x] = iters;
 }
 
+constexpr int PEAK_I8_SMEM = 48 * 1024 + 1024; // + alignment slack
+
 } // namespace
+
+int hb_microbench_init_attrs(hb_ctx* c)
+{
+  HB_CUDA(cudaFuncSetAttribute(k_peak_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, PEAK_I8_SMEM));
+  return HB_OK;
+}
 
 // which: 0 = FP64 DMMA (TFLOP/s), 1 = INT8 wgmma (TOP/s, 2 ops per MAC)
 extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
@@ -86,12 +94,7 @@ extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
     }
   } else {
     const int blocks = c->num_sms, iters = 20000;
-    const int smem = 48 * 1024 + 1024; // + alignment slack
-    static bool attr[16] = {false};
-    if(c->device < 16 && !attr[c->device]) {
-      HB_CUDA(cudaFuncSetAttribute(k_peak_i8, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      attr[c->device] = true;
-    }
+    const int smem = PEAK_I8_SMEM;
     HB_CHECK(hb_ws_reserve(c, sizeof(int) * (size_t)blocks));
     k_peak_i8<<<blocks, 256, smem, c->stream>>>(200, (int*)c->ws);
     HB_LAUNCHED();

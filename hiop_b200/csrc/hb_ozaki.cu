@@ -426,7 +426,6 @@ k_oz_fixup(int M, int n_tiles, const int2* __restrict__ tile_ij, int splits, con
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled g_encode = nullptr;
 
 struct OzState
 {
@@ -445,6 +444,7 @@ struct OzState
   OzItem* d_items = nullptr;
   int2* d_tiles = nullptr;
   CUtensorMap mapA, mapB;
+  PFN_encodeTiled encode = nullptr; // cuTensorMapEncodeTiled, resolved on first use
 };
 // one state per CONTEXT (it used to be per device: two contexts on one GPU would have shared the slice buffer across their streams)
 void oz_state_free(void* p)
@@ -467,11 +467,6 @@ template <int S>
 int launch_gemm(hb_ctx* c, OzState& st, int chunk_blocks, double* partial)
 {
   const size_t smem = OzCfg<S>::SMEM;
-  static bool attr[16] = {false}; // function attributes are per device
-  if(c->device >= 16 || !attr[c->device]) {
-    HB_CUDA(cudaFuncSetAttribute(k_oz_gemm<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if(c->device < 16) attr[c->device] = true;
-  }
   const int G = st.n_items < c->num_sms ? st.n_items : c->num_sms;
   k_oz_gemm<S><<<G, OZ_THREADS, smem, c->stream>>>(st.mapA, st.mapB, st.d_items, st.n_items, chunk_blocks, partial);
   HB_LAUNCHED();
@@ -479,6 +474,14 @@ int launch_gemm(hb_ctx* c, OzState& st, int chunk_blocks, double* partial)
 }
 
 } // namespace
+
+int hb_ozaki_init_attrs(hb_ctx* c)
+{
+  HB_CUDA(cudaFuncSetAttribute(k_oz_gemm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OzCfg<6>::SMEM));
+  HB_CUDA(cudaFuncSetAttribute(k_oz_gemm<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OzCfg<7>::SMEM));
+  HB_CUDA(cudaFuncSetAttribute(k_oz_gemm<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OzCfg<8>::SMEM));
+  return HB_OK;
+}
 
 // Same contract as hb_syrk_rows (C = A diag(d) A^T, both triangles), computed with S int8 slices on the integer tensor cores.
 // dot_x/dot_out (optional, device): dot_out[i] = sum_k row_i[k] d[k] dot_x[k] over the local columns, produced by the row-maximum pass
@@ -491,12 +494,12 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
     return HB_OK;
   }
-  if(!g_encode) {
-    cudaDriverEntryPointQueryResult qres;
-    HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&g_encode, cudaEnableDefault, &qres));
-    if(!g_encode) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver%s", "");
-  }
   OzState& st = oz_state(c);
+  if(!st.encode) {
+    cudaDriverEntryPointQueryResult qres;
+    HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&st.encode, cudaEnableDefault, &qres));
+    if(!st.encode) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver%s", "");
+  }
   const int Mpad = ((M + TM - 1) / TM) * TM;
   const long long Kpad = ((K + KS - 1) / KS) * KS;
   const size_t qbytes = (size_t)S * Mpad * Kpad;
@@ -574,9 +577,9 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Mpad, (cuuint64_t)S};
     cuuint64_t strides[2] = {(cuuint64_t)Kpad, (cuuint64_t)Kpad * Mpad};
     cuuint32_t boxA[3] = {KS, TM, 1}, boxB[3] = {KS, TN, (cuuint32_t)S}, es[3] = {1, 1, 1};
-    CUresult r1 = g_encode(&st.mapA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxA, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r1 = st.encode(&st.mapA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxA, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CUresult r2 = g_encode(&st.mapB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxB, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r2 = st.encode(&st.mapB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxB, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if(r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled failed%s", "");
     st.M = M; st.K = K; st.S = S; st.Mpad = Mpad; st.Kpad = Kpad; st.splits = splits; st.n_tiles = nt; st.n_items = (int)items.size();

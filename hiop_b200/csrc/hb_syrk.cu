@@ -62,11 +62,6 @@ __device__ __forceinline__ void cp_async_wait()
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
 // Loads one K chunk (BK columns starting at column k0) of the row tile(s) into a stage.
 template <bool ALIGN16>
 __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_a, const double* const* srow_b, bool diag,
@@ -413,16 +408,32 @@ struct Schedule
   Seg* d_segs = nullptr;
 };
 constexpr int SCHED_WAYS = 4;
-Schedule g_sched[16][SCHED_WAYS]; // per device, small LRU cache keyed by (M, K)
-long long g_sched_clock = 0;
+struct ScheduleCache // per context (c->syrk_sched), small LRU cache keyed by (M, K)
+{
+  Schedule ways[SCHED_WAYS];
+  long long clock = 0;
+};
+void schedule_cache_free(void* p)
+{
+  ScheduleCache* sc = static_cast<ScheduleCache*>(p);
+  for(Schedule& S : sc->ways) {
+    cudaFree(S.d_cta_seg_begin); cudaFree(S.d_tile_slot_begin); cudaFree(S.d_tile_slots); cudaFree(S.d_tile_ij); cudaFree(S.d_segs);
+  }
+  delete sc;
+}
 
 int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
 {
-  Schedule* ways = g_sched[c->device];
+  if(!c->syrk_sched) {
+    c->syrk_sched = new ScheduleCache;
+    c->syrk_free = schedule_cache_free;
+  }
+  ScheduleCache& sc = *static_cast<ScheduleCache*>(c->syrk_sched);
+  Schedule* ways = sc.ways;
   int victim = 0;
   for(int w = 0; w < SCHED_WAYS; w++) {
     if(ways[w].M == M && ways[w].K == K && ways[w].bk == bk && ways[w].G == c->num_sms) {
-      ways[w].stamp = ++g_sched_clock;
+      ways[w].stamp = ++sc.clock;
       Sout = &ways[w];
       return HB_OK;
     }
@@ -430,7 +441,7 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   }
   Schedule& S = ways[victim];
   Sout = &S;
-  S.stamp = ++g_sched_clock;
+  S.stamp = ++sc.clock;
   HB_CUDA(cudaStreamSynchronize(c->stream));
   cudaFree(S.d_cta_seg_begin); cudaFree(S.d_tile_slot_begin); cudaFree(S.d_tile_slots); cudaFree(S.d_tile_ij); cudaFree(S.d_segs);
   const int T = (M + BM - 1) / BM;
@@ -511,9 +522,15 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   return HB_OK;
 }
 
-bool g_attr_set = false;
-
 } // namespace
+
+int hb_syrk_init_attrs(hb_ctx* c)
+{
+  HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+  HB_CUDA(cudaFuncSetAttribute(k_syrk_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WSMEM_BYTES));
+  return HB_OK;
+}
 
 // true when an (M+1)-th row adds no tile row to the SYRK of M rows (hb_syrk_rows' fuse_rx costs no extra MMA)
 bool hb_syrk_extra_row_is_free(int M) { return (M + BM) / BM == (M + BM - 1) / BM; }
@@ -532,7 +549,6 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
     if(tdot) HB_CUDA(cudaMemsetAsync(tdot, 0, sizeof(double) * M, c->stream));
     return HB_OK;
   }
-  HB_REQUIRE(c->device < 16, "device ordinal too large");
   const bool d_aligned = (reinterpret_cast<uintptr_t>(d) & 15u) == 0 && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
   const char* force_generic = getenv("HB_SYRK_GENERIC");
   const bool use_ws = aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0) && !(force_generic && force_generic[0] == '1');
@@ -540,12 +556,6 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
   HB_CHECK(build_schedule(c, Sp, M + (fuse_rx ? 1 : 0), K, use_ws ? WBK : BK));
   Schedule& S = *Sp;
   HB_CHECK(hb_ws_reserve(c, (size_t)S.nslots * BM * BM * sizeof(double)));
-  if(!g_attr_set) {
-    HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    HB_CUDA(cudaFuncSetAttribute(k_syrk_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WSMEM_BYTES));
-    g_attr_set = true;
-  }
   const int G = S.Gl;
   if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
   if(use_ws)

@@ -10,7 +10,8 @@ from test_gpu_parity import ctx, _setup_kkt, _as_dict  # noqa: F401
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("n,m,mode", [(3000, 20, -1), (4099, 37, -1), (10000, 1, -1), (40000, 100, 0), (40000, 100, 8), (2500, 0, -1)])
+@pytest.mark.parametrize("n,m,mode", [(3000, 20, -1), (4099, 37, -1), (10000, 1, -1), (40000, 100, 0), (40000, 100, 8), (2500, 0, -1),
+                                      (3000, 64, -1), (3000, 65, -1), (8000, 2049, -1)])  # both sides of the cooperative Cholesky's range
 def test_lsq_duals_against_oracle(ctx, n, m, mode):
     P = synth.make_qn_problem(n, m, 0, seed=5 + n)
     p = _as_dict(P)
