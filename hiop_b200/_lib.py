@@ -53,6 +53,7 @@ def lib() -> ctypes.CDLL:
     f("hb_version", ctypes.c_char_p)
     f("hb_last_error", ctypes.c_char_p)
     f("hb_launch_count", c_ll)
+    f("hb_debug_live_resources", c_ll)
     f("hb_ctx_create", c_i, c_i, P(c_vp))
     f("hb_ctx_destroy", c_i, c_vp)
     f("hb_ctx_sync", c_i, c_vp)

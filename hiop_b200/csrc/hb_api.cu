@@ -10,6 +10,10 @@ extern "C" const char* hb_version(void) { return "hiopb200 0.1.0 (sm_90a)"; }
 extern "C" const char* hb_last_error(void) { return g_hb_err; }
 extern "C" long long hb_launch_count(void) { return g_hb_launches; }
 
+namespace {
+void comm_destroy(hb_ctx* c);
+}
+
 extern "C" int hb_ctx_create(int device, hb_ctx** out)
 {
   HB_REQUIRE(out != nullptr, "hb_ctx_create: out is null");
@@ -29,17 +33,17 @@ extern "C" int hb_ctx_create(int device, hb_ctx** out)
              prop.major, prop.minor);
     return HB_ERR_CUDA;
   }
-  hb_ctx* c = new hb_ctx;
+  std::unique_ptr<hb_ctx> c(new hb_ctx);
   c->device = device;
   c->num_sms = prop.multiProcessorCount;
-  HB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-  HB_CUDA(cudaMalloc(&c->red_dev, sizeof(double) * HB_RED_SLOTS));
-  HB_CUDA(cudaMallocHost(&c->red_host, sizeof(double) * 64));
-  HB_CHECK(hb_syrk_init_attrs(c));
-  HB_CHECK(hb_ozaki_init_attrs(c));
-  HB_CHECK(hb_microbench_init_attrs(c));
-  HB_CHECK(hb_dense_init(c));
-  *out = c;
+  HB_CHECK(c->stream.create(cudaStreamNonBlocking));
+  HB_CHECK(c->red_dev.reserve(c.get(), HB_RED_SLOTS, "reduction scratch"));
+  HB_CHECK(c->red_host.reserve(c.get(), 64, "reduction landing slots"));
+  HB_CHECK(hb_syrk_init_attrs(c.get()));
+  HB_CHECK(hb_ozaki_init_attrs(c.get()));
+  HB_CHECK(hb_microbench_init_attrs(c.get()));
+  HB_CHECK(hb_dense_init(c.get()));
+  *out = c.release();
   return HB_OK;
 }
 
@@ -48,15 +52,7 @@ extern "C" int hb_ctx_destroy(hb_ctx* c)
   if(!c) return HB_OK;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  if(c->oz_state && c->oz_free) c->oz_free(c->oz_state);
-  if(c->syrk_sched && c->syrk_free) c->syrk_free(c->syrk_sched);
-  cudaFree(c->bkc_prof);
-  for(cudaEvent_t e : c->ev_phase) if(e) cudaEventDestroy(e);
-  if(c->ws) cudaFree(c->ws);
-  if(c->ev_syrk0) { cudaEventDestroy(c->ev_syrk0); cudaEventDestroy(c->ev_syrk1); }
-  cudaFree(c->red_dev);
-  cudaFreeHost(c->red_host);
-  cudaStreamDestroy(c->stream);
+  comm_destroy(c);
   delete c;
   return HB_OK;
 }
@@ -64,9 +60,9 @@ extern "C" int hb_ctx_destroy(hb_ctx* c)
 extern "C" int hb_ctx_enable_timing(hb_ctx* c, int on)
 {
   HB_REQUIRE(c, "null ctx");
-  if(on && !c->ev_syrk0) {
-    HB_CUDA(cudaEventCreate(&c->ev_syrk0));
-    HB_CUDA(cudaEventCreate(&c->ev_syrk1));
+  if(on) {
+    HB_CHECK(c->ev_syrk0.create(cudaEventDefault));
+    HB_CHECK(c->ev_syrk1.create(cudaEventDefault));
   }
   c->timing = on != 0;
   c->syrk_timed = false;
@@ -90,8 +86,7 @@ extern "C" int hb_ctx_phase_timeline(hb_ctx* c, int on, float* ms_host10)
 {
   HB_REQUIRE(c, "null ctx");
   if(on) {
-    for(int i = 0; i < HB_PH_COUNT; i++)
-      if(!c->ev_phase[i]) HB_CUDA(cudaEventCreate(&c->ev_phase[i]));
+    for(hb_event& e : c->ev_phase) HB_CHECK(e.create(cudaEventDefault));
     c->phase_mask = 0;
     c->phases = true;
     return HB_OK;
@@ -121,22 +116,65 @@ extern "C" int hb_ctx_device(hb_ctx* c) { return c ? c->device : -1; }
 
 int hb_ws_reserve(hb_ctx* c, size_t bytes)
 {
-  if(bytes <= c->ws_bytes) return HB_OK;
-  if(c->ws) {
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    HB_CUDA(cudaFree(c->ws));
-    c->ws = nullptr;
-    c->ws_bytes = 0;
-  }
-  size_t want = bytes + (bytes >> 3);
-  if(cudaMalloc(&c->ws, want) != cudaSuccess) {
+  const size_t doubles = (bytes + sizeof(double) - 1) / sizeof(double);
+  if(c->ws && doubles <= c->ws.capacity()) return HB_OK;
+  return c->ws.reserve(c, doubles + (doubles >> 3), "workspace");
+}
+
+// ---- owners (hb_common.cuh) ----
+std::atomic<long long> g_hb_live{0};
+extern "C" long long hb_debug_live_resources(void) { return g_hb_live; }
+
+int hb_mem_alloc(void** p, size_t count, size_t elem, bool pinned, const char* what)
+{
+  *p = nullptr;
+  const bool fits = count <= SIZE_MAX / elem;
+  if(!fits || (pinned ? cudaMallocHost(p, count * elem) : cudaMalloc(p, count * elem)) != cudaSuccess) {
     cudaGetLastError();
-    snprintf(g_hb_err, sizeof(g_hb_err), "workspace allocation of %zu bytes failed", want);
+    *p = nullptr;
+    snprintf(g_hb_err, sizeof(g_hb_err), "cannot allocate %.0f bytes of %s memory for %s", (double)count * (double)elem,
+             pinned ? "pinned host" : "device", what);
     return HB_ERR_ALLOC;
   }
-  c->ws_bytes = want;
+  g_hb_live++;
   return HB_OK;
 }
+void hb_mem_free(void* p, bool pinned)
+{
+  if(pinned) cudaFreeHost(p);
+  else cudaFree(p);
+  g_hb_live--;
+}
+
+namespace {
+cudaError_t create_handle(cudaStream_t* s, unsigned flags, int priority) { return cudaStreamCreateWithPriority(s, flags, priority); }
+cudaError_t create_handle(cudaEvent_t* e, unsigned flags, int) { return cudaEventCreateWithFlags(e, flags); }
+void destroy_handle(cudaStream_t s) { cudaStreamDestroy(s); }
+void destroy_handle(cudaEvent_t e) { cudaEventDestroy(e); }
+} // namespace
+
+template <typename H>
+int hb_handle<H>::create(unsigned flags, int priority)
+{
+  if(h_) return HB_OK;
+  const cudaError_t e = create_handle(&h_, flags, priority);
+  if(e != cudaSuccess) {
+    cudaGetLastError();
+    h_ = nullptr;
+    return hb_fail(HB_ERR_CUDA, "stream / event creation failed: %s", cudaGetErrorString(e));
+  }
+  g_hb_live++;
+  return HB_OK;
+}
+template <typename H>
+hb_handle<H>::~hb_handle()
+{
+  if(!h_) return;
+  destroy_handle(h_);
+  g_hb_live--;
+}
+template class hb_handle<cudaStream_t>;
+template class hb_handle<cudaEvent_t>;
 
 extern "C" int hb_malloc(hb_ctx* c, size_t bytes, void** p)
 {
@@ -243,6 +281,12 @@ int nccl_load()
   if(!g_nccl.get_uid || !g_nccl.comm_init || !g_nccl.allreduce) return hb_fail(HB_ERR_COMM, "NCCL symbols missing%s", "");
   g_nccl.h = h;
   return HB_OK;
+}
+
+void comm_destroy(hb_ctx* c)
+{
+  if(c->nccl_comm && g_nccl.comm_destroy) g_nccl.comm_destroy(c->nccl_comm);
+  c->nccl_comm = nullptr;
 }
 } // namespace
 

@@ -696,15 +696,14 @@ int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* i
 int hb_bkc_profile(hb_ctx* c, int on, long long* prof_host8)
 {
   if(on) {
-    if(!c->bkc_prof) HB_CUDA(cudaMalloc(&c->bkc_prof, sizeof(long long) * 8));
+    HB_CHECK(c->bkc_prof.reserve(c, 8, "Bunch-Kaufman profile counters"));
     HB_CUDA(cudaMemsetAsync(c->bkc_prof, 0, sizeof(long long) * 8, c->stream));
   } else if(c->bkc_prof) {
     if(prof_host8) {
       HB_CUDA(cudaMemcpyAsync(prof_host8, c->bkc_prof, sizeof(long long) * 8, cudaMemcpyDeviceToHost, c->stream));
       HB_CUDA(cudaStreamSynchronize(c->stream));
     }
-    cudaFree(c->bkc_prof);
-    c->bkc_prof = nullptr;
+    c->bkc_prof.reset();
   }
   return HB_OK;
 }

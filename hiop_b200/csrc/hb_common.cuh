@@ -1,10 +1,13 @@
 // Shared internals of libhiopb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <atomic>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/hiopb200.h"
@@ -54,43 +57,135 @@ inline int hb_fail(int code, const char* fmt, const char* a = "", int line = 0)
     }                                                                                              \
   } while(0)
 
+// ---- ownership ----------------------------------------------------------------------------------------------------------
+// Every device buffer, pinned buffer, stream and event the engine keeps is held by one of the owners below, and every handle is an
+// aggregate of owners: deleting a handle releases what it holds, and a failed allocation leaves the owner empty, so the next call
+// simply allocates it again. Owners release without synchronising; each *_destroy entry point synchronises the context stream first.
+// g_hb_live counts what the owners hold (hb_debug_live_resources).
+extern std::atomic<long long> g_hb_live;
+struct hb_ctx;
+
+// count elements of elem bytes, in pinned host memory or on the device. On failure *p stays null, the runtime error is cleared and
+// the result is HB_ERR_ALLOC with a message naming `what` and the byte count.
+int hb_mem_alloc(void** p, size_t count, size_t elem, bool pinned, const char* what);
+void hb_mem_free(void* p, bool pinned);
+
+template <typename T, bool PINNED>
+class hb_array
+{
+public:
+  hb_array() = default;
+  hb_array(hb_array&& o) noexcept : p_(o.p_), cap_(o.cap_) { o.p_ = nullptr; o.cap_ = 0; }
+  hb_array& operator=(hb_array&& o) noexcept
+  {
+    std::swap(p_, o.p_);
+    std::swap(cap_, o.cap_);
+    return *this;
+  }
+  ~hb_array() { reset(); }
+  operator T*() const { return p_; }
+  T* get() const { return p_; }
+  size_t capacity() const { return cap_; }
+  void reset()
+  {
+    if(p_) hb_mem_free(p_, PINNED);
+    p_ = nullptr;
+    cap_ = 0;
+  }
+  // Holds at least max(count, 1) elements afterwards, or nothing when the allocation fails (HB_ERR_ALLOC). Growing waits for the
+  // context stream, frees the old array and then allocates: the contents are not kept.
+  int reserve(hb_ctx* c, size_t count, const char* what);
+
+private:
+  T* p_ = nullptr;
+  size_t cap_ = 0;
+};
+template <typename T> using hb_dev = hb_array<T, false>;
+template <typename T> using hb_pinned = hb_array<T, true>;
+
+// an owned cudaStream_t (hb_stream) or cudaEvent_t (hb_event)
+template <typename H>
+class hb_handle
+{
+public:
+  hb_handle() = default;
+  hb_handle(const hb_handle&) = delete;
+  hb_handle& operator=(const hb_handle&) = delete;
+  ~hb_handle();
+  operator H() const { return h_; }
+  int create(unsigned flags, int priority = 0); // no-op while one is held; the priority applies to streams
+
+private:
+  H h_ = nullptr;
+};
+using hb_stream = hb_handle<cudaStream_t>;
+using hb_event = hb_handle<cudaEvent_t>;
+
+// per-context state defined in one kernel file each: the int8-slice condensation (hb_ozaki.cu), the SYRK schedule cache (hb_syrk.cu)
+struct OzState;
+struct ScheduleCache;
+void hb_delete(OzState* p);
+void hb_delete(ScheduleCache* p);
+struct hb_deleter
+{
+  template <typename S> void operator()(S* p) const { hb_delete(p); }
+};
+template <typename S> using hb_state = std::unique_ptr<S, hb_deleter>;
+
+// phase marks of the quasi-Newton step (ids are the HB_PH_* below); a no-op unless hb_ctx_phase_timeline switched them on
+enum { HB_PH_START = 0, HB_PH_UPDATE, HB_PH_OZ_ROWMAX, HB_PH_OZ_SLICE, HB_PH_CAUG, HB_PH_ALLREDUCE, HB_PH_VN, HB_PH_CHOL, HB_PH_HSOLVE1, HB_PH_JX, HB_PH_SPDSOLVE, HB_PH_JTY, HB_PH_HSOLVE2, HB_PH_COUNT };
+
 struct hb_ctx
 {
   int device = 0;
   int num_sms = HB_NUM_SMS_DEFAULT;
-  cudaStream_t stream = nullptr;
+  hb_stream stream;
   // scratch for reductions: per-CTA partials + a pinned host landing slot
-  double* red_dev = nullptr;     // RED_SLOTS doubles
-  double* red_host = nullptr;    // pinned, 64 doubles
-  // generic workspace (grown on demand)
-  void* ws = nullptr;
-  size_t ws_bytes = 0;
+  hb_dev<double> red_dev;     // RED_SLOTS doubles
+  hb_pinned<double> red_host; // 64 doubles
+  // generic workspace (grown on demand by hb_ws_reserve)
+  hb_dev<double> ws;
   // optional kernel timing (roofline reporting)
   bool timing = false;
-  cudaEvent_t ev_syrk0 = nullptr, ev_syrk1 = nullptr;
+  hb_event ev_syrk0, ev_syrk1;
   bool syrk_timed = false;
   // phase timeline (hb_ctx_phase_timeline): events recorded at fixed points of one update + condense + solve when enabled
   bool phases = false;
-  cudaEvent_t ev_phase[16] = {nullptr};
+  hb_event ev_phase[HB_PH_COUNT];
   unsigned phase_mask = 0;
   // per-context state of the int8-slice condensation (hb_ozaki.cu): slice buffer, exponents, tensor maps, work list
-  void* oz_state = nullptr;
-  void (*oz_free)(void*) = nullptr;
+  hb_state<OzState> oz;
   // schedule cache of the FP64 condensation (hb_syrk.cu)
-  void* syrk_sched = nullptr;
-  void (*syrk_free)(void*) = nullptr;
+  hb_state<ScheduleCache> syrk_sched;
   // dense symmetric solvers: size thresholds (with their environment overrides, set by hb_dense_init in hb_symdense.cu) and the
   // number of CTAs of the cooperative Cholesky resident at once (0: no cooperative kernels -- unsupported, or HB_CHOL_COOP=0)
   int bk_cluster_min = 0, big_min_chol = 0, big_min_ldl = 0, pair_min = 0;
   int coop_ctas = 0;
-  long long* bkc_prof = nullptr; // diagnostics: 8 cycle counters of the cluster Bunch-Kaufman panel while profiling is on
-  // NCCL
+  hb_dev<long long> bkc_prof; // diagnostics: 8 cycle counters of the cluster Bunch-Kaufman panel while profiling is on
+  // NCCL (destroyed by hb_ctx_destroy)
   void* nccl_comm = nullptr;
   int nranks = 1, rank = 0;
 };
 
+template <typename T, bool PINNED>
+int hb_array<T, PINNED>::reserve(hb_ctx* c, size_t count, const char* what)
+{
+  if(p_ && count <= cap_) return HB_OK;
+  if(p_) {
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    reset();
+  }
+  const size_t n = count ? count : 1;
+  void* q = nullptr;
+  HB_CHECK(hb_mem_alloc(&q, n, sizeof(T), PINNED, what));
+  p_ = static_cast<T*>(q);
+  cap_ = n;
+  return HB_OK;
+}
+
 static constexpr int HB_RED_SLOTS = 4096;
 
+// c->ws holds at least `bytes` afterwards
 int hb_ws_reserve(hb_ctx* ctx, size_t bytes);
 
 // set once by hb_ctx_create: the dynamic-shared-memory / cluster attributes of each kernel file's kernels (function attributes are
@@ -100,8 +195,6 @@ int hb_ozaki_init_attrs(hb_ctx* c);
 int hb_microbench_init_attrs(hb_ctx* c);
 int hb_dense_init(hb_ctx* c);
 
-// phase marks of the quasi-Newton step (ids are the HB_PH_* below); a no-op unless hb_ctx_phase_timeline switched them on
-enum { HB_PH_START = 0, HB_PH_UPDATE, HB_PH_OZ_ROWMAX, HB_PH_OZ_SLICE, HB_PH_CAUG, HB_PH_ALLREDUCE, HB_PH_VN, HB_PH_CHOL, HB_PH_HSOLVE1, HB_PH_JX, HB_PH_SPDSOLVE, HB_PH_JTY, HB_PH_HSOLVE2, HB_PH_COUNT };
 inline void hb_phase_mark(hb_ctx* c, int id)
 {
   if(c->phases && c->ev_phase[id]) {

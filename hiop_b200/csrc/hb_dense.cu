@@ -949,7 +949,7 @@ int hb_dense_sytrf_blocked(hb_ctx* c, int N, double* A, int lda, int* ipiv_dev, 
   if(N == 0) return HB_OK;
   // device state word (k0, kb, info) in the workspace
   HB_CHECK(hb_ws_reserve(c, 64));
-  int* state = reinterpret_cast<int*>(c->ws);
+  int* state = reinterpret_cast<int*>(c->ws.get());
   HB_CUDA(cudaMemsetAsync(state, 0, sizeof(int) * 4, c->stream));
   const int max_panels = (N + (NB - 1) - 1) / (NB - 1) + 1;
   for(int p = 0; p < max_panels; p++) {
@@ -989,7 +989,7 @@ int hb_dense_inertia_ipiv(hb_ctx* c, int N, const double* A, int lda, const int*
 {
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * 2 * (size_t)(N > 0 ? N : 1) + 256));
   k_inertia<<<1, 1024, 0, c->stream>>>(A, lda, N, ipiv_dev, HB_FACT_BUNCH_KAUFMAN, out3_dev,
-                                       reinterpret_cast<double*>(reinterpret_cast<char*>(c->ws) + 256));
+                                       reinterpret_cast<double*>(reinterpret_cast<char*>(c->ws.get()) + 256));
   HB_LAUNCHED();
   return HB_OK;
 }

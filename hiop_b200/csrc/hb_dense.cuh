@@ -97,20 +97,24 @@ int hb_dense_spd_solve_coop(hb_ctx* c, int N, const double* F, int ldf, const do
 // ---- large-N path (hb_dense_big.cu): blocked Cholesky / no-pivot LDL^T with look-ahead, 128 x 128 diagonal-block inverses, blocked solves ----
 struct hb_big
 {
-  cudaStream_t panel_stream = nullptr;
-  cudaEvent_t ev_panel = nullptr, ev_upd = nullptr, ev_upd2 = nullptr;
-  double* InvAll = nullptr;         // ceil(N/128) inverses of the 128 x 128 diagonal triangles of the factor (column-major, zeros above)
-  double* W[2] = {nullptr, nullptr}; // LDL^T: W = L*D of the current PAIR of panels, 256 p-major rows (double-buffered across the look-ahead)
-  double* dinv = nullptr;
-  double* partial = nullptr;        // solve: per-CTA partial products
-  int* counter = nullptr;           // solve: ticket of the "last CTA finishes the step" pattern (self-resetting)
-  double* xtmp = nullptr;           // permuted rhs (Bunch-Kaufman)
+  hb_stream panel_stream;
+  hb_event ev_panel, ev_upd, ev_upd2;
+  hb_dev<double> InvAll;  // ceil(N/128) inverses of the 128 x 128 diagonal triangles of the factor (column-major, zeros above)
+  hb_dev<double> W[2];    // LDL^T: W = L*D of the current PAIR of panels, 256 p-major rows (double-buffered across the look-ahead)
+  hb_dev<double> dinv;
+  hb_dev<double> partial; // solve: per-CTA partial products
+  hb_dev<int> counter;    // solve: ticket of the "last CTA finishes the step" pattern (self-resetting)
+  hb_dev<double> xtmp;    // permuted rhs (Bunch-Kaufman)
   int capN = 0;
   bool inv_valid = false;
+  // the panel stream may still run the last panel of a factorization when its owner is destroyed
+  ~hb_big()
+  {
+    if(panel_stream) cudaStreamSynchronize(panel_stream);
+  }
 };
 int hb_big_init_attrs(hb_ctx* c);
 int hb_big_init(hb_ctx* c, hb_big* b);
-void hb_big_release(hb_big* b);
 int hb_big_reserve(hb_ctx* c, hb_big* b, int N, bool need_w);
 // pairs: factor the 128-column blocks in pairs (K = 256 trailing updates)
 int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ldl, bool pairs, int* info_dev);

@@ -870,57 +870,34 @@ int hb_big_init(hb_ctx* c, hb_big* b)
   if(!b->panel_stream) {
     int lo = 0, hi = 0;
     HB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    HB_CUDA(cudaStreamCreateWithPriority(&b->panel_stream, cudaStreamNonBlocking, hi));
-    HB_CUDA(cudaEventCreateWithFlags(&b->ev_panel, cudaEventDisableTiming));
-    HB_CUDA(cudaEventCreateWithFlags(&b->ev_upd, cudaEventDisableTiming));
-    HB_CUDA(cudaEventCreateWithFlags(&b->ev_upd2, cudaEventDisableTiming));
+    HB_CHECK(b->panel_stream.create(cudaStreamNonBlocking, hi));
   }
+  HB_CHECK(b->ev_panel.create(cudaEventDisableTiming));
+  HB_CHECK(b->ev_upd.create(cudaEventDisableTiming));
+  HB_CHECK(b->ev_upd2.create(cudaEventDisableTiming));
   return HB_OK;
-}
-
-void hb_big_release(hb_big* b)
-{
-  if(b->panel_stream) {
-    cudaStreamSynchronize(b->panel_stream);
-    cudaStreamDestroy(b->panel_stream);
-    cudaEventDestroy(b->ev_panel);
-    cudaEventDestroy(b->ev_upd);
-    cudaEventDestroy(b->ev_upd2);
-    b->panel_stream = nullptr;
-  }
-  cudaFree(b->InvAll); cudaFree(b->W[0]); cudaFree(b->W[1]); cudaFree(b->dinv); cudaFree(b->partial); cudaFree(b->counter); cudaFree(b->xtmp);
-  b->InvAll = b->W[0] = b->W[1] = b->dinv = b->partial = b->xtmp = nullptr;
-  b->counter = nullptr;
-  b->capN = 0;
 }
 
 int hb_big_reserve(hb_ctx* c, hb_big* b, int N, bool need_w)
 {
   HB_CHECK(hb_big_init(c, b));
-  const int nblk = (N + BB - 1) / BB;
-  if(b->capN < N) {
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    cudaFree(b->InvAll); cudaFree(b->partial); cudaFree(b->xtmp); cudaFree(b->W[0]); cudaFree(b->W[1]);
-    b->W[0] = b->W[1] = nullptr;
-    if(cudaMalloc(&b->InvAll, sizeof(double) * (size_t)nblk * BB * BB) != cudaSuccess || cudaMalloc(&b->partial, sizeof(double) * (size_t)(N / 64 + 2) * SB) != cudaSuccess ||
-       cudaMalloc(&b->xtmp, sizeof(double) * (size_t)(N + 2)) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "hb_big_reserve: scratch allocation failed%s", "");
-    }
-    HB_CUDA(cudaMemsetAsync(b->InvAll, 0, sizeof(double) * (size_t)nblk * BB * BB, c->stream)); // the kernels only write the lower triangles
-    if(!b->dinv) HB_CUDA(cudaMalloc(&b->dinv, sizeof(double) * (BB + 8 * 16 * 17)));
-    if(!b->counter) {
-      HB_CUDA(cudaMalloc(&b->counter, sizeof(int) * 4));
-      HB_CUDA(cudaMemsetAsync(b->counter, 0, sizeof(int) * 4, c->stream));
-    }
-    b->capN = N;
+  const size_t inv = (size_t)((N + BB - 1) / BB) * BB * BB;
+  if(!b->InvAll || b->InvAll.capacity() < inv) {
+    HB_CHECK(b->InvAll.reserve(c, inv, "diagonal-block inverses"));
+    HB_CUDA(cudaMemsetAsync(b->InvAll, 0, sizeof(double) * b->InvAll.capacity(), c->stream)); // the kernels only write the lower triangles
   }
-  if(need_w && !b->W[0]) {
+  HB_CHECK(b->partial.reserve(c, (size_t)(N / 64 + 2) * SB, "blocked-solve partials"));
+  HB_CHECK(b->xtmp.reserve(c, (size_t)(N + 2), "permuted rhs"));
+  HB_CHECK(b->dinv.reserve(c, BB + 8 * 16 * 17, "diagonal-block scratch"));
+  if(!b->counter) {
+    HB_CHECK(b->counter.reserve(c, 4, "blocked-solve ticket"));
+    HB_CUDA(cudaMemsetAsync(b->counter, 0, sizeof(int) * 4, c->stream));
+  }
+  if(b->capN < N) b->capN = N;
+  if(need_w) {
     const size_t ldw = (size_t)((N + 7) & ~7);
-    if(cudaMalloc(&b->W[0], sizeof(double) * ldw * 2 * BB) != cudaSuccess || cudaMalloc(&b->W[1], sizeof(double) * ldw * 2 * BB) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "hb_big_reserve: panel scratch allocation failed%s", "");
-    }
+    HB_CHECK(b->W[0].reserve(c, ldw * 2 * BB, "LDL panel scratch"));
+    HB_CHECK(b->W[1].reserve(c, ldw * 2 * BB, "LDL panel scratch"));
   }
   return HB_OK;
 }
@@ -975,7 +952,7 @@ int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ld
   for(int a = 0; GW * a < nblk; a++) {
     const int b0 = GW * a, b1 = GW == 2 ? 2 * a + 1 : nblk; // b1 >= nblk: no second block
     const int k0 = b0 * BB;                                   // first column of the group
-    double* Wp = ldl ? b->W[a & 1] : nullptr;                 // W = L*D of the group's panels, p-major rows
+    double* Wp = ldl ? b->W[a & 1].get() : nullptr;           // W = L*D of the group's panels, p-major rows
     // ---- panel stream ----
     HB_CUDA(cudaStreamWaitEvent(sp, b->ev_upd, 0));
     HB_CHECK(panel(b0, Wp));
@@ -1016,18 +993,17 @@ int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ld
 int hb_big_diag_profile(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int k0, bool ldl, long long* prof_host8)
 {
   HB_CHECK(hb_big_reserve(c, b, N, false));
-  long long* prof = nullptr;
-  HB_CUDA(cudaMalloc(&prof, sizeof(long long) * 8));
+  hb_dev<long long> prof;
+  hb_dev<int> info;
+  HB_CHECK(prof.reserve(c, 8, "profile counters"));
+  HB_CHECK(info.reserve(c, 1, "profile info word"));
   HB_CUDA(cudaMemsetAsync(prof, 0, sizeof(long long) * 8, c->stream));
-  int* info = nullptr;
-  HB_CUDA(cudaMalloc(&info, sizeof(int)));
   HB_CUDA(cudaMemsetAsync(info, 0, sizeof(int), c->stream));
   if(ldl) k_diag128<true><<<1, DTHREADS, sizeof(DiagSmem), c->stream>>>(A, lda, N, k0, b->dinv + BB, b->dinv, info, prof);
   else k_diag128<false><<<1, DTHREADS, sizeof(DiagSmem), c->stream>>>(A, lda, N, k0, b->dinv + BB, b->dinv, info, prof);
   HB_LAUNCHED();
   HB_CUDA(cudaMemcpyAsync(prof_host8, prof, sizeof(long long) * 8, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  cudaFree(prof); cudaFree(info);
   return HB_OK;
 }
 

@@ -283,7 +283,7 @@ extern "C" int hb_iterate_adjust_small_slacks(hb_lowrank* k, double* const* it, 
   const double small_val = eps * fmin(1.0, mu);
   const double scale_fact = pow(eps, 0.75);
   HB_CHECK(hb_ws_reserve(c, 64));
-  int* cnt = (int*)c->ws;
+  int* cnt = (int*)c->ws.get();
   HB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int), c->stream));
   struct Blk { int s, z; const double* bound; const double* sel; long long len; };
   const Blk blks[4] = {{SXL, ZL, xl, k->ixl, k->n}, {SXU, ZU, xu, k->ixu, k->n}, {SDL, VL, dl, k->idl, (long long)k->mineq},

@@ -100,18 +100,11 @@ constexpr int KRY_EXTRA = 4 * 2048 + 64;
 int ensure_ws(hb_lowrank* k, const Layout& L, int nvec)
 {
   if(!k->kry) {
-    if(cudaMalloc(&k->kry, sizeof(double) * (size_t)L.total * nvec) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "BiCGStab workspace allocation failed%s", "");
-    }
-    // 2 m-vectors + the device scalars and per-CTA partial sums of the recurrence (KRY_EXTRA doubles)
-    if(cudaMalloc(&k->kry_m, sizeof(double) * (size_t)(2 * k->m + 2 + KRY_EXTRA)) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "BiCGStab m-workspace%s", "");
-    }
+    HB_CHECK(k->kry.reserve(k->ctx, (size_t)L.total * nvec, "the BiCGStab workspace"));
     HB_CUDA(cudaMemsetAsync(k->kry, 0, sizeof(double) * (size_t)L.total * nvec, k->ctx->stream));
   }
-  return HB_OK;
+  // 2 m-vectors + the device scalars and per-CTA partial sums of the recurrence (KRY_EXTRA doubles)
+  return k->kry_m.reserve(k->ctx, (size_t)(2 * k->m + 2 + KRY_EXTRA), "the BiCGStab m-workspace");
 }
 
 // y = K x on compound buffers (y and x must not alias)

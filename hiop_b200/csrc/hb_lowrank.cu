@@ -395,16 +395,6 @@ __global__ void k_fused_rhs(int m, int meq, int l, double sigma, const double* _
 // =============================================================================================================
 namespace {
 
-int dmalloc(double** p, size_t count)
-{
-  if(cudaMalloc(p, sizeof(double) * (count ? count : 1)) != cudaSuccess) {
-    cudaGetLastError();
-    snprintf(g_hb_err, sizeof(g_hb_err), "device allocation of %zu doubles failed", count);
-    return HB_ERR_ALLOC;
-  }
-  return HB_OK;
-}
-
 int refresh_rowptr(hb_lowrank* k)
 {
   if(!k->rowptr_dirty) return HB_OK;
@@ -552,12 +542,12 @@ int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
     k->condense_used = mode;
     if(mode == 0) {
       const bool fuse = fuse_rx && m > 0 && hb_syrk_extra_row_is_free(Ma) && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
-      HB_CHECK(hb_syrk_rows(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, fuse ? fuse_rx : nullptr, fuse ? k->tdot : nullptr));
+      HB_CHECK(hb_syrk_rows(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
       k->tdot_valid = fuse;
     } else {
       const bool fuse = fuse_rx && m > 0;
       if(fuse && k->n == 0) HB_CUDA(cudaMemsetAsync(k->tdot, 0, sizeof(double) * Ma, c->stream));
-      HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot : nullptr));
+      HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
       k->tdot_valid = fuse;
     }
   }
@@ -574,7 +564,7 @@ int condense_finish(hb_lowrank* k)
   if(Ma > 0 && c->nranks > 1) {
     // the symmetric C_aug travels as its packed upper triangle: Ma(Ma+1)/2 doubles instead of Ma^2
     const long long tot = (long long)Ma * (Ma + 1) / 2;
-    if(!k->tri) HB_CHECK(dmalloc(&k->tri, (size_t)(k->m + 2 * k->lmax) * (k->m + 2 * k->lmax + 1) / 2 + (size_t)(k->m + 2 * k->lmax)));
+    HB_CHECK(k->tri.reserve(c, (size_t)(k->m + 2 * k->lmax) * (k->m + 2 * k->lmax + 1) / 2 + (size_t)(k->m + 2 * k->lmax), "packed C_aug"));
     const int g = (int)((tot + 255) / 256 < (long long)c->num_sms * 8 ? (tot + 255) / 256 : (long long)c->num_sms * 8);
     k_pack_upper<<<g, 256, 0, c->stream>>>(Ma, k->Caug, Ma, k->tri);
     HB_LAUNCHED();
@@ -627,36 +617,37 @@ extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_i
 {
   HB_REQUIRE(c && out && n_local >= 0 && m_eq >= 0 && m_ineq >= 0 && l_max >= 0 && l_max <= 256, "hb_lowrank_create: bad arguments");
   HB_CUDA(cudaSetDevice(c->device));
-  hb_lowrank* k = new hb_lowrank;
+  std::unique_ptr<hb_lowrank> k(new hb_lowrank);
   k->ctx = c; k->n = n_local; k->meq = m_eq; k->mineq = m_ineq; k->m = m_eq + m_ineq; k->lmax = l_max;
   if(const char* e = getenv("HB_CONDENSE")) { // "oz6" | "oz7" | "oz8" | "dmma"
     if(e[0] == 'o' && e[1] == 'z' && e[2] >= '6' && e[2] <= '8') k->condense_mode = e[2] - '0';
     else if(e[0] == 'd') k->condense_mode = 0;
   }
   const int m = k->m, Mamax = m + 2 * l_max, l2 = 2 * l_max;
-  HB_CHECK(dmalloc(&k->Dx, n_local)); HB_CHECK(dmalloc(&k->DhInv, n_local));
-  HB_CHECK(dmalloc(&k->Dd, m_ineq)); HB_CHECK(dmalloc(&k->Dd_inv, m_ineq));
-  HB_CHECK(dmalloc(&k->Caug, (size_t)Mamax * Mamax));
-  HB_CHECK(dmalloc(&k->SSt, (size_t)l_max * l_max)); HB_CHECK(dmalloc(&k->Ld, (size_t)l_max * l_max)); HB_CHECK(dmalloc(&k->Dd_sec, l_max));
-  HB_CHECK(dmalloc(&k->V, (size_t)l2 * l2)); HB_CHECK(dmalloc(&k->Mdir, (size_t)l2 * l2));
-  HB_CHECK(dmalloc(&k->U, (size_t)m * l2)); HB_CHECK(dmalloc(&k->Z, (size_t)m * l2));
-  HB_CHECK(dmalloc(&k->Nmat, (size_t)m * m)); HB_CHECK(dmalloc(&k->F, (size_t)m * m));
-  HB_CHECK(dmalloc(&k->svec, m)); HB_CHECK(dmalloc(&k->rhs, m)); HB_CHECK(dmalloc(&k->dy, m)); HB_CHECK(dmalloc(&k->work, 2 * (size_t)m + 2));
-  HB_CHECK(dmalloc(&k->Finv, HB_CHOL_INV_DOUBLES(m > 0 ? m : 1)));
-  HB_CHECK(dmalloc(&k->stats, 4));
-  HB_CHECK(dmalloc(&k->nv1, n_local)); HB_CHECK(dmalloc(&k->nv2, n_local));
-  HB_CHECK(dmalloc(&k->tdot, (size_t)Mamax));
-  HB_CHECK(dmalloc(&k->p2l, l2));
+  HB_CHECK(k->Dx.reserve(c, n_local, "Dx")); HB_CHECK(k->DhInv.reserve(c, n_local, "DhInv"));
+  HB_CHECK(k->Dd.reserve(c, m_ineq, "Dd")); HB_CHECK(k->Dd_inv.reserve(c, m_ineq, "Dd_inv"));
+  HB_CHECK(k->Caug.reserve(c, (size_t)Mamax * Mamax, "C_aug"));
+  HB_CHECK(k->SSt.reserve(c, (size_t)l_max * l_max, "S S^T")); HB_CHECK(k->Ld.reserve(c, (size_t)l_max * l_max, "L")); HB_CHECK(k->Dd_sec.reserve(c, l_max, "D"));
+  HB_CHECK(k->V.reserve(c, (size_t)l2 * l2, "V")); HB_CHECK(k->Mdir.reserve(c, (size_t)l2 * l2, "M"));
+  HB_CHECK(k->U.reserve(c, (size_t)m * l2, "U")); HB_CHECK(k->Z.reserve(c, (size_t)m * l2, "Z"));
+  HB_CHECK(k->Nmat.reserve(c, (size_t)m * m, "N")); HB_CHECK(k->F.reserve(c, (size_t)m * m, "the factor of N"));
+  HB_CHECK(k->svec.reserve(c, m, "the scaling of N")); HB_CHECK(k->rhs.reserve(c, m, "rhs")); HB_CHECK(k->dy.reserve(c, m, "dy"));
+  HB_CHECK(k->work.reserve(c, 2 * (size_t)m + 2, "refinement scratch"));
+  HB_CHECK(k->Finv.reserve(c, HB_CHOL_INV_DOUBLES(m > 0 ? m : 1), "diagonal-block inverses of N"));
+  HB_CHECK(k->stats.reserve(c, 4, "solve statistics"));
+  HB_CHECK(k->nv1.reserve(c, n_local, "n-vector scratch")); HB_CHECK(k->nv2.reserve(c, n_local, "n-vector scratch"));
+  HB_CHECK(k->tdot.reserve(c, (size_t)Mamax, "fused row dots"));
+  HB_CHECK(k->p2l.reserve(c, l2, "multi-dot result"));
   k->md_grid = stream_grid(c, n_local);
-  HB_CHECK(dmalloc(&k->md_partial, (size_t)k->md_grid * (l2 > 0 ? l2 : 1)));
-  HB_CHECK(dmalloc(&k->mi1, m_ineq)); HB_CHECK(dmalloc(&k->mi2, m_ineq)); HB_CHECK(dmalloc(&k->mi3, m_ineq));
-  HB_CUDA(cudaMalloc(&k->ipivV, sizeof(int) * (l2 + 1))); HB_CUDA(cudaMalloc(&k->ipivM, sizeof(int) * (l2 + 1)));
-  HB_CUDA(cudaMalloc(&k->info, sizeof(int) * 4));
-  HB_CUDA(cudaMalloc(&k->rowptr_dev, sizeof(double*) * (Mamax + 2)));
-  HB_CUDA(cudaMallocHost(&k->rowptr_host, sizeof(double*) * (Mamax + 2)));
-  HB_CUDA(cudaMallocHost(&k->info_host, sizeof(int) * 4));
-  HB_CUDA(cudaMallocHost(&k->stats_host, sizeof(double) * 4));
-  *out = k;
+  HB_CHECK(k->md_partial.reserve(c, (size_t)k->md_grid * (l2 > 0 ? l2 : 1), "multi-dot partials"));
+  HB_CHECK(k->mi1.reserve(c, m_ineq, "m_ineq scratch")); HB_CHECK(k->mi2.reserve(c, m_ineq, "m_ineq scratch"));
+  HB_CHECK(k->ipivV.reserve(c, (size_t)l2 + 1, "pivots of V")); HB_CHECK(k->ipivM.reserve(c, (size_t)l2 + 1, "pivots of M"));
+  HB_CHECK(k->info.reserve(c, 4, "info words"));
+  HB_CHECK(k->rowptr_dev.reserve(c, (size_t)Mamax + 2, "row pointers"));
+  HB_CHECK(k->rowptr_host.reserve(c, (size_t)Mamax + 2, "row pointers"));
+  HB_CHECK(k->info_host.reserve(c, 4, "info words"));
+  HB_CHECK(k->stats_host.reserve(c, 4, "solve statistics"));
+  *out = k.release();
   return HB_OK;
 }
 
@@ -665,18 +656,6 @@ extern "C" int hb_lowrank_destroy(hb_lowrank* k)
   if(!k) return HB_OK;
   cudaSetDevice(k->ctx->device);
   cudaStreamSynchronize(k->ctx->stream);
-  double* bufs[] = {k->Dx, k->DhInv, k->Dd, k->Dd_inv, k->Jpack, k->Caug, k->SSt, k->Ld, k->Dd_sec, k->V, k->Mdir, k->U, k->Z, k->Nmat, k->F,
-                    k->svec, k->rhs, k->dy, k->work, k->stats, k->nv1, k->nv2, k->p2l, k->md_partial, k->mi1, k->mi2, k->mi3, k->hJ, k->kry, k->kry_m, k->sec_S, k->sec_Y, k->sec_xprev, k->sec_gprev, k->sec_Jprev, k->lsq_M, k->Finv, k->Ctmp, k->tri, k->tdot};
-  for(double* b : bufs) if(b) cudaFree(b);
-  for(double* b : k->hbuf) if(b) cudaFree(b);
-  cudaFree(k->ipivV); cudaFree(k->ipivM); cudaFree(k->info); cudaFree(k->rowptr_dev);
-  hb_big_release(&k->big);
-  cudaFreeHost(k->rowptr_host); cudaFreeHost(k->info_host); cudaFreeHost(k->stats_host);
-  if(k->copy_stream) {
-    cudaStreamDestroy(k->copy_stream);
-    for(cudaEvent_t e : k->chunk_ev) if(e) cudaEventDestroy(e);
-    cudaFree(k->chunk_rowptr_dev); cudaFreeHost(k->chunk_rowptr_host);
-  }
   delete k;
   return HB_OK;
 }
@@ -700,7 +679,7 @@ extern "C" int hb_lowrank_set_jacobian(hb_lowrank* k, const double* Jc, const do
   if(k->meq == 0) J = Jd;
   else if(k->mineq == 0 || Jd == Jc + (size_t)k->meq * k->n) J = Jc;
   else {
-    if(!k->Jpack) HB_CHECK(dmalloc(&k->Jpack, (size_t)k->m * k->n));
+    HB_CHECK(k->Jpack.reserve(c, (size_t)k->m * k->n, "the packed Jacobian"));
     HB_CUDA(cudaMemcpyAsync(k->Jpack, Jc, sizeof(double) * (size_t)k->meq * k->n, cudaMemcpyDeviceToDevice, c->stream));
     HB_CUDA(cudaMemcpyAsync(k->Jpack + (size_t)k->meq * k->n, Jd, sizeof(double) * (size_t)k->mineq * k->n, cudaMemcpyDeviceToDevice, c->stream));
     J = k->Jpack;
@@ -917,15 +896,15 @@ extern "C" int hb_lowrank_hess_times_vec(hb_lowrank* k, double beta, double* y, 
     HB_CHECK(hb_dense_bk_small_solve(c, 2 * l, k->Mdir, 2 * l, k->ipivM, k->p2l, 2 * l, 1));
   }
   k_lowrank_apply<<<stream_grid(c, k->n), ET, sizeof(double) * 2 * (l > 0 ? l : 1), c->stream>>>(
-      k->n, l, k->sigma, k->St, k->Yt, k->n, k->p2l, nullptr, x, k->sigma, add_log_term ? k->Dx : nullptr, beta, alpha, y);
+      k->n, l, k->sigma, k->St, k->Yt, k->n, k->p2l, nullptr, x, k->sigma, add_log_term ? k->Dx.get() : nullptr, beta, alpha, y);
   HB_LAUNCHED();
   return HB_OK;
 }
 
-extern "C" const double* hb_lowrank_Dx(hb_lowrank* k) { return k ? k->Dx : nullptr; }
-extern "C" const double* hb_lowrank_DhInv(hb_lowrank* k) { return k ? k->DhInv : nullptr; }
-extern "C" const double* hb_lowrank_Dd_inv(hb_lowrank* k) { return k ? k->Dd_inv : nullptr; }
-extern "C" const double* hb_lowrank_N(hb_lowrank* k) { return k ? k->Nmat : nullptr; }
+extern "C" const double* hb_lowrank_Dx(hb_lowrank* k) { return k ? k->Dx.get() : nullptr; }
+extern "C" const double* hb_lowrank_DhInv(hb_lowrank* k) { return k ? k->DhInv.get() : nullptr; }
+extern "C" const double* hb_lowrank_Dd_inv(hb_lowrank* k) { return k ? k->Dd_inv.get() : nullptr; }
+extern "C" const double* hb_lowrank_N(hb_lowrank* k) { return k ? k->Nmat.get() : nullptr; }
 
 // ---- one whole KKT system from host buffers ----------------------------------------------------------------------------
 extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, const double* Jd_host, const double* zl, const double* sxl,
@@ -940,8 +919,7 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   // device staging: 0..3 x-side iterate, 4..7 d-side iterate, 8 rx, 9 ryc, 10 ryd, 11 dx, 12 dyc, 13 dyd
   const size_t sz[14] = {(size_t)n, (size_t)n, (size_t)n, (size_t)n, (size_t)mi, (size_t)mi, (size_t)mi, (size_t)mi, (size_t)n, (size_t)meq, (size_t)mi,
                          (size_t)n, (size_t)meq, (size_t)mi};
-  for(int i = 0; i < 14; i++)
-    if(!k->hbuf[i]) HB_CHECK(dmalloc(&k->hbuf[i], sz[i]));
+  for(int i = 0; i < 14; i++) HB_CHECK(k->hbuf[i].reserve(c, sz[i], "host-call staging"));
   const double* src[11] = {zl, sxl, zu, sxu, vl, sdl, vu, sdu, rx, ryc, ryd};
   for(int i = 0; i < 11; i++)
     if(sz[i]) {
@@ -955,7 +933,7 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   // partial C_aug are added in chunk order, so the result does not depend on timing.
   static const size_t chunk_min_bytes = getenv("HB_HOST_CHUNK_MIN_BYTES") ? (size_t)atoll(getenv("HB_HOST_CHUNK_MIN_BYTES")) : ((size_t)256 << 20);
   const bool chunked = have_J && Ma > 0 && (k->condense_mode <= 0) && (size_t)m * n * sizeof(double) >= chunk_min_bytes && n >= 2048;
-  if(have_J && !k->hJ) HB_CHECK(dmalloc(&k->hJ, (size_t)k->m * n));
+  if(have_J) HB_CHECK(k->hJ.reserve(c, (size_t)k->m * n, "the staged Jacobian"));
   if(have_J && !chunked) {
     if(meq) HB_CUDA(cudaMemcpyAsync(k->hJ, Jc_host, sizeof(double) * (size_t)meq * n, cudaMemcpyHostToDevice, c->stream));
     if(mi) HB_CUDA(cudaMemcpyAsync(k->hJ + (size_t)meq * n, Jd_host, sizeof(double) * (size_t)mi * n, cudaMemcpyHostToDevice, c->stream));
@@ -966,13 +944,11 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   // update + solveCompressed does; breakdowns are reported after the solve.
   if(chunked) {
     constexpr int NCH = 16;
-    if(!k->copy_stream) {
-      HB_CUDA(cudaStreamCreateWithFlags(&k->copy_stream, cudaStreamNonBlocking));
-      for(int q = 0; q < 32; q++) HB_CUDA(cudaEventCreateWithFlags(&k->chunk_ev[q], cudaEventDisableTiming));
-      HB_CUDA(cudaMalloc(&k->chunk_rowptr_dev, sizeof(double*) * 32 * (size_t)(k->m + 2 * k->lmax)));
-      HB_CUDA(cudaMallocHost(&k->chunk_rowptr_host, sizeof(double*) * 32 * (size_t)(k->m + 2 * k->lmax)));
-    }
-    if(!k->Ctmp) HB_CHECK(dmalloc(&k->Ctmp, (size_t)(k->m + 2 * k->lmax) * (k->m + 2 * k->lmax)));
+    HB_CHECK(k->copy_stream.create(cudaStreamNonBlocking));
+    for(hb_event& e : k->chunk_ev) HB_CHECK(e.create(cudaEventDisableTiming));
+    HB_CHECK(k->chunk_rowptr_dev.reserve(c, 32 * (size_t)(k->m + 2 * k->lmax), "chunk row pointers"));
+    HB_CHECK(k->chunk_rowptr_host.reserve(c, 32 * (size_t)(k->m + 2 * k->lmax), "chunk row pointers"));
+    HB_CHECK(k->Ctmp.reserve(c, (size_t)(k->m + 2 * k->lmax) * (k->m + 2 * k->lmax), "partial C_aug"));
     HB_CHECK(refresh_rowptr(k)); // k->rowptr_host: full-length rows of [J; S; Y]
     long long csz = ((n + NCH - 1) / NCH + 63) & ~63LL;
     int nch = (int)((n + csz - 1) / csz);

@@ -50,10 +50,7 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   const int m = k->m, me = k->meq, mi = k->mineq;
   const long long n = k->n;
   if(m == 0) return HB_OK;
-  if(!k->lsq_M && cudaMalloc(&k->lsq_M, sizeof(double) * ((size_t)m * m + 2 * m)) != cudaSuccess) {
-    cudaGetLastError();
-    return hb_fail(HB_ERR_ALLOC, "LSQ workspace allocation failed%s", "");
-  }
+  HB_CHECK(k->lsq_M.reserve(c, (size_t)m * m + 2 * m, "the LSQ workspace"));
   double* M = k->lsq_M;
   double* rhs = M + (size_t)m * m;
   HB_CHECK(hb_lr_refresh_rowptr(k));

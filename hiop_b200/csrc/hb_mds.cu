@@ -12,12 +12,12 @@ struct hb_mds
   hb_ctx* ctx = nullptr;
   int nxs = 0, nxd = 0, neq = 0, nineq = 0, nnz_c = 0, nnz_d = 0;
   // stacked sparse Jacobian Js = [Jcs; Jds] ((neq+nineq) x nxs): CSR (values in triplet order) + CSC (gather map)
-  int *csr_ptr = nullptr, *csr_col = nullptr;
-  int *csc_ptr = nullptr, *csc_row = nullptr, *csc_src = nullptr;
-  double* vals = nullptr; // nnz_c + nnz_d
-  double *Dx = nullptr, *Hxs = nullptr, *Dd_inv = nullptr, *rhs = nullptr, *rxs = nullptr;
-  int* counts = nullptr;      // device: [neg, zero]
-  int* counts_host = nullptr; // pinned
+  hb_dev<int> csr_ptr, csr_col;
+  hb_dev<int> csc_ptr, csc_row, csc_src;
+  hb_dev<double> vals; // nnz_c + nnz_d
+  hb_dev<double> Dx, Hxs, Dd_inv, rhs, rxs;
+  hb_dev<int> counts;          // device: [neg, zero]
+  hb_pinned<int> counts_host;
   bool have_structure = false, have_update = false, built = false;
 };
 
@@ -162,16 +162,6 @@ __global__ void k_mds_unpack(int nxs, int nxd, int neq, int nineq, const double*
   }
 }
 
-template <class X>
-int dalloc(X** p, size_t count)
-{
-  if(cudaMalloc(p, sizeof(X) * (count ? count : 1)) != cudaSuccess) {
-    cudaGetLastError();
-    return hb_fail(HB_ERR_ALLOC, "hb_mds: device allocation failed%s", "");
-  }
-  return HB_OK;
-}
-
 inline int grid1(hb_ctx* c, long long items)
 {
   long long g = (items + T - 1) / T, cap = (long long)c->num_sms * 8;
@@ -184,16 +174,16 @@ extern "C" int hb_mds_create(hb_ctx* c, int nxs, int nxd, int neq, int nineq, hb
 {
   HB_REQUIRE(c && out && nxs >= 0 && nxd >= 0 && neq >= 0 && nineq >= 0, "hb_mds_create: bad arguments");
   HB_CUDA(cudaSetDevice(c->device));
-  hb_mds* h = new hb_mds;
+  std::unique_ptr<hb_mds> h(new hb_mds);
   h->ctx = c; h->nxs = nxs; h->nxd = nxd; h->neq = neq; h->nineq = nineq;
-  HB_CHECK(dalloc(&h->Dx, (size_t)nxs + nxd));
-  HB_CHECK(dalloc(&h->Hxs, nxs));
-  HB_CHECK(dalloc(&h->rxs, nxs));
-  HB_CHECK(dalloc(&h->Dd_inv, nineq));
-  HB_CHECK(dalloc(&h->rhs, (size_t)nxd + neq + nineq));
-  HB_CHECK(dalloc(&h->counts, 2));
-  HB_CUDA(cudaMallocHost(&h->counts_host, sizeof(int) * 2));
-  *out = h;
+  HB_CHECK(h->Dx.reserve(c, (size_t)nxs + nxd, "hb_mds Dx"));
+  HB_CHECK(h->Hxs.reserve(c, nxs, "hb_mds Hxs"));
+  HB_CHECK(h->rxs.reserve(c, nxs, "hb_mds rxs"));
+  HB_CHECK(h->Dd_inv.reserve(c, nineq, "hb_mds Dd_inv"));
+  HB_CHECK(h->rhs.reserve(c, (size_t)nxd + neq + nineq, "hb_mds rhs"));
+  HB_CHECK(h->counts.reserve(c, 2, "hb_mds inertia counts"));
+  HB_CHECK(h->counts_host.reserve(c, 2, "hb_mds inertia counts"));
+  *out = h.release();
   return HB_OK;
 }
 
@@ -202,9 +192,6 @@ extern "C" int hb_mds_destroy(hb_mds* h)
   if(!h) return HB_OK;
   cudaSetDevice(h->ctx->device);
   cudaStreamSynchronize(h->ctx->stream);
-  cudaFree(h->csr_ptr); cudaFree(h->csr_col); cudaFree(h->csc_ptr); cudaFree(h->csc_row); cudaFree(h->csc_src); cudaFree(h->vals);
-  cudaFree(h->Dx); cudaFree(h->Hxs); cudaFree(h->rxs); cudaFree(h->Dd_inv); cudaFree(h->rhs); cudaFree(h->counts);
-  cudaFreeHost(h->counts_host);
   delete h;
   return HB_OK;
 }
@@ -238,12 +225,11 @@ extern "C" int hb_mds_set_sparsity(hb_mds* h, int nnz_c, const int* iRow_c, cons
     crow[p] = row[k];
     csrc[p] = k;
   }
-  HB_CUDA(cudaStreamSynchronize(c->stream));
-  cudaFree(h->csr_ptr); cudaFree(h->csr_col); cudaFree(h->csc_ptr); cudaFree(h->csc_row); cudaFree(h->csc_src); cudaFree(h->vals);
-  h->csr_ptr = h->csr_col = h->csc_ptr = h->csc_row = h->csc_src = nullptr; h->vals = nullptr;
-  HB_CHECK(dalloc(&h->csr_ptr, m + 1)); HB_CHECK(dalloc(&h->csr_col, nnz));
-  HB_CHECK(dalloc(&h->csc_ptr, h->nxs + 1)); HB_CHECK(dalloc(&h->csc_row, nnz)); HB_CHECK(dalloc(&h->csc_src, nnz));
-  HB_CHECK(dalloc(&h->vals, nnz));
+  h->have_structure = false;
+  HB_CHECK(h->csr_ptr.reserve(c, (size_t)m + 1, "hb_mds CSR pointers")); HB_CHECK(h->csr_col.reserve(c, nnz, "hb_mds CSR columns"));
+  HB_CHECK(h->csc_ptr.reserve(c, (size_t)h->nxs + 1, "hb_mds CSC pointers")); HB_CHECK(h->csc_row.reserve(c, nnz, "hb_mds CSC rows"));
+  HB_CHECK(h->csc_src.reserve(c, nnz, "hb_mds CSC gather map")); HB_CHECK(h->vals.reserve(c, nnz, "hb_mds Jacobian values"));
+  HB_CUDA(cudaStreamSynchronize(c->stream)); // the synchronous uploads below must not overwrite arrays a queued kernel still reads
   HB_CUDA(cudaMemcpy(h->csr_ptr, ptr.data(), sizeof(int) * (m + 1), cudaMemcpyHostToDevice));
   HB_CUDA(cudaMemcpy(h->csc_ptr, cptr.data(), sizeof(int) * (h->nxs + 1), cudaMemcpyHostToDevice));
   if(nnz) {
@@ -316,9 +302,9 @@ extern "C" int hb_mds_hxs_inertia(hb_mds* h, int* n_neg, int* n_zero)
   return HB_OK;
 }
 
-extern "C" const double* hb_mds_Dx(hb_mds* h) { return h ? h->Dx : nullptr; }
-extern "C" const double* hb_mds_Hxs(hb_mds* h) { return h ? h->Hxs : nullptr; }
-extern "C" const double* hb_mds_Dd_inv(hb_mds* h) { return h ? h->Dd_inv : nullptr; }
+extern "C" const double* hb_mds_Dx(hb_mds* h) { return h ? h->Dx.get() : nullptr; }
+extern "C" const double* hb_mds_Hxs(hb_mds* h) { return h ? h->Hxs.get() : nullptr; }
+extern "C" const double* hb_mds_Dd_inv(hb_mds* h) { return h ? h->Dd_inv.get() : nullptr; }
 
 extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc,
                                        double* dyd)

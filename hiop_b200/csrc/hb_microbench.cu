@@ -72,9 +72,9 @@ extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
 {
   HB_REQUIRE(c && result_host && (which == 0 || which == 1), "hb_microbench_peak: bad arguments");
   HB_CUDA(cudaSetDevice(c->device));
-  cudaEvent_t e0, e1;
-  HB_CUDA(cudaEventCreate(&e0));
-  HB_CUDA(cudaEventCreate(&e1));
+  hb_event e0, e1;
+  HB_CHECK(e0.create(cudaEventDefault));
+  HB_CHECK(e1.create(cudaEventDefault));
   float ms = 0.f;
   double best = 0.0;
   if(which == 0) {
@@ -96,11 +96,11 @@ extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
     const int blocks = c->num_sms, iters = 20000;
     const int smem = PEAK_I8_SMEM;
     HB_CHECK(hb_ws_reserve(c, sizeof(int) * (size_t)blocks));
-    k_peak_i8<<<blocks, 256, smem, c->stream>>>(200, (int*)c->ws);
+    k_peak_i8<<<blocks, 256, smem, c->stream>>>(200, (int*)c->ws.get());
     HB_LAUNCHED();
     for(int rep = 0; rep < 3; rep++) {
       HB_CUDA(cudaEventRecord(e0, c->stream));
-      k_peak_i8<<<blocks, 256, smem, c->stream>>>(iters, (int*)c->ws);
+      k_peak_i8<<<blocks, 256, smem, c->stream>>>(iters, (int*)c->ws.get());
       HB_LAUNCHED();
       HB_CUDA(cudaEventRecord(e1, c->stream));
       HB_CUDA(cudaEventSynchronize(e1));
@@ -109,8 +109,6 @@ extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
       if(tops > best) best = tops;
     }
   }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   *result_host = best;
   return HB_OK;
 }

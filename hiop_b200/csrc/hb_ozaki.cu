@@ -427,41 +427,27 @@ k_oz_fixup(int M, int n_tiles, const int2* __restrict__ tile_ij, int splits, con
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+} // namespace
+
+// one state per CONTEXT (it used to be per device: two contexts on one GPU would have shared the slice buffer across their streams)
 struct OzState
 {
-  int M = -1, S = 0, splits = 0, n_tiles = 0, n_items = 0;
+  int M = -1, S = 0, splits = 0, n_tiles = 0, n_items = 0; // (M, K, S): the shape the work list and tensor maps were built for
   long long K = -1, Kpad = 0;
   int Mpad = 0;
-  int8_t* Q = nullptr;
-  size_t Qbytes = 0;
-  double* sd = nullptr;
-  long long sd_n = 0;
-  unsigned long long* mx = nullptr;
-  int* e = nullptr;
-  int mcap = 0;
-  double* dot_partial = nullptr; // [chunks][M] partial row dots of the fused row-maximum pass
-  size_t dot_cap = 0;
-  OzItem* d_items = nullptr;
-  int2* d_tiles = nullptr;
+  hb_dev<int8_t> Q;
+  hb_dev<double> sd;
+  hb_dev<unsigned long long> mx;
+  hb_dev<int> e;
+  hb_dev<double> dot_partial; // [chunks][M] partial row dots of the fused row-maximum pass
+  hb_dev<OzItem> d_items;
+  hb_dev<int2> d_tiles;
   CUtensorMap mapA, mapB;
   PFN_encodeTiled encode = nullptr; // cuTensorMapEncodeTiled, resolved on first use
 };
-// one state per CONTEXT (it used to be per device: two contexts on one GPU would have shared the slice buffer across their streams)
-void oz_state_free(void* p)
-{
-  OzState* st = static_cast<OzState*>(p);
-  if(!st) return;
-  cudaFree(st->Q); cudaFree(st->sd); cudaFree(st->mx); cudaFree(st->e); cudaFree(st->d_items); cudaFree(st->d_tiles); cudaFree(st->dot_partial);
-  delete st;
-}
-OzState& oz_state(hb_ctx* c)
-{
-  if(!c->oz_state) {
-    c->oz_state = new OzState;
-    c->oz_free = oz_state_free;
-  }
-  return *static_cast<OzState*>(c->oz_state);
-}
+void hb_delete(OzState* p) { delete p; }
+
+namespace {
 
 template <int S>
 int launch_gemm(hb_ctx* c, OzState& st, int chunk_blocks, double* partial)
@@ -494,7 +480,8 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
     return HB_OK;
   }
-  OzState& st = oz_state(c);
+  if(!c->oz) c->oz.reset(new OzState);
+  OzState& st = *c->oz;
   if(!st.encode) {
     cudaDriverEntryPointQueryResult qres;
     HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&st.encode, cudaEnableDefault, &qres));
@@ -503,29 +490,16 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
   const int Mpad = ((M + TM - 1) / TM) * TM;
   const long long Kpad = ((K + KS - 1) / KS) * KS;
   const size_t qbytes = (size_t)S * Mpad * Kpad;
-  if(st.Qbytes < qbytes) {
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    cudaFree(st.Q);
-    st.Q = nullptr; st.Qbytes = 0;
-    if(cudaMalloc(&st.Q, qbytes) != cudaSuccess) { cudaGetLastError(); return hb_fail(HB_ERR_ALLOC, "hb_syrk_rows_ozaki: cannot allocate the int8 slice buffer%s", ""); }
-    st.Qbytes = qbytes;
-    st.M = -1;
+  if(!st.Q || st.Q.capacity() < qbytes) {
+    st.M = -1; // the tensor maps hold the address of Q
+    HB_CHECK(st.Q.reserve(c, qbytes, "the int8 slice buffer"));
   }
-  if(st.sd_n < K) {
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    cudaFree(st.sd);
-    HB_CUDA(cudaMalloc(&st.sd, sizeof(double) * K));
-    st.sd_n = K;
-  }
-  if(st.mcap < Mpad) {
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    cudaFree(st.mx); cudaFree(st.e);
-    HB_CUDA(cudaMalloc(&st.mx, sizeof(unsigned long long) * Mpad));
-    HB_CUDA(cudaMalloc(&st.e, sizeof(int) * Mpad));
-    st.mcap = Mpad;
-  }
+  HB_CHECK(st.sd.reserve(c, K, "sqrt(d)"));
+  HB_CHECK(st.mx.reserve(c, Mpad, "row maxima"));
+  HB_CHECK(st.e.reserve(c, Mpad, "row exponents"));
   if(st.M != M || st.K != K || st.S != S) {
     // schedule: tiles (bi, bj) with bj >= (TM / TN) bi cover the upper triangle; split K so that ~all SMs get one item
+    st.M = -1;
     HB_CUDA(cudaStreamSynchronize(c->stream));
     const int nbi = Mpad / TM, nbj = Mpad / TN;
     std::vector<int2> tiles;
@@ -569,9 +543,8 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
         it.slot = t * splits + s;
         items.push_back(it);
       }
-    cudaFree(st.d_items); cudaFree(st.d_tiles);
-    HB_CUDA(cudaMalloc(&st.d_items, sizeof(OzItem) * items.size()));
-    HB_CUDA(cudaMalloc(&st.d_tiles, sizeof(int2) * nt));
+    HB_CHECK(st.d_items.reserve(c, items.size(), "the int8-slice work list"));
+    HB_CHECK(st.d_tiles.reserve(c, nt, "the int8-slice tile list"));
     HB_CUDA(cudaMemcpy(st.d_items, items.data(), sizeof(OzItem) * items.size(), cudaMemcpyHostToDevice));
     HB_CUDA(cudaMemcpy(st.d_tiles, tiles.data(), sizeof(int2) * nt, cudaMemcpyHostToDevice));
     cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Mpad, (cuuint64_t)S};
@@ -595,12 +568,7 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
   {
     if(dot_x && dot_out && K > 0) {
       const int nchunks = (int)((K + RD_COLS - 1) / RD_COLS);
-      if(st.dot_cap < (size_t)nchunks * M) {
-        HB_CUDA(cudaStreamSynchronize(c->stream));
-        cudaFree(st.dot_partial);
-        HB_CUDA(cudaMalloc(&st.dot_partial, sizeof(double) * (size_t)nchunks * M));
-        st.dot_cap = (size_t)nchunks * M;
-      }
+      HB_CHECK(st.dot_partial.reserve(c, (size_t)nchunks * M, "fused row-dot partials"));
       int rsplit = (2 * c->num_sms + nchunks - 1) / nchunks; // short shards: split the rows of a chunk over several CTAs
       rsplit = rsplit < 1 ? 1 : (rsplit > 8 ? 8 : rsplit);
       // pairs of columns need 16-byte aligned rows AND an even first column per lane (RD_COLS is even)

@@ -89,16 +89,6 @@ inline int egrid(hb_ctx* c, long long items)
   return (int)(g < 1 ? 1 : g);
 }
 
-int dalloc(double** p, size_t count)
-{
-  if(*p) return HB_OK;
-  if(cudaMalloc(p, sizeof(double) * (count ? count : 1)) != cudaSuccess) {
-    cudaGetLastError();
-    return hb_fail(HB_ERR_ALLOC, "secant memory allocation failed%s", "");
-  }
-  return HB_OK;
-}
-
 int install(hb_lowrank* k)
 {
   const int l = k->sec_lcurr > 0 ? k->sec_lcurr : 0;
@@ -117,10 +107,11 @@ extern "C" int hb_lowrank_secant_reset(hb_lowrank* k, double sigma0, int sigma_s
   k->sec_strategy = sigma_strategy;
   k->sec_sigma0 = sigma0;
   k->sigma = sigma0;
-  HB_CHECK(dalloc(&k->sec_S, (size_t)k->lmax * k->n));
-  HB_CHECK(dalloc(&k->sec_Y, (size_t)k->lmax * k->n));
-  HB_CHECK(dalloc(&k->sec_xprev, (size_t)k->n));
-  HB_CHECK(dalloc(&k->sec_gprev, (size_t)k->n));
+  hb_ctx* c = k->ctx;
+  HB_CHECK(k->sec_S.reserve(c, (size_t)k->lmax * k->n, "secant memory S"));
+  HB_CHECK(k->sec_Y.reserve(c, (size_t)k->lmax * k->n, "secant memory Y"));
+  HB_CHECK(k->sec_xprev.reserve(c, (size_t)k->n, "previous iterate"));
+  HB_CHECK(k->sec_gprev.reserve(c, (size_t)k->n, "previous gradient"));
   return hb_lowrank_set_secant(k, 0, sigma0, k->sec_S, k->sec_Y, k->sec_L, k->sec_D);
 }
 
@@ -136,7 +127,7 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
   const int m = k->m, lmax = k->lmax;
   const bool needJ = m > 0 && !jacobian_is_constant;
   int st = 0;
-  if(needJ) HB_CHECK(dalloc(&k->sec_Jprev, (size_t)m * n));
+  if(needJ) HB_CHECK(k->sec_Jprev.reserve(c, (size_t)m * n, "previous Jacobian"));
   if(k->sec_lcurr < 0) {
     // first optimization iterate: only remember it                                     hiopHessianLowRank.cpp:372-381
     k->sec_lcurr = 0;

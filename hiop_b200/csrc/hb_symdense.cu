@@ -131,24 +131,23 @@ struct hb_symdense
 {
   hb_ctx* ctx = nullptr;
   int N = 0;
-  double* M = nullptr;      // N x N row-major, upper triangle valid on entry, factor in place
-  double* W = nullptr;      // panel scratch (lazy)
-  double* xbuf = nullptr;   // staging for the *_host variants (lazy)
-  size_t xbuf_cap = 0;      // doubles allocated in xbuf (per handle)
-  double* Fpad = nullptr;   // odd N: copy of M with an even leading dimension (the large-N kernels use 16-byte accesses)
+  hb_dev<double> M;         // N x N row-major, upper triangle valid on entry, factor in place
+  hb_dev<double> W;         // panel scratch (lazy)
+  hb_dev<double> xbuf;      // staging for the *_host variants (lazy)
+  hb_dev<double> Fpad;      // odd N: copy of M with an even leading dimension (the large-N kernels use 16-byte accesses)
   double* F = nullptr;      // where the current factor lives (M or Fpad)
   long long ldf = 0;
   hb_big big;               // large-N path: streams, diagonal-block inverses, solve scratch
   Plan plan{};              // the paths of the current factor
   // cluster Bunch-Kaufman (hb_bk_cluster.cu): permuted factor P A P^T = L D L^T
-  double* dsub = nullptr;   // sub-diagonal of the 2x2 blocks of D
-  int* perm = nullptr;      // gather order of the right-hand side
-  int* bk_state = nullptr;  // device: k0, kb, info, -
-  int* swaplog = nullptr;
-  double* Wp = nullptr;     // W = L*D of the current panel
-  int* ipiv = nullptr;
-  int* info = nullptr;      // device: [0] info, [1..3] inertia
-  int* info_host = nullptr; // pinned
+  hb_dev<double> dsub;      // sub-diagonal of the 2x2 blocks of D
+  hb_dev<int> perm;         // gather order of the right-hand side
+  hb_dev<int> bk_state;     // device: k0, kb, info, -
+  hb_dev<int> swaplog;
+  hb_dev<double> Wp;        // W = L*D of the current panel
+  hb_dev<int> ipiv;
+  hb_dev<int> info;         // device: [0] info, [1..3] inertia
+  hb_pinned<int> info_host;
   int mode = -1;
   bool factored = false;
   int n_neg = 0, n_null = 0, n_pos = 0;
@@ -158,19 +157,15 @@ extern "C" int hb_symdense_create(hb_ctx* c, int N, hb_symdense** out)
 {
   HB_REQUIRE(c && out && N >= 0, "hb_symdense_create: bad arguments");
   HB_CUDA(cudaSetDevice(c->device));
-  hb_symdense* s = new hb_symdense;
+  std::unique_ptr<hb_symdense> s(new hb_symdense);
   s->ctx = c;
   s->N = N;
-  if(cudaMalloc(&s->M, sizeof(double) * (size_t)(N ? N : 1) * (N ? N : 1)) != cudaSuccess) {
-    cudaGetLastError();
-    delete s;
-    return hb_fail(HB_ERR_ALLOC, "hb_symdense_create: cannot allocate the %s system matrix", "N x N");
-  }
-  HB_CUDA(cudaMalloc(&s->ipiv, sizeof(int) * (N + 1)));
-  HB_CUDA(cudaMalloc(&s->info, sizeof(int) * 4));
-  HB_CUDA(cudaMallocHost(&s->info_host, sizeof(int) * 4));
-  HB_CUDA(cudaMemsetAsync(s->M, 0, sizeof(double) * (size_t)(N ? N : 1) * (N ? N : 1), c->stream));
-  *out = s;
+  HB_CHECK(s->M.reserve(c, (size_t)N * N, "the N x N system matrix"));
+  HB_CHECK(s->ipiv.reserve(c, (size_t)N + 1, "pivots"));
+  HB_CHECK(s->info.reserve(c, 4, "info words"));
+  HB_CHECK(s->info_host.reserve(c, 4, "info words"));
+  HB_CUDA(cudaMemsetAsync(s->M, 0, sizeof(double) * s->M.capacity(), c->stream));
+  *out = s.release();
   return HB_OK;
 }
 
@@ -179,15 +174,11 @@ extern "C" int hb_symdense_destroy(hb_symdense* s)
   if(!s) return HB_OK;
   cudaSetDevice(s->ctx->device);
   cudaStreamSynchronize(s->ctx->stream);
-  hb_big_release(&s->big);
-  cudaFree(s->dsub); cudaFree(s->perm); cudaFree(s->bk_state); cudaFree(s->swaplog); cudaFree(s->Wp);
-  cudaFree(s->M); cudaFree(s->W); cudaFree(s->xbuf); cudaFree(s->ipiv); cudaFree(s->info); cudaFree(s->Fpad);
-  cudaFreeHost(s->info_host);
   delete s;
   return HB_OK;
 }
 
-extern "C" double* hb_symdense_matrix(hb_symdense* s) { return s ? s->M : nullptr; }
+extern "C" double* hb_symdense_matrix(hb_symdense* s) { return s ? s->M.get() : nullptr; }
 
 extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
 {
@@ -206,27 +197,21 @@ extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
   if((big || p.f == F_BK_CLUSTER) && (N & 1)) { // even leading dimension for the 16-byte operand copies
     const long long ld = (N + 7) & ~7LL;
     if(!s->Fpad) {
-      if(cudaMalloc(&s->Fpad, sizeof(double) * (size_t)ld * N) != cudaSuccess) { cudaGetLastError(); return hb_fail(HB_ERR_ALLOC, "hb_symdense_matrix_changed: cannot allocate the padded factor%s", ""); }
+      HB_CHECK(s->Fpad.reserve(c, (size_t)ld * N, "the padded factor"));
       HB_CUDA(cudaMemsetAsync(s->Fpad, 0, sizeof(double) * (size_t)ld * N, c->stream));
     }
     HB_CUDA(cudaMemcpy2DAsync(s->Fpad, sizeof(double) * ld, s->M, sizeof(double) * N, sizeof(double) * N, N, cudaMemcpyDeviceToDevice, c->stream));
     s->F = s->Fpad; s->ldf = ld;
   }
   const long long ldw = (N + 7) & ~7LL;
-  if(p.f == F_BK_CLUSTER && !s->dsub) {
-    if(cudaMalloc(&s->dsub, sizeof(double) * (N + 2)) != cudaSuccess || cudaMalloc(&s->perm, sizeof(int) * (N + 2)) != cudaSuccess ||
-       cudaMalloc(&s->bk_state, sizeof(int) * 4) != cudaSuccess || cudaMalloc(&s->swaplog, sizeof(int) * HB_BKC_SWAPLOG_INTS(N)) != cudaSuccess ||
-       cudaMalloc(&s->Wp, sizeof(double) * HB_BKC_W_DOUBLES(ldw)) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "hb_symdense_matrix_changed: cannot allocate the Bunch-Kaufman scratch%s", "");
-    }
+  if(p.f == F_BK_CLUSTER) {
+    HB_CHECK(s->dsub.reserve(c, (size_t)N + 2, "Bunch-Kaufman sub-diagonal"));
+    HB_CHECK(s->perm.reserve(c, (size_t)N + 2, "Bunch-Kaufman permutation"));
+    HB_CHECK(s->bk_state.reserve(c, 4, "Bunch-Kaufman state"));
+    HB_CHECK(s->swaplog.reserve(c, HB_BKC_SWAPLOG_INTS(N), "Bunch-Kaufman swap log"));
+    HB_CHECK(s->Wp.reserve(c, HB_BKC_W_DOUBLES(ldw), "Bunch-Kaufman panel scratch"));
   }
-  if((p.f == F_PANEL_LDL || p.f == F_SYTRF_BLOCKED) && !s->W) {
-    if(cudaMalloc(&s->W, sizeof(double) * (size_t)2 * 64 * N) != cudaSuccess) {
-      cudaGetLastError();
-      return hb_fail(HB_ERR_ALLOC, "hb_symdense_matrix_changed: cannot allocate panel scratch%s", "");
-    }
-  }
+  if(p.f == F_PANEL_LDL || p.f == F_SYTRF_BLOCKED) HB_CHECK(s->W.reserve(c, (size_t)2 * 64 * N, "panel scratch"));
   switch(p.f) {
   case F_SYTF2: HB_CHECK(hb_dense_sytf2(c, N, s->M, N, s->ipiv, s->info)); break;
   case F_SYTRF_BLOCKED: HB_CHECK(hb_dense_sytrf_blocked(c, N, s->M, N, s->ipiv, s->W, s->info)); break;
@@ -276,7 +261,7 @@ extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
     const bool bkc = s->plan.f == F_BK_CLUSTER;
     const int dmode = bkc ? 2 : (s->mode == HB_FACT_CHOLESKY ? 0 : 1);
     for(int r = 0; r < nrhs; r++)
-      HB_CHECK(hb_big_solve(c, &s->big, s->N, s->F, s->ldf, dmode, s->ipiv, s->dsub, bkc ? s->perm : nullptr, x + (size_t)r * s->N));
+      HB_CHECK(hb_big_solve(c, &s->big, s->N, s->F, s->ldf, dmode, s->ipiv, s->dsub, bkc ? s->perm.get() : nullptr, x + (size_t)r * s->N));
     break;
   }
   case S_SYTRS: HB_CHECK(bk_sytrs(c, s->N, s->M, s->N, s->ipiv, x, s->N, nrhs)); break;
@@ -301,11 +286,7 @@ extern "C" int hb_symdense_solve_host(hb_symdense* s, double* x_host, int nrhs)
   HB_REQUIRE(x_host, "hb_symdense_solve_host: null rhs");
   hb_ctx* c = s->ctx;
   const size_t need = (size_t)s->N * nrhs;
-  if(!s->xbuf || s->xbuf_cap < need) {
-    if(s->xbuf) { HB_CUDA(cudaStreamSynchronize(c->stream)); cudaFree(s->xbuf); s->xbuf = nullptr; }
-    if(cudaMalloc(&s->xbuf, sizeof(double) * need) != cudaSuccess) { cudaGetLastError(); return hb_fail(HB_ERR_ALLOC, "rhs staging allocation failed%s", ""); }
-    s->xbuf_cap = need;
-  }
+  HB_CHECK(s->xbuf.reserve(c, need, "rhs staging"));
   HB_CUDA(cudaMemcpyAsync(s->xbuf, x_host, sizeof(double) * need, cudaMemcpyHostToDevice, c->stream));
   int rc = hb_symdense_solve(s, s->xbuf, nrhs);
   if(rc != 1) return rc;

@@ -396,39 +396,34 @@ k_syrk_fixup(int M, const int2* __restrict__ tile_ij, const int* __restrict__ ti
 
 struct Schedule
 {
-  int M = -1;
+  int M = -1;      // (M, K, bk, G): the key this way was built for, M = -1 while it holds none
   long long K = -1;
   int bk = 0;      // K-chunk (columns per iteration) the schedule counts in
   int G = 0;       // SM count the schedule was built for
   int Gl = 0;      // CTAs to launch
   long long stamp = 0;
   int ntiles = 0, nslots = 0;
-  int *d_cta_seg_begin = nullptr, *d_tile_slot_begin = nullptr, *d_tile_slots = nullptr;
-  int2* d_tile_ij = nullptr;
-  Seg* d_segs = nullptr;
+  hb_dev<int> d_cta_seg_begin, d_tile_slot_begin, d_tile_slots;
+  hb_dev<int2> d_tile_ij;
+  hb_dev<Seg> d_segs;
 };
 constexpr int SCHED_WAYS = 4;
+
+} // namespace
+
 struct ScheduleCache // per context (c->syrk_sched), small LRU cache keyed by (M, K)
 {
   Schedule ways[SCHED_WAYS];
   long long clock = 0;
 };
-void schedule_cache_free(void* p)
-{
-  ScheduleCache* sc = static_cast<ScheduleCache*>(p);
-  for(Schedule& S : sc->ways) {
-    cudaFree(S.d_cta_seg_begin); cudaFree(S.d_tile_slot_begin); cudaFree(S.d_tile_slots); cudaFree(S.d_tile_ij); cudaFree(S.d_segs);
-  }
-  delete sc;
-}
+void hb_delete(ScheduleCache* p) { delete p; }
+
+namespace {
 
 int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
 {
-  if(!c->syrk_sched) {
-    c->syrk_sched = new ScheduleCache;
-    c->syrk_free = schedule_cache_free;
-  }
-  ScheduleCache& sc = *static_cast<ScheduleCache*>(c->syrk_sched);
+  if(!c->syrk_sched) c->syrk_sched.reset(new ScheduleCache);
+  ScheduleCache& sc = *c->syrk_sched;
   Schedule* ways = sc.ways;
   int victim = 0;
   for(int w = 0; w < SCHED_WAYS; w++) {
@@ -442,8 +437,8 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   Schedule& S = ways[victim];
   Sout = &S;
   S.stamp = ++sc.clock;
+  S.M = -1;
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  cudaFree(S.d_cta_seg_begin); cudaFree(S.d_tile_slot_begin); cudaFree(S.d_tile_slots); cudaFree(S.d_tile_ij); cudaFree(S.d_segs);
   const int T = (M + BM - 1) / BM;
   const int ntiles = T * (T + 1) / 2;
   const long long kiters = (K + bk - 1) / bk;
@@ -508,11 +503,11 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   tsb[ntiles] = (int)tsl.size();
   if(tsl.empty()) tsl.push_back(0);
   if(segs.empty()) segs.push_back(Seg{0, 0, 0, 0, 0});
-  HB_CUDA(cudaMalloc(&S.d_cta_seg_begin, sizeof(int) * (G + 1)));
-  HB_CUDA(cudaMalloc(&S.d_tile_slot_begin, sizeof(int) * (ntiles + 1)));
-  HB_CUDA(cudaMalloc(&S.d_tile_slots, sizeof(int) * tsl.size()));
-  HB_CUDA(cudaMalloc(&S.d_tile_ij, sizeof(int2) * ntiles));
-  HB_CUDA(cudaMalloc(&S.d_segs, sizeof(Seg) * segs.size()));
+  HB_CHECK(S.d_cta_seg_begin.reserve(c, (size_t)G + 1, "SYRK schedule"));
+  HB_CHECK(S.d_tile_slot_begin.reserve(c, (size_t)ntiles + 1, "SYRK schedule"));
+  HB_CHECK(S.d_tile_slots.reserve(c, tsl.size(), "SYRK schedule"));
+  HB_CHECK(S.d_tile_ij.reserve(c, ntiles, "SYRK schedule"));
+  HB_CHECK(S.d_segs.reserve(c, segs.size(), "SYRK schedule"));
   HB_CUDA(cudaMemcpy(S.d_cta_seg_begin, cta_begin.data(), sizeof(int) * (G + 1), cudaMemcpyHostToDevice));
   HB_CUDA(cudaMemcpy(S.d_tile_slot_begin, tsb.data(), sizeof(int) * (ntiles + 1), cudaMemcpyHostToDevice));
   HB_CUDA(cudaMemcpy(S.d_tile_slots, tsl.data(), sizeof(int) * tsl.size(), cudaMemcpyHostToDevice));

@@ -46,6 +46,10 @@ const char* hb_version(void);
 const char* hb_last_error(void);
 /* number of kernel launches issued by this library since load (all contexts); feeds bench.py's gpu_launches */
 long long hb_launch_count(void);
+/* diagnostics: device buffers, pinned buffers, streams and events held by the library's contexts and handles right now (all contexts;
+ * memory from hb_malloc / hb_malloc_host belongs to the caller and is not counted). Back to its earlier value once everything created
+ * since then is destroyed. */
+long long hb_debug_live_resources(void);
 
 /* Replaces the ExecSpace/MemBackend plumbing (src/ExecBackends/) for this path: one device, one stream. */
 int hb_ctx_create(int device, hb_ctx** out);
