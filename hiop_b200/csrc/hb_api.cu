@@ -330,7 +330,7 @@ extern "C" int hb_allreduce_sum(hb_ctx* c, double* buf, long long count)
   return HB_OK;
 }
 
-int hb_allreduce_op(hb_ctx* c, double* buf, long long count, int op /*0 sum,2 max,3 min*/)
+int hb_allreduce_op(hb_ctx* c, double* buf, long long count, hb_op op)
 {
   if(c->nranks == 1 || count == 0) return HB_OK;
   if(!c->nccl_comm) return hb_fail(HB_ERR_COMM, "communicator not initialised%s", "");

@@ -2,9 +2,11 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <atomic>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <string>
 #include <utility>
@@ -188,6 +190,32 @@ static constexpr int HB_RED_SLOTS = 4096;
 // c->ws holds at least `bytes` afterwards
 int hb_ws_reserve(hb_ctx* ctx, size_t bytes);
 
+// grid of a grid-stride streaming kernel: one thread per item, at most 8 CTAs per SM, at least one CTA
+inline int hb_grid(const hb_ctx* c, long long items, int threads = 256)
+{
+  const long long g = (items + threads - 1) / threads, cap = (long long)c->num_sms * 8;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// reduction operations; the values are NCCL's op codes (ncclSum, ncclMax, ncclMin)
+enum hb_op { HB_SUM = 0, HB_MAX = 2, HB_MIN = 3 };
+
+// in-place all-reduce of `count` doubles over the context's ranks, on the context stream (nothing to do on one rank)
+int hb_allreduce_op(hb_ctx* c, double* buf, long long count, hb_op op);
+
+// Second stage of the per-CTA reductions: out[q] = ops[q] over partial[b * slots + q], b < nblocks, slots = ops.size() <= 8. Fixed
+// order: warp q owns slot q, lane l combines b = l, l + 32, ... in turn, then the warp combines its lanes with an xor tree.
+int hb_reduce_slots(hb_ctx* c, int nblocks, const double* partial, double* out, std::initializer_list<hb_op> ops);
+// out = [a (na doubles); b (nb doubles)]
+int hb_stack(hb_ctx* c, int na, const double* a, int nb, const double* b, double* out);
+
+// C = A diag(d) A^T over the rows of a device row-pointer table: FP64 DMMA (hb_syrk.cu) and int8 slices (hb_ozaki.cu)
+int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
+                 const double* fuse_rx = nullptr, double* tdot = nullptr);
+bool hb_syrk_extra_row_is_free(int M);
+int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
+                       const double* dot_x, double* dot_out);
+
 // set once by hb_ctx_create: the dynamic-shared-memory / cluster attributes of each kernel file's kernels (function attributes are
 // per device) and the dense solvers' thresholds
 int hb_syrk_init_attrs(hb_ctx* c);
@@ -228,21 +256,40 @@ __device__ __forceinline__ double hb_warp_min(double v)
   return v;
 }
 
-// Block-wide sum in a FIXED order (warp shuffles then warp 0) -> deterministic for a fixed launch geometry.
-template <int THREADS>
-__device__ __forceinline__ double hb_block_sum(double v, double* sm /* >= THREADS/32 doubles */)
+template <hb_op OP>
+__device__ __forceinline__ double hb_identity()
 {
-  v = hb_warp_sum(v);
+  return OP == HB_SUM ? 0.0 : (OP == HB_MAX ? -INFINITY : INFINITY);
+}
+template <hb_op OP>
+__device__ __forceinline__ double hb_combine(double a, double b)
+{
+  return OP == HB_SUM ? a + b : (OP == HB_MAX ? fmax(a, b) : fmin(a, b));
+}
+template <hb_op OP>
+__device__ __forceinline__ double hb_warp_reduce(double v)
+{
+  return OP == HB_SUM ? hb_warp_sum(v) : (OP == HB_MAX ? hb_warp_max(v) : hb_warp_min(v));
+}
+
+// Block-wide reduction in a FIXED order (warp xor trees, then warp 0 runs one over the per-warp values) -> deterministic for a fixed
+// launch geometry. Starts with a barrier, so `sm` may be reused by consecutive calls.
+template <hb_op OP, int THREADS>
+__device__ __forceinline__ double hb_block_reduce(double v, double* sm /* >= THREADS/32 doubles */)
+{
+  v = hb_warp_reduce<OP>(v);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   __syncthreads();
   if(l == 0) sm[w] = v;
   __syncthreads();
-  double r = 0.0;
-  if(w == 0) {
-    r = (l < THREADS / 32) ? sm[l] : 0.0;
-    r = hb_warp_sum(r);
-  }
+  double r = hb_identity<OP>();
+  if(w == 0) r = hb_warp_reduce<OP>((l < THREADS / 32) ? sm[l] : hb_identity<OP>());
   return r; // valid on warp 0 (all lanes)
+}
+template <int THREADS>
+__device__ __forceinline__ double hb_block_sum(double v, double* sm)
+{
+  return hb_block_reduce<HB_SUM, THREADS>(v, sm);
 }
 
 // stream-K style even split of `total` items over `parts`

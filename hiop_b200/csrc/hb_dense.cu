@@ -1006,9 +1006,7 @@ int hb_dense_tri_solve(hb_ctx* c, int N, const double* F, int ldf, bool ldl, dou
 int hb_dense_equilibrate(hb_ctx* c, int N, const double* Nfull, int ldn, double* F, int ldf, double* s)
 {
   if(N == 0) return HB_OK;
-  long long total = (long long)N * N;
-  int g = (int)((total + 255) / 256 < (long long)c->num_sms * 8 ? (total + 255) / 256 : (long long)c->num_sms * 8);
-  k_equilibrate<<<g, 256, 0, c->stream>>>(Nfull, ldn, N, F, ldf, s);
+  k_equilibrate<<<hb_grid(c, (long long)N * N), 256, 0, c->stream>>>(Nfull, ldn, N, F, ldf, s);
   HB_LAUNCHED();
   return HB_OK;
 }

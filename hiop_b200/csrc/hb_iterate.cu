@@ -12,8 +12,6 @@
 #include "../../include/hiopb200.h"
 #include <cmath>
 
-int hb_allreduce_op(hb_ctx* c, double* buf, long long count, int op);
-
 namespace {
 
 constexpr int ET = 256;
@@ -22,19 +20,6 @@ enum { X, D, YC, YD, SXL, SXU, SDL, SDU, ZL, ZU, VL, VU };
 __device__ __forceinline__ double ftb(double x, double dx, double sel, double tau) // hiopVectorPar.cpp:1038-1061
 {
   return (dx >= 0 || sel == 0.0) ? 1.0 : fmin(1.0, -tau * x / dx);
-}
-template <int T>
-__device__ __forceinline__ double block_min(double v, double* sm)
-{
-#pragma unroll
-  for(int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = v;
-  if(threadIdx.x == 0)
-    for(int w = 0; w < T / 32; w++) r = fmin(r, sm[w]);
-  return r;
 }
 
 // partial[b] = {min over the block's slacks (primal step), min over its bound duals (dual step)}
@@ -51,19 +36,10 @@ k_ftb_block(long long n, double tau, const double* __restrict__ sl, const double
     ap = fmin(ap, fmin(ftb(sl[i], dsl[i], l, tau), ftb(su[i], dsu[i], u, tau)));
     ad = fmin(ad, fmin(ftb(zl[i], dzl[i], l, tau), ftb(zu[i], dzu[i], u, tau)));
   }
-  double v = block_min<ET>(ap, sm);
+  double v = hb_block_reduce<HB_MIN, ET>(ap, sm);
   if(threadIdx.x == 0) partial[2 * blockIdx.x] = v;
-  v = block_min<ET>(ad, sm);
+  v = hb_block_reduce<HB_MIN, ET>(ad, sm);
   if(threadIdx.x == 0) partial[2 * blockIdx.x + 1] = v;
-}
-__global__ void k_min2_final(int nb, const double* __restrict__ partial, double* __restrict__ out)
-{
-  const int q = threadIdx.x >> 5, lane = threadIdx.x & 31; // 2 warps
-  double v = 1.0;
-  for(int b = lane; b < nb; b += 32) v = fmin(v, partial[2 * b + q]);
-#pragma unroll
-  for(int o = 16; o > 0; o >>= 1) v = fmin(v, __shfl_xor_sync(0xffffffffu, v, o));
-  if(lane == 0) out[q] = v;
 }
 
 // log-barrier pieces of one primal block: partial[b] = {sum log(sl)|il + sum log(su)|iu, sum sl|(il & !iu) + sum su|(iu & !il)};
@@ -94,14 +70,6 @@ k_logbar_block(long long n, const double* __restrict__ sl, const double* __restr
   if(threadIdx.x == 0) partial[2 * blockIdx.x] = v;
   v = hb_block_sum<ET>(dt, sm);
   if(threadIdx.x == 0) partial[2 * blockIdx.x + 1] = v;
-}
-__global__ void k_sum2_final(int nb, const double* __restrict__ partial, double* __restrict__ out)
-{
-  const int q = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double v = 0.0;
-  for(int b = lane; b < nb; b += 32) v += partial[2 * b + q];
-  v = hb_warp_sum(v);
-  if(lane == 0) out[q] = v;
 }
 
 // out = a + alpha * d (copyFrom + axpy), for up to 6 blocks in one launch
@@ -180,14 +148,6 @@ k_adjust_small_slack(long long n, double mu, double small_val, double scale_fact
   if(local) atomicAdd(cnt, local);
 }
 
-inline int grid_for(hb_ctx* c, long long n)
-{
-  long long g = (n + ET - 1) / ET;
-  const long long cap = (long long)c->num_sms * 8;
-  if(g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 } // namespace
 
 extern "C" int hb_iterate_fraction_to_bdry(hb_lowrank* k, const double* const* it, const double* const* dir, double tau, double* alpha_primal,
@@ -198,20 +158,18 @@ extern "C" int hb_iterate_fraction_to_bdry(hb_lowrank* k, const double* const* i
   hb_ctx* c = k->ctx;
   const long long n = k->n;
   const int mi = k->mineq;
-  const int gx = grid_for(c, n), gd = grid_for(c, mi);
+  const int gx = hb_grid(c, n, ET), gd = hb_grid(c, mi, ET);
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * (2 * (size_t)(gx + gd) + 4)));
   double* px = (double*)c->ws;
   double* pd = px + 2 * (size_t)gx;
   double* out = pd + 2 * (size_t)gd; // {x primal, x dual, d primal, d dual}
   k_ftb_block<<<gx, ET, 0, c->stream>>>(n, tau, it[SXL], dir[SXL], it[SXU], dir[SXU], it[ZL], dir[ZL], it[ZU], dir[ZU], k->ixl, k->ixu, px);
   HB_LAUNCHED();
-  k_min2_final<<<1, 64, 0, c->stream>>>(gx, px, out);
-  HB_LAUNCHED();
-  if(c->nranks > 1) HB_CHECK(hb_allreduce_op(c, out, 2, 3)); // x-side blocks are sharded: MPI_MIN of the reference (:356-360)
+  HB_CHECK(hb_reduce_slots(c, gx, px, out, {HB_MIN, HB_MIN}));
+  if(c->nranks > 1) HB_CHECK(hb_allreduce_op(c, out, 2, HB_MIN)); // x-side blocks are sharded: MPI_MIN of the reference (:356-360)
   k_ftb_block<<<gd, ET, 0, c->stream>>>(mi, tau, it[SDL], dir[SDL], it[SDU], dir[SDU], it[VL], dir[VL], it[VU], dir[VU], k->idl, k->idu, pd);
   HB_LAUNCHED();
-  k_min2_final<<<1, 64, 0, c->stream>>>(gd, pd, out + 2);
-  HB_LAUNCHED();
+  HB_CHECK(hb_reduce_slots(c, gd, pd, out + 2, {HB_MIN, HB_MIN}));
   double h[4];
   HB_CUDA(cudaMemcpyAsync(h, out, sizeof(double) * 4, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
@@ -240,7 +198,7 @@ extern "C" int hb_iterate_take_step(hb_lowrank* k, const double* const* it, cons
       if(len > mx) mx = len;
     }
     if(A.count == 0) return HB_OK;
-    k_take_step<<<grid_for(c, mx), ET, 0, c->stream>>>(A);
+    k_take_step<<<hb_grid(c, mx, ET), ET, 0, c->stream>>>(A);
     HB_LAUNCHED();
     return HB_OK;
   };
@@ -263,11 +221,11 @@ extern "C" int hb_iterate_adjust_duals_plh(hb_lowrank* k, double* const* it, dou
   HB_REQUIRE(k->n == 0 || k->ixl, "hb_iterate_adjust_duals_plh: patterns not set");
   hb_ctx* c = k->ctx;
   if(k->n > 0) {
-    k_adjust_duals<<<grid_for(c, k->n), ET, 0, c->stream>>>(k->n, mu, kappa_sigma, it[SXL], it[SXU], k->ixl, k->ixu, it[ZL], it[ZU]);
+    k_adjust_duals<<<hb_grid(c, k->n, ET), ET, 0, c->stream>>>(k->n, mu, kappa_sigma, it[SXL], it[SXU], k->ixl, k->ixu, it[ZL], it[ZU]);
     HB_LAUNCHED();
   }
   if(k->mineq > 0) {
-    k_adjust_duals<<<grid_for(c, k->mineq), ET, 0, c->stream>>>(k->mineq, mu, kappa_sigma, it[SDL], it[SDU], k->idl, k->idu, it[VL], it[VU]);
+    k_adjust_duals<<<hb_grid(c, k->mineq, ET), ET, 0, c->stream>>>(k->mineq, mu, kappa_sigma, it[SDL], it[SDU], k->idl, k->idu, it[VL], it[VU]);
     HB_LAUNCHED();
   }
   return HB_OK;
@@ -293,7 +251,7 @@ extern "C" int hb_iterate_adjust_small_slacks(hb_lowrank* k, double* const* it, 
     double smin = 0.0;
     HB_CHECK(hb_vec_min_w_pattern(c, b.len, it[b.s], b.sel, &smin)); // slack.min_w_pattern(select) :432
     if(!(smin < small_val)) continue;
-    k_adjust_small_slack<<<grid_for(c, b.len), ET, 0, c->stream>>>(b.len, mu, small_val, scale_fact, b.bound, it_curr[b.z], b.sel, it[b.s], cnt);
+    k_adjust_small_slack<<<hb_grid(c, b.len, ET), ET, 0, c->stream>>>(b.len, mu, small_val, scale_fact, b.bound, it_curr[b.z], b.sel, it[b.s], cnt);
     HB_LAUNCHED();
   }
   int h = 0;
@@ -313,7 +271,7 @@ extern "C" int hb_iterate_logbar(hb_lowrank* k, const double* const* it, double 
   hb_ctx* c = k->ctx;
   const long long n = k->n;
   const int mi = k->mineq;
-  const int gx = grid_for(c, n), gd = grid_for(c, mi);
+  const int gx = hb_grid(c, n, ET), gd = hb_grid(c, mi, ET);
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * (2 * (size_t)(gx + gd) + 4)));
   double* px = (double*)c->ws;
   double* pd = px + 2 * (size_t)gx;
@@ -322,13 +280,11 @@ extern "C" int hb_iterate_logbar(hb_lowrank* k, const double* const* it, double 
   const bool damp = kappa_d > 0.0;
   k_logbar_block<<<gx, ET, 0, c->stream>>>(n, it[SXL], it[SXU], k->ixl, k->ixu, mu, ct, damp, grad_f, grad_x_logbar, px);
   HB_LAUNCHED();
-  k_sum2_final<<<1, 64, 0, c->stream>>>(gx, px, out);
-  HB_LAUNCHED();
-  if(c->nranks > 1) HB_CHECK(hb_allreduce_op(c, out, 2, 0)); // :529-533, :561-565
+  HB_CHECK(hb_reduce_slots(c, gx, px, out, {HB_SUM, HB_SUM}));
+  if(c->nranks > 1) HB_CHECK(hb_allreduce_op(c, out, 2, HB_SUM)); // :529-533, :561-565
   k_logbar_block<<<gd, ET, 0, c->stream>>>(mi, it[SDL], it[SDU], k->idl, k->idu, mu, ct, damp, nullptr, grad_d_logbar, pd);
   HB_LAUNCHED();
-  k_sum2_final<<<1, 64, 0, c->stream>>>(gd, pd, out + 2);
-  HB_LAUNCHED();
+  HB_CHECK(hb_reduce_slots(c, gd, pd, out + 2, {HB_SUM, HB_SUM}));
   double h[4];
   HB_CUDA(cudaMemcpyAsync(h, out, sizeof(double) * 4, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));

@@ -46,14 +46,6 @@ Layout make_layout(const hb_lowrank* k)
   return L;
 }
 
-inline int egrid(hb_ctx* c, long long items)
-{
-  long long g = (items + ET - 1) / ET;
-  const long long cap = (long long)c->num_sms * 8;
-  if(g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 // One primal block (x with its bound slacks/duals, or d with its): the rows of hiopMatVecKKTFullOpr::times_vec that are
 // elementwise (hiopKKTLinSys.cpp:1672-1730), same operation order:
 //   y0   = (y0 - dzl) + dzu                 y0 arrives holding H dx + J^T dy  (x block)  or  -dyd  (d block)
@@ -88,12 +80,6 @@ __global__ void k_split_jdx(int me, int mi, const double* __restrict__ jdx, cons
   if(i < me) yryc[i] = jdx[i];
   else if(i < me + mi) yryd[i - me] = __dsub_rn(jdx[i], dd[i - me]);
 }
-__global__ void k_stack(int me, int mi, const double* __restrict__ a, const double* __restrict__ b, double* __restrict__ out)
-{
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if(i < me) out[i] = a[i];
-  else if(i < me + mi) out[i] = b[i - me];
-}
 
 constexpr int KRY_EXTRA = 4 * 2048 + 64;
 
@@ -120,16 +106,15 @@ int full_times_vec(hb_lowrank* k, const Layout& L, double* y, const double* x)
   // rx = H dx + Jc^T dyc + Jd^T dyd - dzl + dzu                                         :1672-1678 (all deltas are 0: QN path)
   HB_CHECK(hb_lowrank_hess_times_vec(k, 0.0, Y(PX), 1.0, X(PX), 0));
   if(m > 0) {
-    k_stack<<<(m + 127) / 128, 128, 0, c->stream>>>(me, mi, X(PYC), X(PYD), dy);
-    HB_LAUNCHED();
-    HB_CHECK(hb_lr_gemv_cols(k, k->J, m, 1.0, Y(PX), 1.0, dy));
+    HB_CHECK(hb_stack(c, me, X(PYC), mi, X(PYD), dy));
+    HB_CHECK(gemv_cols(c, m, n, k->J, n, 1.0, Y(PX), 1.0, dy));
     // ryc = Jc dx; ryd = Jd dx - dd                                                      :1687-1694
-    HB_CHECK(hb_lr_gemv_rows(k, k->J, m, 0.0, jdx, 1.0, X(PX)));
+    HB_CHECK(gemv_rows(c, m, n, k->J, n, 0.0, jdx, 1.0, X(PX)));
     k_split_jdx<<<(m + 127) / 128, 128, 0, c->stream>>>(me, mi, jdx, X(PD), Y(PYC), Y(PYD));
     HB_LAUNCHED();
   }
   if(n > 0) {
-    k_kkt_full_block<<<egrid(c, n), ET, 0, c->stream>>>(n, X(PX), X(PSXL), X(PSXU), X(PZL), X(PZU), k->sxl, k->zl, k->sxu, k->zu, k->ixl, k->ixu, Y(PX),
+    k_kkt_full_block<<<hb_grid(c, n, ET), ET, 0, c->stream>>>(n, X(PX), X(PSXL), X(PSXU), X(PZL), X(PZU), k->sxl, k->zl, k->sxu, k->zu, k->ixl, k->ixu, Y(PX),
                                                         Y(PSXL), Y(PSXU), Y(PZL), Y(PZU));
     HB_LAUNCHED();
   }
@@ -137,7 +122,7 @@ int full_times_vec(hb_lowrank* k, const Layout& L, double* y, const double* x)
     // rd = -dyd - dvl + dvu                                                              :1680-1685
     k_neg<<<(mi + 127) / 128, 128, 0, c->stream>>>(mi, Y(PD), X(PYD));
     HB_LAUNCHED();
-    k_kkt_full_block<<<egrid(c, mi), ET, 0, c->stream>>>(mi, X(PD), X(PSDL), X(PSDU), X(PVL), X(PVU), k->sdl, k->vl, k->sdu, k->vu, k->idl, k->idu,
+    k_kkt_full_block<<<hb_grid(c, mi, ET), ET, 0, c->stream>>>(mi, X(PD), X(PSDL), X(PSDU), X(PVL), X(PVU), k->sdl, k->vl, k->sdu, k->vu, k->idl, k->idu,
                                                          Y(PD), Y(PSDL), Y(PSDU), Y(PVL), Y(PVU));
     HB_LAUNCHED();
   }
@@ -241,16 +226,6 @@ k_kry_pass(long long len, long long red_len, const double* __restrict__ sc, int 
   if(threadIdx.x == 0) {
     partial[blockIdx.x * 4 + 0] = r0; partial[blockIdx.x * 4 + 1] = r1; partial[blockIdx.x * 4 + 2] = r2; partial[blockIdx.x * 4 + 3] = r3;
   }
-}
-// sums[q] = sum over the per-CTA partials, fixed order (one warp per q)
-__global__ void __launch_bounds__(128)
-k_kry_final(int np, const double* __restrict__ partial, double* __restrict__ sums)
-{
-  const int q = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  double a = 0.0;
-  for(int i = lane; i < np; i += 32) a += partial[i * 4 + q];
-  a = hb_warp_sum(a);
-  if(lane == 0) sums[q] = a;
 }
 // the scalar recurrences and breakdown guards (hiopKrylovSolver.cpp:476-486, 505-513, 576-590), one thread
 __global__ void k_kry_scalars(int op, int ii, double* __restrict__ sc, const double* __restrict__ sums)
@@ -358,7 +333,7 @@ extern "C" int hb_lowrank_compute_directions_w_ir(hb_lowrank* k, const double* c
   bool returned_xk = false; // the two "tol is too small" exits copy xk into b before the closing min-residual test (:546, :623)
   // device scalar block + per-CTA partial sums live behind the m-workspace; the host mirror is the pinned stats buffer of the handle
   hb_ctx* c = k->ctx;
-  int kg = egrid(c, L.total);
+  int kg = hb_grid(c, L.total, KT);
   if(kg > 2048) kg = 2048;
   double* partial = k->kry_m + (size_t)(2 * k->m + 2); // (the context workspace is used by the kernels inside precond / K)
   double* sc = partial + (size_t)kg * 4;
@@ -366,8 +341,7 @@ extern "C" int hb_lowrank_compute_directions_w_ir(hb_lowrank* k, const double* c
   double sc_host[SC_COUNT];
   const long long red_len = cv.red_len();
   auto group = [&](int op, int ii_) -> int { // partials -> 4 sums (all-reduced) -> scalar program
-    k_kry_final<<<1, 128, 0, c->stream>>>(kg, partial, sums);
-    HB_LAUNCHED();
+    HB_CHECK(hb_reduce_slots(c, kg, partial, sums, {HB_SUM, HB_SUM, HB_SUM, HB_SUM}));
     HB_CHECK(hb_allreduce_sum(c, sums, 4));
     k_kry_scalars<<<1, 32, 0, c->stream>>>(op, ii_, sc, sums);
     HB_LAUNCHED();

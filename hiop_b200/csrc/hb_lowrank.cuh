@@ -1,4 +1,4 @@
-// Shared between hb_lowrank.cu and hb_krylov.cu: the quasi-Newton KKT handle and the two Jacobian gemv helpers.
+// The quasi-Newton KKT handle and the helpers of hb_lowrank.cu that the other files of the IPM vector path call.
 #pragma once
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
@@ -57,12 +57,12 @@ struct hb_lowrank
   double sec_sigma0 = 1.0;
 };
 
-
-// y = beta*y + alpha*A x over the local columns (+ all-reduce, beta*y on rank 0 only); A is m x n_local row-major
-int hb_lr_gemv_rows(hb_lowrank* k, const double* A, int m, double beta, double* y, double alpha, const double* x);
-// y = beta*y + alpha*A^T x (local columns only, no reduction)
-int hb_lr_gemv_cols(hb_lowrank* k, const double* A, int m, double beta, double* y, double alpha, const double* x);
+// The Jacobian gemvs (hb_lowrank.cu) for an m x n row-major A with leading dimension lda (elements), n = the local columns.
+// y = beta*y + alpha*A x, summed over the ranks (beta*y on rank 0 only)
+int gemv_rows(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
+// y = beta*y + alpha*A^T x over the local columns (no reduction)
+int gemv_cols(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
 // k->p2l (device, 2l doubles) = [sigma_s * S (w.*x); Y (w.*x)], all-reduced; w may be NULL
-int hb_lr_multidot(hb_lowrank* k, const double* w, const double* x, double sigma_s);
+int multidot(hb_lowrank* k, const double* w, const double* x, double sigma_s);
 // device table of row pointers [J rows (m); S rows (l); Y rows (l)] -> k->rowptr_dev, k->rows_aligned
-int hb_lr_refresh_rowptr(hb_lowrank* k);
+int refresh_rowptr(hb_lowrank* k);

@@ -12,11 +12,6 @@
 #include "hb_dense.cuh"
 #include "../../include/hiopb200.h"
 
-int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
-                 const double* fuse_rx = nullptr, double* tdot = nullptr);
-int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
-                       const double* dot_x, double* dot_out);
-
 namespace {
 constexpr int ET = 256;
 // vecx = (grad_f - zl) + zu                                                             :281-283
@@ -53,7 +48,7 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   HB_CHECK(k->lsq_M.reserve(c, (size_t)m * m + 2 * m, "the LSQ workspace"));
   double* M = k->lsq_M;
   double* rhs = M + (size_t)m * m;
-  HB_CHECK(hb_lr_refresh_rowptr(k));
+  HB_CHECK(refresh_rowptr(k));
   // J J^T: rows 0..m-1 of the row-pointer table are the Jacobian rows
   const int mode = k->condense_mode < 0 ? 0 : k->condense_mode; // AUTO = exact FP64 DMMA, as for the condensation
   if(mode == 0) HB_CHECK(hb_syrk_rows(c, m, n, k->rowptr_dev, k->rows_aligned, nullptr, M, m));
@@ -61,12 +56,10 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   HB_CHECK(hb_allreduce_sum(c, M, (long long)m * m));
   // rhs = -J vecx (all-reduced), then the d-side terms on the replicated part
   if(n > 0) {
-    long long g = (n + ET - 1) / ET;
-    const long long cap = (long long)c->num_sms * 8;
-    k_lsq_vecx<<<(int)(g > cap ? cap : g), ET, 0, c->stream>>>(n, grad_f, zl, zu, k->nv1);
+    k_lsq_vecx<<<hb_grid(c, n, ET), ET, 0, c->stream>>>(n, grad_f, zl, zu, k->nv1);
     HB_LAUNCHED();
   }
-  HB_CHECK(hb_lr_gemv_rows(k, k->J, m, 0.0, rhs, -1.0, k->nv1));
+  HB_CHECK(gemv_rows(c, m, n, k->J, n, 0.0, rhs, -1.0, k->nv1));
   if(mi > 0) {
     k_lsq_dpart<<<(mi + 127) / 128, 128, 0, c->stream>>>(me, mi, m, M, rhs, vl, vu);
     HB_LAUNCHED();

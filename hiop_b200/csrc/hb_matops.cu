@@ -12,13 +12,6 @@
 namespace {
 
 constexpr int MT = 256;
-inline int mgrid(hb_ctx* c, long long items)
-{
-  long long g = (items + MT - 1) / MT;
-  const long long cap = (long long)c->num_sms * 8;
-  if(g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
 
 // C(i,j) = beta C(i,j) + alpha sum_k A(i,k) B(j,k): one warp per output entry, lanes along k (rows are contiguous)
 __global__ void __launch_bounds__(MT)
@@ -102,16 +95,6 @@ k_curv_sums(long long n, const double* __restrict__ x, const double* __restrict_
   const double ra = hb_block_sum<MT>(a, sm), rb = hb_block_sum<MT>(b, sm);
   if(threadIdx.x == 0) { partial[2 * blockIdx.x] = ra; partial[2 * blockIdx.x + 1] = rb; }
 }
-__global__ void k_curv_final(int np1, int np2, const double* __restrict__ p1, const double* __restrict__ p2, double* __restrict__ out /* 4 */)
-{
-  const int lane = threadIdx.x & 31, q = threadIdx.x >> 5; // warp q: 0,1 -> x sums, 2,3 -> d sums
-  const double* p = q < 2 ? p1 : p2;
-  const int np = q < 2 ? np1 : np2;
-  double s = 0.0;
-  for(int i = lane; i < np; i += 32) s += p[2 * i + (q & 1)];
-  s = hb_warp_sum(s);
-  if(lane == 0) out[q] = s;
-}
 
 } // namespace
 
@@ -120,7 +103,7 @@ extern "C" int hb_mat_times_mat_trans(hb_ctx* c, int m, int k, long long n, cons
 {
   HB_REQUIRE(c && m >= 0 && k >= 0 && n >= 0 && lda >= n && ldb >= n && ldc >= k, "hb_mat_times_mat_trans: bad arguments");
   if(m == 0 || k == 0) return HB_OK;
-  k_times_mat_trans<<<mgrid(c, (long long)m * k * 32), MT, 0, c->stream>>>(m, k, n, A, lda, B, ldb, beta, C, ldc, alpha);
+  k_times_mat_trans<<<hb_grid(c, (long long)m * k * 32, MT), MT, 0, c->stream>>>(m, k, n, A, lda, B, ldb, beta, C, ldc, alpha);
   HB_LAUNCHED();
   if(c->nranks > 1) return hb_fail(HB_ERR_INVALID, "hb_mat_times_mat_trans: local (non-reduced) product only%s", "");
   return HB_OK;
@@ -138,7 +121,7 @@ extern "C" int hb_mat_add_matrix(hb_ctx* c, int m, int n, double* Y, long long l
 {
   HB_REQUIRE(c && m >= 0 && n >= 0 && ldy >= n && ldx >= n, "hb_mat_add_matrix: bad arguments");
   if(m == 0 || n == 0) return HB_OK;
-  k_add_matrix<<<mgrid(c, (long long)m * n), MT, 0, c->stream>>>(m, n, Y, ldy, alpha, X, ldx);
+  k_add_matrix<<<hb_grid(c, (long long)m * n, MT), MT, 0, c->stream>>>(m, n, Y, ldy, alpha, X, ldx);
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -146,7 +129,7 @@ extern "C" int hb_mat_copy_rows_from(hb_ctx* c, int n_rows, int n_cols, double* 
 {
   HB_REQUIRE(c && n_rows >= 0 && n_cols >= 0 && (rows_idx_dev || n_rows == 0), "hb_mat_copy_rows_from: bad arguments");
   if(n_rows == 0 || n_cols == 0) return HB_OK;
-  k_copy_block<<<mgrid(c, (long long)n_rows * n_cols), MT, 0, c->stream>>>(n_rows, n_cols, dst, ldd, 0, 0, src, lds, rows_idx_dev, 0, 0);
+  k_copy_block<<<hb_grid(c, (long long)n_rows * n_cols, MT), MT, 0, c->stream>>>(n_rows, n_cols, dst, ldd, 0, 0, src, lds, rows_idx_dev, 0, 0);
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -155,7 +138,7 @@ extern "C" int hb_mat_copy_block(hb_ctx* c, int m, int n, double* dst, long long
 {
   HB_REQUIRE(c && m >= 0 && n >= 0 && dst_i >= 0 && dst_j >= 0 && src_i >= 0 && src_j >= 0, "hb_mat_copy_block: bad arguments");
   if(m == 0 || n == 0) return HB_OK;
-  k_copy_block<<<mgrid(c, (long long)m * n), MT, 0, c->stream>>>(m, n, dst, ldd, dst_i, dst_j, src, lds, nullptr, src_i, src_j);
+  k_copy_block<<<hb_grid(c, (long long)m * n, MT), MT, 0, c->stream>>>(m, n, dst, ldd, dst_i, dst_j, src, lds, nullptr, src_i, src_j);
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -164,7 +147,7 @@ extern "C" int hb_mat_trans_add_to_sym_upper(hb_ctx* c, int m, int n, const doub
 {
   HB_REQUIRE(c && m >= 0 && n >= 0 && row_start >= 0 && col_start >= row_start, "hb_mat_trans_add_to_sym_upper: the block must lie in the upper triangle");
   if(m == 0 || n == 0) return HB_OK;
-  k_trans_add_upper<<<mgrid(c, (long long)m * n), MT, 0, c->stream>>>(m, n, A, lda, row_start, col_start, alpha, W, ldw);
+  k_trans_add_upper<<<hb_grid(c, (long long)m * n, MT), MT, 0, c->stream>>>(m, n, A, lda, row_start, col_start, alpha, W, ldw);
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -172,7 +155,7 @@ extern "C" int hb_mat_add_upper_to_sym_upper(hb_ctx* c, int n, const double* A, 
 {
   HB_REQUIRE(c && n >= 0 && diag_start >= 0, "hb_mat_add_upper_to_sym_upper: bad arguments");
   if(n == 0) return HB_OK;
-  k_add_upper_to_upper<<<mgrid(c, (long long)n * n), MT, 0, c->stream>>>(n, A, lda, diag_start, alpha, W, ldw);
+  k_add_upper_to_upper<<<hb_grid(c, (long long)n * n, MT), MT, 0, c->stream>>>(n, A, lda, diag_start, alpha, W, ldw);
   HB_LAUNCHED();
   return HB_OK;
 }
@@ -190,7 +173,7 @@ extern "C" int hb_lowrank_test_direction(hb_lowrank* k, const double* dx, const 
     HB_CHECK(hb_lowrank_hess_times_vec(k, 0.0, k->nv2, 1.0, dx, 0)); // B dx (compact form)
     HB_CHECK(hb_vec_dot(c, k->n, k->nv2, dx, &bxx));                  // all-reduced
   }
-  const int g1 = mgrid(c, k->n), g2 = mgrid(c, k->mineq);
+  const int g1 = hb_grid(c, k->n, MT), g2 = hb_grid(c, k->mineq, MT);
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * (2 * (size_t)(g1 + g2) + 8)));
   double* p1 = (double*)c->ws;
   double* p2 = p1 + 2 * g1;
@@ -199,8 +182,8 @@ extern "C" int hb_lowrank_test_direction(hb_lowrank* k, const double* dx, const 
   HB_LAUNCHED();
   k_curv_sums<<<g2, MT, 0, c->stream>>>(k->mineq, dd, k->Dd, delta_wd, p2);
   HB_LAUNCHED();
-  k_curv_final<<<1, 128, 0, c->stream>>>(g1, g2, p1, p2, out);
-  HB_LAUNCHED();
+  HB_CHECK(hb_reduce_slots(c, g1, p1, out, {HB_SUM, HB_SUM}));
+  HB_CHECK(hb_reduce_slots(c, g2, p2, out + 2, {HB_SUM, HB_SUM}));
   if(c->nranks > 1) {
     // the x-sized sums are sharded, the d-sized ones replicated: only rank 0 contributes the latter
     if(c->rank != 0) HB_CUDA(cudaMemsetAsync(out + 2, 0, 2 * sizeof(double), c->stream));

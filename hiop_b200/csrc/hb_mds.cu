@@ -5,7 +5,6 @@
 // :307-403 (solveCompressed); matrix kernels src/LinAlg/hiopMatrixDenseRowMajor.cpp:719-829 and
 // src/LinAlg/hiopMatrixSparseTriplet.cpp:390-525. The sparse block stays on ONE GPU (north star).
 #include "hb_common.cuh"
-#include <algorithm>
 
 struct hb_mds
 {
@@ -162,12 +161,6 @@ __global__ void k_mds_unpack(int nxs, int nxd, int neq, int nineq, const double*
   }
 }
 
-inline int grid1(hb_ctx* c, long long items)
-{
-  long long g = (items + T - 1) / T, cap = (long long)c->num_sms * 8;
-  return (int)std::max(1LL, std::min(g, cap));
-}
-
 } // namespace
 
 extern "C" int hb_mds_create(hb_ctx* c, int nxs, int nxd, int neq, int nineq, hb_mds** out)
@@ -251,7 +244,7 @@ extern "C" int hb_mds_update(hb_mds* h, const double* zl, const double* sxl, con
   HB_REQUIRE(n == 0 || (zl && sxl && zu && sxu && ixl && ixu), "hb_mds_update: null argument");
   hb_ctx* c = h->ctx;
   if(n > 0) {
-    k_mds_update<<<grid1(c, n), T, 0, c->stream>>>(n, zl, sxl, zu, sxu, ixl, ixu, h->Dx);
+    k_mds_update<<<hb_grid(c, n, T), T, 0, c->stream>>>(n, zl, sxl, zu, sxu, ixl, ixu, h->Dx);
     HB_LAUNCHED();
   }
   h->have_update = true;
@@ -275,15 +268,15 @@ extern "C" int hb_mds_build_kkt_matrix(hb_mds* h, const double* Hd, const double
   if(h->nnz_d) HB_CUDA(cudaMemcpyAsync(h->vals + h->nnz_c, Jds_vals, sizeof(double) * h->nnz_d, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(int) * 2, c->stream));
   if(h->nxs) {
-    k_mds_hxs<<<grid1(c, h->nxs), T, 0, c->stream>>>(h->nxs, h->Dx, delta_wx, Hs_diag, h->Hxs, h->counts);
+    k_mds_hxs<<<hb_grid(c, h->nxs, T), T, 0, c->stream>>>(h->nxs, h->Dx, delta_wx, Hs_diag, h->Hxs, h->counts);
     HB_LAUNCHED();
   }
   if(h->nineq) {
-    k_mds_ddinv<<<grid1(c, h->nineq), T, 0, c->stream>>>(h->nineq, delta_wd, vl, sdl, vu, sdu, idl, idu, h->Dd_inv);
+    k_mds_ddinv<<<hb_grid(c, h->nineq, T), T, 0, c->stream>>>(h->nineq, delta_wd, vl, sdl, vu, sdu, idl, idu, h->Dd_inv);
     HB_LAUNCHED();
   }
   if(N > 0) {
-    k_mds_build<<<grid1(c, (long long)N * N), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, Hd, Jcd, Jdd, h->Dx, delta_wx, h->csr_ptr,
+    k_mds_build<<<hb_grid(c, (long long)N * N, T), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, Hd, Jcd, Jdd, h->Dx, delta_wx, h->csr_ptr,
                                                                h->csr_col, h->vals, h->Hxs, delta_cc, h->Dd_inv, delta_cd, Msys);
     HB_LAUNCHED();
   }
@@ -314,18 +307,18 @@ extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* 
   hb_ctx* c = h->ctx;
   const int N = h->nxd + h->neq + h->nineq;
   if(h->nxs) {
-    k_mds_rxs<<<grid1(c, h->nxs), T, 0, c->stream>>>(h->nxs, rx, h->Hxs, h->rxs);
+    k_mds_rxs<<<hb_grid(c, h->nxs, T), T, 0, c->stream>>>(h->nxs, rx, h->Hxs, h->rxs);
     HB_LAUNCHED();
   }
   if(N) {
-    k_mds_pack_rhs<<<grid1(c, N), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, rx, ryc, ryd, h->csr_ptr, h->csr_col, h->vals, h->rxs, h->rhs);
+    k_mds_pack_rhs<<<hb_grid(c, N, T), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, rx, ryc, ryd, h->csr_ptr, h->csr_col, h->vals, h->rxs, h->rhs);
     HB_LAUNCHED();
     const int rc = hb_symdense_solve(s, h->rhs, 1);
     if(rc != 1) return rc < 0 ? rc : hb_fail(HB_ERR_NUMERIC, "hb_mds_solve_compressed: dense solve failed%s", "");
   }
   const int total = h->nxs + h->nxd + h->neq + h->nineq;
   if(total) {
-    k_mds_unpack<<<grid1(c, total), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, h->rhs, rx, h->csc_ptr, h->csc_row, h->csc_src, h->vals,
+    k_mds_unpack<<<hb_grid(c, total, T), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, h->rhs, rx, h->csc_ptr, h->csc_row, h->csc_src, h->vals,
                                                       h->Hxs, dx, dyc, dyd);
     HB_LAUNCHED();
   }
@@ -407,16 +400,16 @@ extern "C" int hb_densekkt_build(hb_ctx* c, int form, int nx, int neq, int nineq
   HB_REQUIRE((neq == 0 || Jc) && Msys, "hb_densekkt_build: null argument");
   HB_CUDA(cudaSetDevice(c->device));
   if(nx) {
-    k_mds_update<<<grid1(c, nx), T, 0, c->stream>>>(nx, zl, sxl, zu, sxu, ixl, ixu, Dx);
+    k_mds_update<<<hb_grid(c, nx, T), T, 0, c->stream>>>(nx, zl, sxl, zu, sxu, ixl, ixu, Dx);
     HB_LAUNCHED();
   }
   if(nineq) {
-    k_dense_dd<<<grid1(c, nineq), T, 0, c->stream>>>(nineq, form, delta_wd, vl, sdl, vu, sdu, idl, idu, Dd);
+    k_dense_dd<<<hb_grid(c, nineq, T), T, 0, c->stream>>>(nineq, form, delta_wd, vl, sdl, vu, sdu, idl, idu, Dd);
     HB_LAUNCHED();
   }
   const long long N = nx + neq + nineq + (form ? nineq : 0);
   if(N) {
-    k_densekkt_build<<<grid1(c, N * N), T, 0, c->stream>>>(form, nx, neq, nineq, H, Jc, Jd, Dx, delta_wx, delta_wd, delta_cd, Dd, Msys);
+    k_densekkt_build<<<hb_grid(c, N * N, T), T, 0, c->stream>>>(form, nx, neq, nineq, H, Jc, Jd, Dx, delta_wx, delta_wd, delta_cd, Dd, Msys);
     HB_LAUNCHED();
   }
   return HB_OK;

@@ -10,32 +10,19 @@
 #include "../../include/hiopb200.h"
 #include <cmath>
 
-int hb_allreduce_op(hb_ctx* c, double* buf, long long count, int op);
-
 namespace {
 
 constexpr int ET = 256;
 constexpr int NP = 6; // per-block partials: max|r0|, sum|r0|, max|r|, sum|r|, max complem (nlp), max complem (barrier)
-
-template <int T>
-__device__ __forceinline__ double block_max(double v, double* sm)
-{
-  v = hb_warp_max(v);
-  __syncthreads();
-  if((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double r = 0.0;
-  if(threadIdx.x == 0)
-    for(int w = 0; w < T / 32; w++) r = fmax(r, sm[w]);
-  return r; // valid in thread 0
-}
+const std::initializer_list<hb_op> NORM_OPS = {HB_MAX, HB_SUM, HB_MAX, HB_SUM, HB_MAX, HB_MAX};
 
 // XSIDE: r0 = (t - zl) + zu with t = grad + J^T y (already in r_opt), damping beta = +1, then negated     hiopResidual.cpp:176-190
 // else : r0 = (yd + vl) - vu,                                           damping beta = -1, not negated   :192-201
 // bound rows: rl = il ? (p - sl) - lo : 0;  ru = iu ? (XSIDE ? (up - p) - su : (up - su) - p) : 0         :239-278
 // complementarity: rz = i ? -(s z) [+ mu] : 0                                                             :285-345
+// 4 CTAs per SM (at most 64 registers): without the bound the six block reductions push the kernel past 64 registers and 3 CTAs
 template <bool XSIDE>
-__global__ void __launch_bounds__(ET)
+__global__ void __launch_bounds__(ET, 4)
 k_resid_block(long long n, const double* tin /* may alias r_opt */, const double* __restrict__ p, const double* __restrict__ sl, const double* __restrict__ su,
               const double* __restrict__ zl, const double* __restrict__ zu, const double* __restrict__ il, const double* __restrict__ iu,
               const double* __restrict__ lo, const double* __restrict__ up, double mu, double ct, bool damp, double* r_opt,
@@ -66,27 +53,12 @@ k_resid_block(long long n, const double* tin /* may alias r_opt */, const double
     rzu[i] = b;
   }
   double v;
-  v = block_max<ET>(m0, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 0] = v;
+  v = hb_block_reduce<HB_MAX, ET>(m0, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 0] = v;
   v = hb_block_sum<ET>(s0, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 1] = v;
-  v = block_max<ET>(m1, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 2] = v;
+  v = hb_block_reduce<HB_MAX, ET>(m1, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 2] = v;
   v = hb_block_sum<ET>(s1, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 3] = v;
-  v = block_max<ET>(c0, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 4] = v;
-  v = block_max<ET>(c1, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 5] = v;
-}
-
-// out[q] = max / sum over the per-block partials, fixed order (one CTA, 6 warps: warp q owns slot q)
-__global__ void k_resid_final(int nblocks, const double* __restrict__ partial, double* __restrict__ out)
-{
-  const int q = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if(q >= NP) return;
-  const bool is_sum = (q == 1 || q == 3);
-  double v = 0.0;
-  for(int b = lane; b < nblocks; b += 32) {
-    const double x = partial[(size_t)b * NP + q];
-    v = is_sum ? v + x : fmax(v, x);
-  }
-  v = is_sum ? hb_warp_sum(v) : hb_warp_max(v);
-  if(lane == 0) out[q] = v;
+  v = hb_block_reduce<HB_MAX, ET>(c0, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 4] = v;
+  v = hb_block_reduce<HB_MAX, ET>(c1, sm); if(threadIdx.x == 0) partial[(size_t)blockIdx.x * NP + 5] = v;
 }
 
 // constraint rows (one CTA): ryc = crhs - c, ryd = d_it - d; out = {max|ryc|, sum|ryc|, max|ryd|, sum|ryd|, viol_dl, viol_du}   :203-237
@@ -112,20 +84,13 @@ k_resid_cons(int me, int mi, const double* __restrict__ crhs, const double* __re
     if(idu[i] == 1.0) vu = fmax(vu, -__dsub_rn(du[i], dv[i]));
   }
   double v;
-  v = block_max<ET>(mc, sm); if(threadIdx.x == 0) out[0] = v;
+  v = hb_block_reduce<HB_MAX, ET>(mc, sm); if(threadIdx.x == 0) out[0] = v;
   v = hb_block_sum<ET>(sc, sm); if(threadIdx.x == 0) out[1] = v;
-  v = block_max<ET>(md, sm); if(threadIdx.x == 0) out[2] = v;
+  v = hb_block_reduce<HB_MAX, ET>(md, sm); if(threadIdx.x == 0) out[2] = v;
   v = hb_block_sum<ET>(sd, sm); if(threadIdx.x == 0) out[3] = v;
-  v = block_max<ET>(vl, sm); if(threadIdx.x == 0) out[4] = v;
-  v = block_max<ET>(vu, sm); if(threadIdx.x == 0) out[5] = v;
+  v = hb_block_reduce<HB_MAX, ET>(vl, sm); if(threadIdx.x == 0) out[4] = v;
+  v = hb_block_reduce<HB_MAX, ET>(vu, sm); if(threadIdx.x == 0) out[5] = v;
 }
-__global__ void k_stack_y(int me, int mi, const double* __restrict__ a, const double* __restrict__ b, double* __restrict__ out)
-{
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if(i < me) out[i] = a[i];
-  else if(i < me + mi) out[i] = b[i - me];
-}
-
 } // namespace
 
 extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it, const double* cvals, const double* dvals, const double* grad_f,
@@ -141,11 +106,7 @@ extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it
   const long long n = k->n;
   const int me = k->meq, mi = k->mineq, m = k->m;
   const double ct = kappa_d * mu * 1.0;
-  long long gx = (n + ET - 1) / ET;
-  if(gx > (long long)c->num_sms * 8) gx = (long long)c->num_sms * 8;
-  if(gx < 1) gx = 1;
-  int gd = (mi + ET - 1) / ET;
-  if(gd < 1) gd = 1;
+  const int gx = hb_grid(c, n, ET), gd = hb_grid(c, mi, ET);
   // workspace: partials of the two blocks, 6 + 6 + 6 results, stacked multipliers
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * ((size_t)(gx + gd) * NP + 18 + (size_t)m + 8)));
   double* px = (double*)c->ws;
@@ -159,22 +120,20 @@ extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it
     // rx <- grad_f + Jc^T yc + Jd^T yd                                                          :176-178
     HB_CUDA(cudaMemcpyAsync(res[RX], grad_f, sizeof(double) * n, cudaMemcpyDeviceToDevice, c->stream));
     if(m > 0) {
-      k_stack_y<<<(m + 127) / 128, 128, 0, c->stream>>>(me, mi, it[YC], it[YD], ystk);
-      HB_LAUNCHED();
-      HB_CHECK(hb_lr_gemv_cols(k, k->J, m, 1.0, res[RX], 1.0, ystk));
+      HB_CHECK(hb_stack(c, me, it[YC], mi, it[YD], ystk));
+      HB_CHECK(gemv_cols(c, m, n, k->J, n, 1.0, res[RX], 1.0, ystk));
     }
-    k_resid_block<true><<<(int)gx, ET, 0, c->stream>>>(n, res[RX], it[X], it[SXL], it[SXU], it[ZL], it[ZU], k->ixl, k->ixu, xl, xu, mu, ct, kappa_d > 0.0,
+    k_resid_block<true><<<gx, ET, 0, c->stream>>>(n, res[RX], it[X], it[SXL], it[SXU], it[ZL], it[ZU], k->ixl, k->ixu, xl, xu, mu, ct, kappa_d > 0.0,
                                                        res[RX], res[RXL], res[RXU], res[RSZL], res[RSZU], px);
     HB_LAUNCHED();
-    k_resid_final<<<1, 32 * NP, 0, c->stream>>>((int)gx, px, outx);
-    HB_LAUNCHED();
+    HB_CHECK(hb_reduce_slots(c, gx, px, outx, NORM_OPS));
   }
   if(c->nranks > 1) { // x-side blocks are sharded: combine the partial norms (d-side and constraint rows are replicated)
     // layout outx = {max, sum, max, sum, max, max}: reduce sums and maxima separately
     double* tmp = ystk + m;
     HB_CUDA(cudaMemcpyAsync(tmp, outx, sizeof(double) * 6, cudaMemcpyDeviceToDevice, c->stream));
-    HB_CHECK(hb_allreduce_op(c, outx, 6, 2));  // max of everything ...
-    HB_CHECK(hb_allreduce_op(c, tmp, 6, 0));   // ... and sum of everything; pick per slot below
+    HB_CHECK(hb_allreduce_op(c, outx, 6, HB_MAX)); // max of everything ...
+    HB_CHECK(hb_allreduce_op(c, tmp, 6, HB_SUM));  // ... and sum of everything; pick per slot below
     HB_CUDA(cudaMemcpyAsync(outx + 1, tmp + 1, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
     HB_CUDA(cudaMemcpyAsync(outx + 3, tmp + 3, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
   }
@@ -182,8 +141,7 @@ extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it
     k_resid_block<false><<<gd, ET, 0, c->stream>>>(mi, it[YD], it[D], it[SDL], it[SDU], it[VL], it[VU], k->idl, k->idu, dl, du, mu, -ct, kappa_d > 0.0,
                                                    res[RD], res[RDL], res[RDU], res[RSVL], res[RSVU], pd);
     HB_LAUNCHED();
-    k_resid_final<<<1, 32 * NP, 0, c->stream>>>(gd, pd, outd);
-    HB_LAUNCHED();
+    HB_CHECK(hb_reduce_slots(c, gd, pd, outd, NORM_OPS));
   }
   if(m > 0) {
     k_resid_cons<<<1, ET, 0, c->stream>>>(me, mi, crhs, cvals, it[D], dvals, dl, du, k->idl, k->idu, res[RYC], res[RYD], outc);

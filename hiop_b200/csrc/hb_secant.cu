@@ -74,20 +74,6 @@ k_secant_pair(long long n, const double* __restrict__ x, const double* __restric
     y[i] = __dsub_rn(g[i], gp[i]);
   }
 }
-__global__ void k_stack2(int me, int mi, const double* __restrict__ a, const double* __restrict__ b, double* __restrict__ out)
-{
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if(i < me) out[i] = a[i];
-  else if(i < me + mi) out[i] = b[i - me];
-}
-
-inline int egrid(hb_ctx* c, long long items)
-{
-  long long g = (items + ET - 1) / ET;
-  const long long cap = (long long)c->num_sms * 8;
-  if(g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
 
 int install(hb_lowrank* k)
 {
@@ -136,14 +122,13 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
     double* s = k->nv1;
     double* y = k->nv2;
     if(n > 0) {
-      k_secant_pair<<<egrid(c, n), ET, 0, c->stream>>>(n, x, k->sec_xprev, grad_f, k->sec_gprev, s, y);
+      k_secant_pair<<<hb_grid(c, n, ET), ET, 0, c->stream>>>(n, x, k->sec_xprev, grad_f, k->sec_gprev, s, y);
       HB_LAUNCHED();
     }
     if(needJ) {
       // y += (J - J_prev)^T [yc; yd], J_prev <- J in the same pass                       :291-297, 366-367
       HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)m));
-      k_stack2<<<(m + 127) / 128, 128, 0, c->stream>>>(k->meq, k->mineq, yc, yd, (double*)c->ws);
-      HB_LAUNCHED();
+      HB_CHECK(hb_stack(c, k->meq, yc, k->mineq, yd, (double*)c->ws));
       if(n > 0) {
         const long long pairs = (n + 1) / 2;
         k_gemv_cols_diff_store<<<(unsigned)((pairs + ET - 1) / ET), ET, 0, c->stream>>>(m, n, k->J, k->sec_Jprev, (const double*)c->ws, y);
@@ -164,7 +149,7 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
           const int l = k->sec_lcurr;
           double yts[64];
           if(l > 0) { // Y^T s with the memory as it is before the new pair enters          :309-310
-            HB_CHECK(hb_lr_multidot(k, nullptr, s, 1.0));
+            HB_CHECK(multidot(k, nullptr, s, 1.0));
             HB_CUDA(cudaMemcpyAsync(yts, k->p2l + l, sizeof(double) * l, cudaMemcpyDeviceToHost, c->stream));
             HB_CUDA(cudaStreamSynchronize(c->stream));
           }
