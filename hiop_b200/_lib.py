@@ -66,6 +66,8 @@ def lib() -> ctypes.CDLL:
     f("hb_free", c_i, c_vp, c_vp)
     f("hb_malloc_host", c_i, c_vp, ctypes.c_size_t, P(c_vp))
     f("hb_free_host", c_i, c_vp, c_vp)
+    f("hb_host_register", c_i, c_vp, c_vp, ctypes.c_size_t)
+    f("hb_host_unregister", c_i, c_vp, c_vp)
     f("hb_memcpy_h2d", c_i, c_vp, c_vp, c_vp, ctypes.c_size_t)
     f("hb_memcpy_d2h", c_i, c_vp, c_vp, c_vp, ctypes.c_size_t)
     f("hb_memcpy_d2d", c_i, c_vp, c_vp, c_vp, ctypes.c_size_t)
@@ -127,6 +129,7 @@ def lib() -> ctypes.CDLL:
     f("hb_lowrank_destroy", c_i, c_vp)
     f("hb_lowrank_set_patterns", c_i, c_vp, c_dp, c_dp, c_dp, c_dp)
     f("hb_lowrank_set_jacobian", c_i, c_vp, c_dp, c_dp)
+    f("hb_lowrank_set_jacobian_host", c_i, c_vp, c_vp, c_vp, c_ll)
     f("hb_lowrank_set_secant", c_i, c_vp, c_i, c_d, c_dp, c_dp, c_vp, c_vp)
     f("hb_lowrank_update", c_i, c_vp, *([c_dp] * 8))
     f("hb_lowrank_condense", c_i, c_vp)

@@ -35,6 +35,9 @@ private:
   int meq_, mineq_, lmax_;
   // device mirrors
   double *dJ_, *dSt_, *dYt_;
+  // HIOP_B200_JAC=host: HiOp's Jacobian buffers are page-locked in place and streamed from the host (no dJ_)
+  bool jac_host_ = false;
+  void* jac_pinned_[2] = {nullptr, nullptr};
   double* dsec_[4] = {nullptr, nullptr, nullptr, nullptr}; // x, grad_f, yc, yd of the iterate handed to the device-side secant update
   bool secant_ready_ = false;
   int n_secant_dev_ = 0;

@@ -189,7 +189,9 @@ hiopKKTLinSysLowRankB200::hiopKKTLinSysLowRankB200(hiopNlpFormulation* nlp)
 #endif
   if(!ok(hb_lowrank_create(ctx_, n_, meq_, mineq_, lmax_ > 0 ? lmax_ : 1, &h_), "hb_lowrank_create", &healthy_)) return;
   const size_t m = (size_t)meq_ + mineq_;
-  bool a = ok(hb_malloc(ctx_, sizeof(double) * m * n_, (void**)&dJ_), "hb_malloc(J)", &healthy_);
+  const char* jac = getenv("HIOP_B200_JAC");
+  jac_host_ = jac && !strcmp(jac, "host");
+  bool a = jac_host_ || ok(hb_malloc(ctx_, sizeof(double) * m * n_, (void**)&dJ_), "hb_malloc(J)", &healthy_);
   a = a && ok(hb_malloc(ctx_, sizeof(double) * (size_t)(lmax_ > 0 ? lmax_ : 1) * n_, (void**)&dSt_), "hb_malloc(S)", &healthy_);
   a = a && ok(hb_malloc(ctx_, sizeof(double) * (size_t)(lmax_ > 0 ? lmax_ : 1) * n_, (void**)&dYt_), "hb_malloc(Y)", &healthy_);
   const size_t psz[4] = {(size_t)n_, (size_t)n_, (size_t)mineq_, (size_t)mineq_};
@@ -220,6 +222,7 @@ hiopKKTLinSysLowRankB200::~hiopKKTLinSysLowRankB200()
   }
   if(h_) hb_lowrank_destroy(h_);
   if(!ctx_) return;
+  for(void* p : jac_pinned_) if(p) hb_host_unregister(ctx_, p);
   hb_free(ctx_, dJ_); hb_free(ctx_, dSt_); hb_free(ctx_, dYt_);
   for(auto* p : dsec_) if(p) hb_free(ctx_, p);
   for(auto* p : dpat_) hb_free(ctx_, p);
@@ -251,8 +254,28 @@ bool hiopKKTLinSysLowRankB200::update(const hiopIterate* iter, const hiopVector*
   //  * small Jacobians (<= 64 MB) are additionally fingerprinted, which catches constant Jacobians of problems that do not declare
   //    themselves linear (the bundled NlpDenseConsEx1/Ex2 re-evaluate theirs every iteration with identical values).
   const size_t jbytes = sizeof(double) * ((size_t)meq_ + mineq_) * n_;
+  if(jac_host_) {
+    // HIOP_B200_JAC=host: the engine reads [Jc; Jd] where HiOp's callbacks write it, streaming it through device panels on every pass.
+    // Its buffers are page-locked once (and again only if the formulation ever hands over different ones).
+    const double* src[2] = {Jac_c->local_data_const(), Jac_d->local_data_const()};
+    const size_t bytes[2] = {sizeof(double) * (size_t)meq_ * n_, sizeof(double) * (size_t)mineq_ * n_};
+    bool reg = false;
+    for(int i = 0; i < 2; i++) {
+      void* p = bytes[i] ? const_cast<double*>(src[i]) : nullptr;
+      if(p == jac_pinned_[i]) continue;
+      if(jac_pinned_[i]) hb_host_unregister(ctx_, jac_pinned_[i]);
+      jac_pinned_[i] = nullptr;
+      if(p && !ok(hb_host_register(ctx_, p, bytes[i]), "hb_host_register(J)", &healthy_)) return false;
+      jac_pinned_[i] = p;
+      reg = true;
+    }
+    if(reg || n_jac_uploads_ == 0) {
+      if(!ok(hb_lowrank_set_jacobian_host(h_, src[0], src[1], 0), "hb_lowrank_set_jacobian_host", &healthy_)) return false;
+      n_jac_uploads_++;
+    }
+  }
   const long long evals = (long long)nlp_->runStats.nEvalJac_con_eq + nlp_->runStats.nEvalJac_con_ineq;
-  bool changed = (n_jac_uploads_ == 0) || (evals != jac_evals_seen_);
+  bool changed = !jac_host_ && ((n_jac_uploads_ == 0) || (evals != jac_evals_seen_));
   unsigned long long hash = 0;
   if(changed && n_jac_uploads_ > 0 && jbytes <= ((size_t)64 << 20)) {
     hash = fnv1a(Jac_c->local_data_const(), sizeof(double) * (size_t)meq_ * n_) ^ (fnv1a(Jac_d->local_data_const(), sizeof(double) * (size_t)mineq_ * n_) * 31);

@@ -212,6 +212,19 @@ extern "C" int hb_free_host(hb_ctx* c, void* p)
   if(p) HB_CUDA(cudaFreeHost(p));
   return HB_OK;
 }
+extern "C" int hb_host_register(hb_ctx* c, void* p, size_t bytes)
+{
+  HB_REQUIRE(c && p && bytes > 0, "hb_host_register: bad arguments");
+  HB_CUDA(cudaSetDevice(c->device));
+  HB_CUDA(cudaHostRegister(p, bytes, cudaHostRegisterDefault));
+  return HB_OK;
+}
+extern "C" int hb_host_unregister(hb_ctx* c, void* p)
+{
+  HB_REQUIRE(c && p, "hb_host_unregister: bad arguments");
+  HB_CUDA(cudaHostUnregister(p));
+  return HB_OK;
+}
 extern "C" int hb_memcpy_h2d(hb_ctx* c, void* dst, const void* src, size_t bytes)
 {
   HB_REQUIRE(c, "null ctx");

@@ -107,9 +107,9 @@ int full_times_vec(hb_lowrank* k, const Layout& L, double* y, const double* x)
   HB_CHECK(hb_lowrank_hess_times_vec(k, 0.0, Y(PX), 1.0, X(PX), 0));
   if(m > 0) {
     HB_CHECK(hb_stack(c, me, X(PYC), mi, X(PYD), dy));
-    HB_CHECK(gemv_cols(c, m, n, k->J, n, 1.0, Y(PX), 1.0, dy));
+    HB_CHECK(jac_cols(k, 1.0, Y(PX), 1.0, dy));
     // ryc = Jc dx; ryd = Jd dx - dd                                                      :1687-1694
-    HB_CHECK(gemv_rows(c, m, n, k->J, n, 0.0, jdx, 1.0, X(PX)));
+    HB_CHECK(jac_rows(k, 0.0, jdx, 1.0, X(PX)));
     k_split_jdx<<<(m + 127) / 128, 128, 0, c->stream>>>(me, mi, jdx, X(PD), Y(PYC), Y(PYD));
     HB_LAUNCHED();
   }

@@ -3,6 +3,8 @@
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
 
+constexpr int HB_PANEL_RING = 3; // device panels of a host-resident Jacobian
+
 struct hb_lowrank
 {
   hb_ctx* ctx = nullptr;
@@ -44,12 +46,21 @@ struct hb_lowrank
   // secant memory owned by the engine (hb_secant.cu): S_t, Y_t (lmax x n), previous iterate / gradient / Jacobian
   hb_dev<double> sec_S, sec_Y, sec_xprev, sec_gprev, sec_Jprev;
   double sec_L[64 * 64] = {0}, sec_D[64] = {0}; // host copies of L (row-major, stride l) and D; lmax <= 64 in this mode
-  // chunked, copy-overlapped condensation of hb_lowrank_kkt_system_host
+  // host-resident Jacobian (hb_lowrank_set_jacobian_host): borrowed page-locked rows of Jc and Jd (ld = n), streamed through a ring of
+  // device panels of panel_cols columns (leading dimension panel_ld); panel_cols == 0: J is on the device (k->J)
+  const double *Jc_host = nullptr, *Jd_host = nullptr;
+  long long panel_cols = 0, panel_ld = 0;
+  hb_dev<double> panel[HB_PANEL_RING];
+  hb_event panel_free[HB_PANEL_RING]; // the context stream is done with a ring slot
+  // column chunks of J copied on a second stream while the context stream consumes earlier ones: the condensation of
+  // hb_lowrank_kkt_system_host and every pass over a host-resident J
   hb_stream copy_stream;
-  hb_event chunk_ev[32];
-  hb_dev<double> Ctmp;
+  hb_event copy_start, chunk_ev[4];
+  hb_dev<double> Ctmp; // partial C_aug (+ partial fused row dots) of one chunk
   hb_dev<const double*> chunk_rowptr_dev;
-  hb_pinned<const double*> chunk_rowptr_host; // 32 x (m + 2 lmax)
+  hb_pinned<const double*> chunk_rowptr_host; // rows of [J; S; Y] per chunk (chunks x (m + 2 l))
+  long long chunk_key[8] = {0};               // what chunk_rowptr_dev was built for
+  bool chunk_rows_aligned = false;
   hb_dev<double> Finv;  // 16 x 16 inverses of the diagonal of F (cooperative Cholesky / solve)
   hb_big big;           // look-ahead Cholesky of large condensed systems: panel stream, events, scratch
   hb_dev<double> lsq_M; // m x m LSQ matrix / Cholesky factor + 2 m-vectors (hb_lsq.cu)
@@ -62,6 +73,16 @@ struct hb_lowrank
 int gemv_rows(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
 // y = beta*y + alpha*A^T x over the local columns (no reduction)
 int gemv_cols(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
+// The registered Jacobian J = [Jc; Jd] of a handle, on the device or streamed from the host in column panels (same results: the J x
+// partials are kept per 2048 columns and summed in one fixed order, each column of J^T y depends on its own column only).
+bool jac_set(const hb_lowrank* k); // a Jacobian is registered (or m == 0)
+// y (m) = beta*y + alpha*J x, all-reduced like gemv_rows
+int jac_rows(hb_lowrank* k, double beta, double* y, double alpha, const double* x);
+// y (n) = beta*y + alpha*J^T x
+int jac_cols(hb_lowrank* k, double beta, double* y, double alpha, const double* x);
+// C (M x M, ldc = M) = R diag(d) R^T over the local columns, R = the first M rows of [J; S; Y]; FP64 DMMA (hb_syrk_rows), with its
+// fused extra row when fuse_rx is given (tdot, M doubles)
+int jac_syrk(hb_lowrank* k, int M, const double* d, double* C, const double* fuse_rx = nullptr, double* tdot = nullptr);
 // k->p2l (device, 2l doubles) = [sigma_s * S (w.*x); Y (w.*x)], all-reduced; w may be NULL
 int multidot(hb_lowrank* k, const double* w, const double* x, double sigma_s);
 // device table of row pointers [J rows (m); S rows (l); Y rows (l)] -> k->rowptr_dev, k->rows_aligned

@@ -37,7 +37,7 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
                                     double* yc, double* yd)
 {
   HB_REQUIRE(k, "null handle");
-  HB_REQUIRE(k->m == 0 || k->J, "hb_lowrank_lsq_duals: register the Jacobian with hb_lowrank_set_jacobian first");
+  HB_REQUIRE(jac_set(k), "hb_lowrank_lsq_duals: register the Jacobian with hb_lowrank_set_jacobian first");
   HB_REQUIRE(k->n == 0 || (grad_f && zl && zu), "hb_lowrank_lsq_duals: null x block");
   HB_REQUIRE(k->mineq == 0 || (vl && vu && yd), "hb_lowrank_lsq_duals: null d block");
   HB_REQUIRE(k->meq == 0 || yc, "hb_lowrank_lsq_duals: null yc");
@@ -48,18 +48,21 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   HB_CHECK(k->lsq_M.reserve(c, (size_t)m * m + 2 * m, "the LSQ workspace"));
   double* M = k->lsq_M;
   double* rhs = M + (size_t)m * m;
-  HB_CHECK(refresh_rowptr(k));
   // J J^T: rows 0..m-1 of the row-pointer table are the Jacobian rows
   const int mode = k->condense_mode < 0 ? 0 : k->condense_mode; // AUTO = exact FP64 DMMA, as for the condensation
-  if(mode == 0) HB_CHECK(hb_syrk_rows(c, m, n, k->rowptr_dev, k->rows_aligned, nullptr, M, m));
-  else HB_CHECK(hb_syrk_rows_ozaki(c, m, n, k->rowptr_dev, k->rows_aligned, nullptr, M, m, mode, nullptr, nullptr));
+  HB_REQUIRE(mode == 0 || !k->panel_cols, "hb_lowrank_lsq_duals: the int8-slice modes 6-8 need the Jacobian on the device");
+  if(mode == 0) HB_CHECK(jac_syrk(k, m, nullptr, M));
+  else {
+    HB_CHECK(refresh_rowptr(k));
+    HB_CHECK(hb_syrk_rows_ozaki(c, m, n, k->rowptr_dev, k->rows_aligned, nullptr, M, m, mode, nullptr, nullptr));
+  }
   HB_CHECK(hb_allreduce_sum(c, M, (long long)m * m));
   // rhs = -J vecx (all-reduced), then the d-side terms on the replicated part
   if(n > 0) {
     k_lsq_vecx<<<hb_grid(c, n, ET), ET, 0, c->stream>>>(n, grad_f, zl, zu, k->nv1);
     HB_LAUNCHED();
   }
-  HB_CHECK(gemv_rows(c, m, n, k->J, n, 0.0, rhs, -1.0, k->nv1));
+  HB_CHECK(jac_rows(k, 0.0, rhs, -1.0, k->nv1));
   if(mi > 0) {
     k_lsq_dpart<<<(mi + 127) / 128, 128, 0, c->stream>>>(me, mi, m, M, rhs, vl, vu);
     HB_LAUNCHED();

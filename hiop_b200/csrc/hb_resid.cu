@@ -99,7 +99,7 @@ extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it
 {
   HB_REQUIRE(k && it && res && norms_host, "hb_lowrank_residual_update: null argument");
   HB_REQUIRE(k->n == 0 || k->ixl, "hb_lowrank_residual_update: patterns not set");
-  HB_REQUIRE(k->m == 0 || k->J, "hb_lowrank_residual_update: register the Jacobian with hb_lowrank_set_jacobian first");
+  HB_REQUIRE(jac_set(k), "hb_lowrank_residual_update: register the Jacobian with hb_lowrank_set_jacobian first");
   enum { X, D, YC, YD, SXL, SXU, SDL, SDU, ZL, ZU, VL, VU };
   enum { RX, RD, RYC, RYD, RXL, RXU, RDL, RDU, RSZL, RSZU, RSVL, RSVU };
   hb_ctx* c = k->ctx;
@@ -121,7 +121,7 @@ extern "C" int hb_lowrank_residual_update(hb_lowrank* k, const double* const* it
     HB_CUDA(cudaMemcpyAsync(res[RX], grad_f, sizeof(double) * n, cudaMemcpyDeviceToDevice, c->stream));
     if(m > 0) {
       HB_CHECK(hb_stack(c, me, it[YC], mi, it[YD], ystk));
-      HB_CHECK(gemv_cols(c, m, n, k->J, n, 1.0, res[RX], 1.0, ystk));
+      HB_CHECK(jac_cols(k, 1.0, res[RX], 1.0, ystk));
     }
     k_resid_block<true><<<gx, ET, 0, c->stream>>>(n, res[RX], it[X], it[SXL], it[SXU], it[ZL], it[ZU], k->ixl, k->ixu, xl, xu, mu, ct, kappa_d > 0.0,
                                                        res[RX], res[RXL], res[RXU], res[RSZL], res[RSZU], px);

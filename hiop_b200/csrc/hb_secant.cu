@@ -106,7 +106,10 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
 {
   HB_REQUIRE(k && (k->n == 0 || (x && grad_f)), "hb_lowrank_secant_update: null argument");
   HB_REQUIRE(k->sec_S, "hb_lowrank_secant_update: call hb_lowrank_secant_reset first");
-  HB_REQUIRE(k->m == 0 || k->J, "hb_lowrank_secant_update: register the current Jacobian with hb_lowrank_set_jacobian first");
+  HB_REQUIRE(jac_set(k), "hb_lowrank_secant_update: register the current Jacobian with hb_lowrank_set_jacobian first");
+  HB_REQUIRE(jacobian_is_constant || k->m == 0 || !k->panel_cols,
+             "hb_lowrank_secant_update: with a host-resident Jacobian only jacobian_is_constant != 0 is supported (J_prev would need a second "
+             "host array)");
   HB_REQUIRE((k->meq == 0 || yc) && (k->mineq == 0 || yd), "hb_lowrank_secant_update: null multiplier block");
   hb_ctx* c = k->ctx;
   const long long n = k->n;

@@ -243,6 +243,15 @@ class KKTLinSysLowRank:
         self._keep["jac"] = (Jc, Jd)
         check(self.ctx.L.hb_lowrank_set_jacobian(self.h, _ptr(Jc), _ptr(Jd)), "hb_lowrank_set_jacobian")
 
+    def set_jacobian_host(self, Jc, Jd, panel_cols: int = 0):
+        """Registers a Jacobian kept in page-locked host memory (pinned CPU float64 tensors, borrowed until the next set_jacobian*);
+        every pass over J streams it through device panels of panel_cols columns (0: about 128 MB each)."""
+        for t in (Jc, Jd):
+            if t is not None and t.numel():
+                assert t.device.type == "cpu" and t.is_pinned(), "set_jacobian_host takes pinned CPU tensors"
+        self._keep["jac"] = (Jc, Jd)
+        check(self.ctx.L.hb_lowrank_set_jacobian_host(self.h, _ptr(Jc), _ptr(Jd), int(panel_cols)), "hb_lowrank_set_jacobian_host")
+
     def set_secant(self, sigma: float, St, Yt, L: np.ndarray, D: np.ndarray):
         l = 0 if St is None else St.shape[0]
         self._keep["sec"] = (St, Yt)

@@ -79,6 +79,9 @@ int hb_malloc(hb_ctx* ctx, size_t bytes, void** dptr);
 int hb_free(hb_ctx* ctx, void* dptr);
 int hb_malloc_host(hb_ctx* ctx, size_t bytes, void** hptr); /* pinned */
 int hb_free_host(hb_ctx* ctx, void* hptr);
+/* page-locks (cudaHostRegister) / releases caller-allocated host memory, e.g. a Jacobian for hb_lowrank_set_jacobian_host */
+int hb_host_register(hb_ctx* ctx, void* hptr, size_t bytes);
+int hb_host_unregister(hb_ctx* ctx, void* hptr);
 int hb_memcpy_h2d(hb_ctx* ctx, void* dst_dev, const void* src_host, size_t bytes); /* async on the ctx stream */
 int hb_memcpy_d2h(hb_ctx* ctx, void* dst_host, const void* src_dev, size_t bytes); /* async on the ctx stream */
 int hb_memcpy_d2d(hb_ctx* ctx, void* dst_dev, const void* src_dev, size_t bytes);
@@ -201,6 +204,17 @@ int hb_lowrank_set_patterns(hb_lowrank* k, const double* ixl, const double* ixu,
  * the next call. If Jd == Jc + m_eq*n_local the engine uses [Jc;Jd] in place (no copy; the reference copies m x n
  * doubles per solve, hiopKKTLinSys.cpp:1127-1128), otherwise it packs them into an internal m x n_local buffer. */
 int hb_lowrank_set_jacobian(hb_lowrank* k, const double* Jc, const double* Jd);
+/* The same Jacobian kept in HOST memory, for a J (8 m n_local bytes) that does not fit in device memory. Jc_host (m_eq x n_local)
+ * and Jd_host (m_ineq x n_local) are row-major with leading dimension n_local, in caller-owned page-locked memory (hb_malloc_host
+ * or cudaHostRegister; HB_ERR_INVALID otherwise), borrowed until the next hb_lowrank_set_jacobian* call. Every pass over J
+ * (condensation, J x, J^T y of the solve, the residual, BiCGStab and the LSQ duals) streams it through a ring of three device
+ * panels of m x panel_cols doubles: the copy of one panel overlaps the kernels on the previous ones. panel_cols <= 0 picks
+ * panels of about 128 MB; otherwise it is rounded up to a multiple of 2048 columns. Results: J x, J^T y and everything built on
+ * them only (residual, full-KKT operator) are bit-identical to a 16-byte aligned device J; N and the directions agree to rounding
+ * (the condensation adds the panels' partial products in panel order). Refused with HB_ERR_INVALID: the int8-slice condensation
+ * (modes 6-8; AUTO runs FP64) and hb_lowrank_secant_update with jacobian_is_constant == 0. hb_lowrank_set_jacobian returns the
+ * handle to a device J and releases the panels. */
+int hb_lowrank_set_jacobian_host(hb_lowrank* k, const double* Jc_host, const double* Jd_host, long long panel_cols);
 /* Compact-BFGS state as hiopHessianLowRank::update leaves it (hiopHessianLowRank.cpp:262-388): S_t, Y_t are l x n_local
  * row-major device arrays (borrowed); L (l x l row-major, strictly lower) and D (l) are HOST arrays (they are
  * "local" DEFAULT-space objects in the reference too, hiopHessianLowRank.cpp:85-87); sigma = B0 scaling. */
