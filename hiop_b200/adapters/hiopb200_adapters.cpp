@@ -349,7 +349,7 @@ bool hiopKKTLinSysLowRankB200::update(const hiopIterate* iter, const hiopVector*
   if(!ok(hb_lowrank_update(h_, dit_[0], dit_[1], dit_[2], dit_[3], dit_[4], dit_[5], dit_[6], dit_[7]), "hb_lowrank_update", &healthy_)) return false;
   // N and its factor depend only on the state set above: condense ONCE per update(); every preconditioner apply of the
   // outer BiCGStab then reuses it (the reference rebuilds and refactorizes N on each solveCompressed call).
-  // HB_ERR_NUMERIC (V singular / N not SPD, after the engine's own FP64 retry) is the reference's "update failed": return false and let
+  // HB_ERR_NUMERIC (V singular / N not SPD; the engine does not retry) is the reference's "update failed": return false and let
   // the driver escalate (hiopAlgFilterIPM.cpp:1216-1229); the adapter stays usable.
   TR("update: condense");
   const int rc = hb_lowrank_condense(h_);

@@ -379,25 +379,6 @@ __global__ void k_fused_rhs(int m, int meq, int l, double sigma, const double* _
 } // namespace
 
 // =============================================================================================================
-int refresh_rowptr(hb_lowrank* k)
-{
-  if(!k->rowptr_dirty) return HB_OK;
-  hb_ctx* c = k->ctx;
-  const int Ma = k->m + 2 * k->l;
-  bool al = true;
-  for(int i = 0; i < k->m; i++) k->rowptr_host[i] = k->J + (size_t)i * k->n;
-  for(int q = 0; q < k->l; q++) {
-    k->rowptr_host[k->m + q] = k->St + (size_t)q * k->n;
-    k->rowptr_host[k->m + k->l + q] = k->Yt + (size_t)q * k->n;
-  }
-  for(int i = 0; i < Ma; i++) al = al && ((reinterpret_cast<uintptr_t>(k->rowptr_host[i]) & 15u) == 0);
-  k->rows_aligned = al;
-  HB_CUDA(cudaMemcpyAsync(k->rowptr_dev, k->rowptr_host, sizeof(double*) * Ma, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream)); // rowptr_host may be rewritten by the next set_* call
-  k->rowptr_dirty = false;
-  return HB_OK;
-}
-
 // p = V^{-1} [sigma*S (w.x); Y (w.x)] style multi-dot into k->p2l (device), all-reduced
 int multidot(hb_lowrank* k, const double* w, const double* x, double sigma_s)
 {
@@ -458,173 +439,127 @@ int gemv_cols_launch(hb_ctx* c, int rg, int m, long long n, const double* A, lon
   return HB_OK;
 }
 
-} // namespace
-
-int gemv_rows(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x)
-{
-  if(m == 0) return HB_OK;
-  const int nchunks = (int)((n + GR_CHUNK - 1) / GR_CHUNK);
-  HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)(nchunks > 0 ? nchunks : 1) * m));
-  HB_CHECK(gemv_rows_partial(c, m, n, A, lda, x, (double*)c->ws));
-  return gemv_rows_final(c, m, n, (const double*)c->ws, beta, y, alpha);
-}
-
-int gemv_cols(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x)
-{
-  return gemv_cols_launch(c, gemv_cols_groups(c, m, n), m, n, A, lda, beta, y, alpha, x);
-}
-
 // ---- the Jacobian in column chunks --------------------------------------------------------------------------------------------
-namespace {
-
-// Column chunks [q csz, q csz + w) of the host rows Jc, Jd (ld = n) and where each lands on the device: slot q % HB_PANEL_RING of the
-// panel ring of a host-resident J (leading dimension k->panel_ld), or its own columns of k->hJ (hb_lowrank_kkt_system_host, ld = n).
-struct jac_chunks
-{
-  const double *Jc, *Jd;
-  long long csz;
-  int nch;
-  bool ring;
-};
-
-jac_chunks host_chunks(const hb_lowrank* k)
-{
-  return {k->Jc_host, k->Jd_host, k->panel_cols, (int)((k->n + k->panel_cols - 1) / k->panel_cols), true};
-}
-
-const double* chunk_dst(const hb_lowrank* k, const jac_chunks& s, int q, long long* ld)
-{
-  *ld = s.ring ? k->panel_ld : k->n;
-  return s.ring ? k->panel[q % HB_PANEL_RING].get() : k->hJ + q * s.csz;
-}
 
 // timing-enabled cudaEventRecord between the kernels serialises the compute stream against the copy engine (with
-// hb_ctx_enable_timing the first kernel starts only when the last copy has ended): off while chunks stream
+// hb_ctx_enable_timing the first kernel starts only when the last copy has ended): off while chunks are copied
 struct timing_off
 {
   hb_ctx* c;
   bool saved;
-  explicit timing_off(hb_ctx* ctx) : c(ctx), saved(ctx->timing) { c->timing = false; }
+  timing_off(hb_ctx* ctx, bool off) : c(ctx), saved(ctx->timing) { c->timing = saved && !off; }
   ~timing_off() { c->timing = saved; }
 };
 
-// Copies the chunks of J on k->copy_stream and calls consume(q, c0, w, P, ld) on the context stream once chunk q (columns c0 .. c0+w-1,
-// m rows at P with leading dimension ld) has landed. Copies run `lookahead` chunks ahead of the consumers. They are submitted only that
-// far ahead: if the two streams ever share a hardware work queue (CUDA_DEVICE_MAX_CONNECTIONS) commands run in submission order, and
-// "all copies, then all kernels" would serialise. A ring slot is overwritten only after the context stream has finished with the chunk
-// it held (lookahead <= HB_PANEL_RING - 1).
+// Calls consume(q, c0, w, P, ld) on the context stream for every chunk q of k->jl: columns c0 .. c0+w-1, m rows at P with leading
+// dimension ld. A layout with host rows copies chunk q on k->copy_stream first, `lookahead` chunks ahead of the consumers. Copies are
+// submitted only that far ahead: if the two streams ever share a hardware work queue (CUDA_DEVICE_MAX_CONNECTIONS) commands run in
+// submission order, and "all copies, then all kernels" would serialise. A reused slot is overwritten only after the context stream
+// has finished with the chunk it held (lookahead <= slots - 1); the copy events are reused four chunks apart (lookahead <= 3).
 template <class F>
-int stream_chunks(hb_lowrank* k, const jac_chunks& s, F&& consume)
+int stream_chunks(hb_lowrank* k, F&& consume)
 {
   hb_ctx* c = k->ctx;
+  const hb_jac_layout& L = k->jl;
   const long long n = k->n;
   const int meq = k->meq, mi = k->mineq;
-  const int lookahead = s.ring ? HB_PANEL_RING - 1 : 3;
-  static_assert(HB_PANEL_RING - 1 <= 3, "the copy events are reused four chunks apart");
-  HB_CHECK(k->copy_stream.create(cudaStreamNonBlocking));
-  HB_CHECK(k->copy_start.create(cudaEventDisableTiming));
-  for(hb_event& e : k->chunk_ev) HB_CHECK(e.create(cudaEventDisableTiming));
-  if(s.ring)
-    for(hb_event& e : k->panel_free) HB_CHECK(e.create(cudaEventDisableTiming));
-  // the copies start after everything enqueued so far on the context stream: its uploads, and the last reads of the ring
-  HB_CUDA(cudaEventRecord(k->copy_start, c->stream));
-  HB_CUDA(cudaStreamWaitEvent(k->copy_stream, k->copy_start, 0));
+  const bool copy = L.from_host();
+  const int lookahead = std::max(1, std::min(3, L.slots - 1));
+  auto width = [&](int q) { return q * L.csz + L.csz <= n ? L.csz : n - q * L.csz; };
   auto submit_copy = [&](int q) -> int {
-    const long long c0 = q * s.csz, w = (c0 + s.csz <= n ? s.csz : n - c0);
-    long long ld;
-    double* P = const_cast<double*>(chunk_dst(k, s, q, &ld));
-    if(s.ring && q >= HB_PANEL_RING) HB_CUDA(cudaStreamWaitEvent(k->copy_stream, k->panel_free[q % HB_PANEL_RING], 0));
+    const long long c0 = q * L.csz, w = width(q);
+    double* P = const_cast<double*>(L.chunk(q));
+    if(q >= L.slots) HB_CUDA(cudaStreamWaitEvent(k->copy_stream, k->slot_free[q % L.slots], 0));
     if(meq)
-      HB_CUDA(cudaMemcpy2DAsync(P, sizeof(double) * ld, s.Jc + c0, sizeof(double) * n, sizeof(double) * w, meq, cudaMemcpyHostToDevice, k->copy_stream));
+      HB_CUDA(cudaMemcpy2DAsync(P, sizeof(double) * L.ld, L.Jc + c0, sizeof(double) * n, sizeof(double) * w, meq, cudaMemcpyHostToDevice, k->copy_stream));
     if(mi)
-      HB_CUDA(cudaMemcpy2DAsync(P + (size_t)meq * ld, sizeof(double) * ld, s.Jd + c0, sizeof(double) * n, sizeof(double) * w, mi, cudaMemcpyHostToDevice,
-                                k->copy_stream));
+      HB_CUDA(cudaMemcpy2DAsync(P + (size_t)meq * L.ld, sizeof(double) * L.ld, L.Jd + c0, sizeof(double) * n, sizeof(double) * w, mi,
+                                cudaMemcpyHostToDevice, k->copy_stream));
     HB_CUDA(cudaEventRecord(k->chunk_ev[q % 4], k->copy_stream));
     return HB_OK;
   };
-  for(int q = 0; q < s.nch && q < lookahead; q++) HB_CHECK(submit_copy(q));
-  timing_off off(c);
-  for(int q = 0; q < s.nch; q++) {
-    const long long c0 = q * s.csz, w = (c0 + s.csz <= n ? s.csz : n - c0);
-    long long ld;
-    const double* P = chunk_dst(k, s, q, &ld);
-    HB_CUDA(cudaStreamWaitEvent(c->stream, k->chunk_ev[q % 4], 0));
-    HB_CHECK(consume(q, c0, w, P, ld));
-    if(s.ring) HB_CUDA(cudaEventRecord(k->panel_free[q % HB_PANEL_RING], c->stream));
-    if(q + lookahead < s.nch) HB_CHECK(submit_copy(q + lookahead));
+  if(copy) {
+    HB_CHECK(k->copy_stream.create(cudaStreamNonBlocking));
+    HB_CHECK(k->copy_start.create(cudaEventDisableTiming));
+    for(hb_event& e : k->chunk_ev) HB_CHECK(e.create(cudaEventDisableTiming));
+    if(L.slots < L.nch)
+      for(hb_event& e : k->slot_free) HB_CHECK(e.create(cudaEventDisableTiming));
+    // the copies start after everything enqueued so far on the context stream: its uploads, and the last reads of the slots
+    HB_CUDA(cudaEventRecord(k->copy_start, c->stream));
+    HB_CUDA(cudaStreamWaitEvent(k->copy_stream, k->copy_start, 0));
+    for(int q = 0; q < L.nch && q < lookahead; q++) HB_CHECK(submit_copy(q));
+  }
+  timing_off off(c, copy);
+  for(int q = 0; q < L.nch; q++) {
+    if(copy) HB_CUDA(cudaStreamWaitEvent(c->stream, k->chunk_ev[q % 4], 0));
+    HB_CHECK(consume(q, q * L.csz, width(q), L.chunk(q), L.ld));
+    if(copy && q + L.slots < L.nch) HB_CUDA(cudaEventRecord(k->slot_free[q % L.slots], c->stream));
+    if(copy && q + lookahead < L.nch) HB_CHECK(submit_copy(q + lookahead));
   }
   return HB_OK;
 }
 
-// k->chunk_rowptr_dev: per chunk, the rows of [J; S; Y] restricted to its columns (rebuilt only when the layout changed)
-int chunk_table(hb_lowrank* k, const jac_chunks& s)
+// The rows of [J; S; Y] restricted to the columns of each chunk of k->jl (nch x (m + 2 l) pointers). A rebuild costs a host
+// synchronisation, so the tables of the last two layouts are kept: hb_lowrank_kkt_system_host condenses a staged upload and then
+// runs on the device J it leaves.
+int jac_table(hb_lowrank* k, const hb_rowtab** out)
 {
   hb_ctx* c = k->ctx;
+  const hb_jac_layout& L = k->jl;
   const int m = k->m, l = k->l, Ma = m + 2 * l;
-  long long ld;
-  const long long key[8] = {(long long)(uintptr_t)chunk_dst(k, s, 0, &ld), ld, s.csz, s.nch, Ma, (long long)(uintptr_t)k->St, (long long)(uintptr_t)k->Yt,
-                            (long long)k->n};
-  if(!memcmp(key, k->chunk_key, sizeof(key))) return HB_OK;
-  memset(k->chunk_key, 0, sizeof(k->chunk_key));
-  HB_CHECK(k->chunk_rowptr_dev.reserve(c, (size_t)s.nch * Ma, "chunk row pointers"));
-  HB_CHECK(k->chunk_rowptr_host.reserve(c, (size_t)s.nch * Ma, "chunk row pointers"));
-  bool al = true;
-  for(int q = 0; q < s.nch; q++) {
-    const long long c0 = q * s.csz;
-    const double* P = chunk_dst(k, s, q, &ld);
-    const double** row = k->chunk_rowptr_host + (size_t)q * Ma;
-    for(int i = 0; i < m; i++) row[i] = P + (size_t)i * ld;
-    for(int j = 0; j < l; j++) {
-      row[m + j] = k->St + (size_t)j * k->n + c0;
-      row[m + l + j] = k->Yt + (size_t)j * k->n + c0;
+  const long long key[9] = {(long long)(uintptr_t)L.base, L.stride, L.slots, L.ld, L.csz, L.nch, l, (long long)(uintptr_t)k->St,
+                            (long long)(uintptr_t)k->Yt};
+  if(memcmp(key, k->rows[0].key, sizeof(key))) std::swap(k->rows[0], k->rows[1]);
+  hb_rowtab& t = k->rows[0];
+  if(memcmp(key, t.key, sizeof(key))) { // neither: the older table is rebuilt
+    memset(t.key, 0, sizeof(t.key));
+    HB_CHECK(t.dev.reserve(c, (size_t)L.nch * Ma, "row pointers"));
+    HB_CHECK(t.host.reserve(c, (size_t)L.nch * Ma, "row pointers"));
+    bool al = true;
+    for(int q = 0; q < L.nch; q++) {
+      const long long c0 = q * L.csz;
+      const double** row = t.host + (size_t)q * Ma;
+      for(int i = 0; i < m; i++) row[i] = L.chunk(q) + (size_t)i * L.ld;
+      for(int j = 0; j < l; j++) {
+        row[m + j] = k->St + (size_t)j * k->n + c0;
+        row[m + l + j] = k->Yt + (size_t)j * k->n + c0;
+      }
+      for(int i = 0; i < Ma; i++) al = al && ((reinterpret_cast<uintptr_t>(row[i]) & 15u) == 0);
     }
-    for(int i = 0; i < Ma; i++) al = al && ((reinterpret_cast<uintptr_t>(row[i]) & 15u) == 0);
+    HB_CUDA(cudaMemcpyAsync(t.dev, t.host, sizeof(double*) * (size_t)L.nch * Ma, cudaMemcpyHostToDevice, c->stream));
+    HB_CUDA(cudaStreamSynchronize(c->stream)); // the host table is rewritten by a later rebuild
+    t.aligned = al;
+    memcpy(t.key, key, sizeof(key));
   }
-  HB_CUDA(cudaMemcpyAsync(k->chunk_rowptr_dev, k->chunk_rowptr_host, sizeof(double*) * (size_t)s.nch * Ma, cudaMemcpyHostToDevice, c->stream));
-  HB_CUDA(cudaStreamSynchronize(c->stream)); // chunk_rowptr_host is rewritten by the next layout
-  k->chunk_rows_aligned = al;
-  memcpy(k->chunk_key, key, sizeof(key));
+  *out = &t;
   return HB_OK;
-}
-
-// C = R diag(d) R^T, R = the first M rows of [J; S; Y], chunk by chunk: the partial products (and fused row dots) are added in chunk
-// order, so the result does not depend on timing
-int syrk_chunks(hb_lowrank* k, const jac_chunks& s, int M, const double* d, double* C, const double* fuse_rx, double* tdot)
-{
-  hb_ctx* c = k->ctx;
-  const size_t Mmax = (size_t)k->m + 2 * k->lmax;
-  HB_CHECK(k->Ctmp.reserve(c, Mmax * Mmax + Mmax, "partial C_aug"));
-  HB_CHECK(chunk_table(k, s));
-  const int Ma = k->m + 2 * k->l;
-  double* Ct = k->Ctmp;
-  double* tt = Ct + (size_t)M * M;
-  return stream_chunks(k, s, [&](int q, long long c0, long long w, const double*, long long) -> int {
-    // every chunk starts at a multiple of 64 columns: its rows keep the 16-byte alignment of the whole rows
-    HB_CHECK(hb_syrk_rows(c, M, w, k->chunk_rowptr_dev + (size_t)q * Ma, k->chunk_rows_aligned, d ? d + c0 : nullptr, q == 0 ? C : Ct, M,
-                          fuse_rx ? fuse_rx + c0 : nullptr, tdot ? (q == 0 ? tdot : tt) : nullptr));
-    if(q > 0) {
-      HB_CHECK(hb_vec_axpy(c, (long long)M * M, C, 1.0, Ct));
-      if(tdot) HB_CHECK(hb_vec_axpy(c, M, tdot, 1.0, tt));
-    }
-    return HB_OK;
-  });
 }
 
 } // namespace
 
-bool jac_set(const hb_lowrank* k) { return k->m == 0 || k->J || k->panel_cols > 0; }
+bool jac_set(const hb_lowrank* k) { return k->m == 0 || k->jl.base; }
+
+int jac_whole(hb_lowrank* k, const char* who, const double** J, const hb_rowtab** rows)
+{
+  if(k->jl.from_host()) {
+    snprintf(g_hb_err, sizeof(g_hb_err), "%s needs the whole Jacobian on the device (hb_lowrank_set_jacobian); this one is streamed from host memory",
+             who);
+    return HB_ERR_INVALID;
+  }
+  if(J) *J = k->jl.base;
+  return rows ? jac_table(k, rows) : HB_OK;
+}
 
 int jac_rows(hb_lowrank* k, double beta, double* y, double alpha, const double* x)
 {
   hb_ctx* c = k->ctx;
   const int m = k->m;
-  if(!k->panel_cols) return gemv_rows(c, m, k->n, k->J, k->n, beta, y, alpha, x);
   if(m == 0) return HB_OK;
-  // every panel starts at a multiple of GR_CHUNK columns: its partials are the ones of the same chunks of the whole J, written in place
+  // every chunk starts at a multiple of GR_CHUNK columns: its partials are the ones of the same columns of the whole J, written in place
   const long long nchunks = (k->n + GR_CHUNK - 1) / GR_CHUNK;
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)(nchunks > 0 ? nchunks : 1) * m));
   double* partial = c->ws;
-  HB_CHECK(stream_chunks(k, host_chunks(k), [&](int, long long c0, long long w, const double* P, long long ld) -> int {
+  HB_CHECK(stream_chunks(k, [&](int, long long c0, long long w, const double* P, long long ld) -> int {
     return gemv_rows_partial(c, m, w, P, ld, x + c0, partial + (size_t)(c0 / GR_CHUNK) * m);
   }));
   return gemv_rows_final(c, m, k->n, partial, beta, y, alpha);
@@ -634,19 +569,35 @@ int jac_cols(hb_lowrank* k, double beta, double* y, double alpha, const double* 
 {
   hb_ctx* c = k->ctx;
   const int m = k->m;
-  if(!k->panel_cols) return gemv_cols(c, m, k->n, k->J, k->n, beta, y, alpha, x);
-  // the row groups the whole J would use: each column then sums its rows in the same order
+  // the row groups the whole J selects: each column then sums its rows in the same order
   const int rg = gemv_cols_groups(c, m, k->n);
-  return stream_chunks(k, host_chunks(k), [&](int, long long c0, long long w, const double* P, long long ld) -> int {
+  return stream_chunks(k, [&](int, long long c0, long long w, const double* P, long long ld) -> int {
     return gemv_cols_launch(c, rg, m, w, P, ld, beta, y + c0, alpha, x);
   });
 }
 
+// C = R diag(d) R^T, R = the first M rows of [J; S; Y], chunk by chunk: the partial products of later chunks (and their fused row
+// dots) are added in chunk order, so the result does not depend on timing
 int jac_syrk(hb_lowrank* k, int M, const double* d, double* C, const double* fuse_rx, double* tdot)
 {
-  if(k->panel_cols) return syrk_chunks(k, host_chunks(k), M, d, C, fuse_rx, tdot);
-  HB_CHECK(refresh_rowptr(k));
-  return hb_syrk_rows(k->ctx, M, k->n, k->rowptr_dev, k->rows_aligned, d, C, M, fuse_rx, tdot);
+  hb_ctx* c = k->ctx;
+  const size_t Mmax = (size_t)k->m + 2 * k->lmax;
+  if(k->jl.nch > 1) HB_CHECK(k->Ctmp.reserve(c, Mmax * Mmax + Mmax, "partial C_aug"));
+  const hb_rowtab* rows;
+  HB_CHECK(jac_table(k, &rows));
+  const int Ma = k->m + 2 * k->l;
+  double* Ct = k->Ctmp;
+  double* tt = Ct ? Ct + (size_t)M * M : nullptr;
+  return stream_chunks(k, [&](int q, long long c0, long long w, const double*, long long) -> int {
+    // every chunk starts at a multiple of 64 columns: its rows keep the 16-byte alignment of the whole rows
+    HB_CHECK(hb_syrk_rows(c, M, w, rows->dev + (size_t)q * Ma, rows->aligned, d ? d + c0 : nullptr, q == 0 ? C : Ct, M,
+                          fuse_rx ? fuse_rx + c0 : nullptr, tdot ? (q == 0 ? tdot : tt) : nullptr));
+    if(q > 0) {
+      HB_CHECK(hb_vec_axpy(c, (long long)M * M, C, 1.0, Ct));
+      if(tdot) HB_CHECK(hb_vec_axpy(c, M, tdot, 1.0, tt));
+    }
+    return HB_OK;
+  });
 }
 
 namespace {
@@ -679,9 +630,6 @@ int do_condense_async(hb_lowrank* k, const double* fuse_rx = nullptr)
   // AUTO = exact FP64 DMMA: on H100 (700 W) at n = 1e6, m = 1000 the int8-slice GEMM takes as long as the DMMA kernel (37.4 against
   // 38.1 ms) and the row-maximum and slicing passes over J come on top (step 49.9 against 44.4 ms), so the emulation runs only on request
   const int mode = k->condense_mode < 0 ? 0 : k->condense_mode;
-  HB_REQUIRE(mode == 0 || !k->panel_cols, "hb_lowrank_condense: the int8-slice condensation (modes 6-8) needs the Jacobian on the device; "
-                                          "a host-resident Jacobian is condensed in FP64 (mode 0 or -1)");
-  if(!k->panel_cols) HB_CHECK(refresh_rowptr(k));
   HB_CHECK(condense_enqueue(k, mode, fuse_rx));
   k->check_pending = true;
   k->cond_valid = true; // optimistic: a failure is reported by the next synchronous call (hb_lowrank_check / hb_lowrank_condense)
@@ -724,17 +672,19 @@ int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
   const int m = k->m, l = k->l, Ma = m + 2 * l;
   k->tdot_valid = false;
   if(Ma > 0) {
-    k->condense_used = mode;
     if(mode == 0) {
       const bool fuse = fuse_rx && m > 0 && hb_syrk_extra_row_is_free(Ma) && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
       HB_CHECK(jac_syrk(k, Ma, k->DhInv, k->Caug, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
       k->tdot_valid = fuse;
     } else {
+      const hb_rowtab* rows;
+      HB_CHECK(jac_whole(k, "hb_lowrank_condense: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)", nullptr, &rows));
       const bool fuse = fuse_rx && m > 0;
       if(fuse && k->n == 0) HB_CUDA(cudaMemsetAsync(k->tdot, 0, sizeof(double) * Ma, c->stream));
-      HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, k->rowptr_dev, k->rows_aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
+      HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
       k->tdot_valid = fuse;
     }
+    k->condense_used = mode;
   }
   return condense_finish(k);
 }
@@ -784,6 +734,15 @@ int condense_finish(hb_lowrank* k)
   return HB_OK;
 }
 
+// a device J: one chunk of all n columns at J (ld n)
+hb_jac_layout device_layout(long long n, const double* J)
+{
+  hb_jac_layout L;
+  L.csz = L.ld = n;
+  L.base = J;
+  return L;
+}
+
 } // namespace
 
 extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_ineq, int l_max, hb_lowrank** out)
@@ -792,6 +751,7 @@ extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_i
   HB_CUDA(cudaSetDevice(c->device));
   std::unique_ptr<hb_lowrank> k(new hb_lowrank);
   k->ctx = c; k->n = n_local; k->meq = m_eq; k->mineq = m_ineq; k->m = m_eq + m_ineq; k->lmax = l_max;
+  k->jl = device_layout(n_local, nullptr);
   if(const char* e = getenv("HB_CONDENSE")) { // "oz6" | "oz7" | "oz8" | "dmma"
     if(e[0] == 'o' && e[1] == 'z' && e[2] >= '6' && e[2] <= '8') k->condense_mode = e[2] - '0';
     else if(e[0] == 'd') k->condense_mode = 0;
@@ -816,8 +776,7 @@ extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_i
   HB_CHECK(k->mi1.reserve(c, m_ineq, "m_ineq scratch")); HB_CHECK(k->mi2.reserve(c, m_ineq, "m_ineq scratch"));
   HB_CHECK(k->ipivV.reserve(c, (size_t)l2 + 1, "pivots of V")); HB_CHECK(k->ipivM.reserve(c, (size_t)l2 + 1, "pivots of M"));
   HB_CHECK(k->info.reserve(c, 4, "info words"));
-  HB_CHECK(k->rowptr_dev.reserve(c, (size_t)Mamax + 2, "row pointers"));
-  HB_CHECK(k->rowptr_host.reserve(c, (size_t)Mamax + 2, "row pointers"));
+  HB_CHECK(k->sst_rows.dev.reserve(c, l_max, "row pointers")); HB_CHECK(k->sst_rows.host.reserve(c, l_max, "row pointers"));
   HB_CHECK(k->info_host.reserve(c, 4, "info words"));
   HB_CHECK(k->stats_host.reserve(c, 4, "solve statistics"));
   *out = k.release();
@@ -848,11 +807,9 @@ extern "C" int hb_lowrank_set_jacobian(hb_lowrank* k, const double* Jc, const do
   HB_REQUIRE(k, "null handle");
   HB_REQUIRE((Jc || k->meq == 0) && (Jd || k->mineq == 0), "hb_lowrank_set_jacobian: null Jacobian");
   hb_ctx* c = k->ctx;
-  if(k->panel_cols) { // back from a host-resident Jacobian: its panels are no longer needed
+  if(k->ring) { // back from a host-resident Jacobian: its slots are no longer needed
     HB_CUDA(cudaStreamSynchronize(c->stream));
-    for(hb_dev<double>& p : k->panel) p.reset();
-    k->panel_cols = k->panel_ld = 0;
-    k->Jc_host = k->Jd_host = nullptr;
+    k->ring.reset();
   }
   const double* J;
   if(k->meq == 0) J = Jd;
@@ -863,8 +820,7 @@ extern "C" int hb_lowrank_set_jacobian(hb_lowrank* k, const double* Jc, const do
     HB_CUDA(cudaMemcpyAsync(k->Jpack + (size_t)k->meq * k->n, Jd, sizeof(double) * (size_t)k->mineq * k->n, cudaMemcpyDeviceToDevice, c->stream));
     J = k->Jpack;
   }
-  if(J != k->J) k->rowptr_dirty = true;
-  k->J = J;
+  k->jl = device_layout(k->n, J);
   k->cond_valid = false;
   return HB_OK;
 }
@@ -896,23 +852,24 @@ extern "C" int hb_lowrank_set_jacobian_host(hb_lowrank* k, const double* Jc_host
   P = (P + GR_CHUNK - 1) / GR_CHUNK * GR_CHUNK;
   const long long Pmax = (n + GR_CHUNK - 1) / GR_CHUNK * GR_CHUNK;
   if(P > Pmax) P = Pmax > 0 ? Pmax : GR_CHUNK;
-  // the leading dimension has the parity of n: the gemv kernels then take the same (vector or scalar) path on a panel as on a device J
-  const long long ld = P + (n & 1);
-  const int slots = (int)std::min<long long>(HB_PANEL_RING, (n + P - 1) / P);
-  for(int s = 0; s < HB_PANEL_RING; s++) {
-    if(s < slots) HB_CHECK(k->panel[s].reserve(c, (size_t)m * ld, "a Jacobian panel"));
-    else if(k->panel[s]) {
-      HB_CUDA(cudaStreamSynchronize(c->stream));
-      k->panel[s].reset();
-    }
+  hb_jac_layout L;
+  L.csz = P;
+  L.nch = (int)((n + P - 1) / P);
+  L.slots = std::min(HB_PANEL_RING, L.nch);
+  // the leading dimension has the parity of n: the gemv kernels then take the same (vector or scalar) path on a panel as on a device
+  // J. The slots share one allocation, each starting 16-byte aligned, as the vector paths of the gemvs and k_syrk_ws require.
+  L.ld = P + (n & 1);
+  L.stride = (m * L.ld + 1) & ~1LL;
+  L.Jc = Jc_host;
+  L.Jd = Jd_host;
+  const size_t need = (size_t)L.slots * L.stride;
+  if(k->ring.capacity() > need) { // fewer or narrower slots than before: hold only these
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    k->ring.reset();
   }
-  memset(k->chunk_key, 0, sizeof(k->chunk_key)); // the chunk table points into the panels
-  k->Jc_host = Jc_host;
-  k->Jd_host = Jd_host;
-  k->panel_cols = P;
-  k->panel_ld = ld;
-  k->J = nullptr;
-  k->rowptr_dirty = true;
+  HB_CHECK(k->ring.reserve(c, need, "the Jacobian panels"));
+  L.base = k->ring;
+  k->jl = L;
   k->cond_valid = false;
   return HB_OK;
 }
@@ -923,7 +880,6 @@ extern "C" int hb_lowrank_set_secant(hb_lowrank* k, int l, double sigma, const d
   HB_REQUIRE(k && l >= 0 && l <= k->lmax, "hb_lowrank_set_secant: bad memory length");
   HB_REQUIRE(l == 0 || (St && Yt && L_host && D_host), "hb_lowrank_set_secant: null argument");
   hb_ctx* c = k->ctx;
-  if(l != k->l || St != k->St || Yt != k->Yt) k->rowptr_dirty = true;
   k->l = l; k->sigma = sigma; k->St = St; k->Yt = Yt;
   k->cond_valid = false;
   k->mdir_valid = false;
@@ -932,15 +888,17 @@ extern "C" int hb_lowrank_set_secant(hb_lowrank* k, int l, double sigma, const d
     HB_CUDA(cudaMemcpyAsync(k->Ld, L_host, sizeof(double) * l * l, cudaMemcpyHostToDevice, c->stream));
     HB_CUDA(cudaMemcpyAsync(k->Dd_sec, D_host, sizeof(double) * l, cudaMemcpyHostToDevice, c->stream));
     HB_CUDA(cudaStreamSynchronize(c->stream)); // L_host / D_host are caller-owned pageable memory
-    // S S^T (l x l) -- depends only on the secant memory, not on the barrier diagonal
-    for(int q = 0; q < l; q++) k->rowptr_host[q] = St + (size_t)q * k->n;
+    // S S^T (l x l) -- depends only on the secant memory, not on the barrier diagonal; over whole rows, wherever J is
+    hb_rowtab& t = k->sst_rows;
     bool al = true;
-    for(int q = 0; q < l; q++) al = al && ((reinterpret_cast<uintptr_t>(k->rowptr_host[q]) & 15u) == 0);
-    HB_CUDA(cudaMemcpyAsync(k->rowptr_dev, k->rowptr_host, sizeof(double*) * l, cudaMemcpyHostToDevice, c->stream));
-    HB_CHECK(hb_syrk_rows(c, l, k->n, k->rowptr_dev, al, nullptr, k->SSt, l));
+    for(int q = 0; q < l; q++) {
+      t.host[q] = St + (size_t)q * k->n;
+      al = al && ((reinterpret_cast<uintptr_t>(t.host[q]) & 15u) == 0);
+    }
+    HB_CUDA(cudaMemcpyAsync(t.dev, t.host, sizeof(double*) * l, cudaMemcpyHostToDevice, c->stream));
+    HB_CHECK(hb_syrk_rows(c, l, k->n, t.dev, al, nullptr, k->SSt, l));
     HB_CHECK(hb_allreduce_sum(c, k->SSt, (long long)l * l));
     HB_CUDA(cudaStreamSynchronize(c->stream));
-    k->rowptr_dirty = true;
   }
   return HB_OK;
 }
@@ -972,8 +930,7 @@ extern "C" int hb_lowrank_update(hb_lowrank* k, const double* zl, const double* 
 extern "C" int hb_lowrank_set_condense_mode(hb_lowrank* k, int mode)
 {
   HB_REQUIRE(k && (mode == -1 || mode == 0 || mode == 6 || mode == 7 || mode == 8), "hb_lowrank_set_condense_mode: mode must be -1, 0, 6, 7 or 8");
-  HB_REQUIRE(mode <= 0 || !k->panel_cols, "hb_lowrank_set_condense_mode: the int8-slice modes 6-8 need a global row-maximum pass over the "
-                                          "Jacobian before slicing; a host-resident Jacobian is condensed in FP64 (mode 0 or -1)");
+  if(mode > 0) HB_CHECK(jac_whole(k, "hb_lowrank_set_condense_mode: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)"));
   k->condense_mode = mode;
   k->cond_valid = false;
   return HB_OK;
@@ -1157,10 +1114,10 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
     }
   const int m = k->m, Ma = m + 2 * k->l;
   const bool have_J = Jc_host || Jd_host;
-  // The 8 m n bytes of J dominate this call (PCIe). When they are large, J is uploaded in column chunks on a second stream and
-  // each chunk is condensed (exact FP64 DMMA kernel, which needs no global row scaling) while the next one is in flight; the
-  // partial C_aug are added in chunk order, so the result does not depend on timing.
-  static const size_t chunk_min_bytes = getenv("HB_HOST_CHUNK_MIN_BYTES") ? (size_t)atoll(getenv("HB_HOST_CHUNK_MIN_BYTES")) : ((size_t)256 << 20);
+  // The 8 m n bytes of J dominate this call (PCIe). From 256 MiB on, J is uploaded in column chunks on a second stream and each chunk
+  // is condensed (exact FP64 DMMA kernel, which needs no global row scaling) while the next one is in flight; the partial C_aug are
+  // added in chunk order, so the result does not depend on timing.
+  constexpr size_t chunk_min_bytes = (size_t)256 << 20;
   const bool chunked = have_J && Ma > 0 && (k->condense_mode <= 0) && (size_t)m * n * sizeof(double) >= chunk_min_bytes && n >= 2048;
   if(have_J) HB_CHECK(k->hJ.reserve(c, (size_t)k->m * n, "the staged Jacobian"));
   if(have_J && !chunked) {
@@ -1172,14 +1129,20 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   // Not chunked: the condensation stays pending so that solve_compressed below runs it with rx fused, exactly as a device-side
   // update + solveCompressed does; breakdowns are reported after the solve.
   if(chunked) {
-    // 16 chunks of a multiple of 64 columns, each landing in its own columns of k->hJ
+    // the staged layout for this one condensation: 16 chunks of a multiple of 64 columns, each copied into its own columns of k->hJ;
+    // J is then whole on the device for the solve
     constexpr int NCH = 16;
-    const long long csz = ((n + NCH - 1) / NCH + 63) & ~63LL;
-    k->condense_used = 0;
-    HB_CHECK(syrk_chunks(k, {Jc_host, Jd_host, csz, (int)((n + csz - 1) / csz), false}, Ma, k->DhInv, k->Caug, nullptr, nullptr));
-    HB_CHECK(condense_finish(k));
-    k->check_pending = true;
-    k->cond_valid = true;
+    hb_jac_layout staged;
+    staged.csz = staged.stride = ((n + NCH - 1) / NCH + 63) & ~63LL;
+    staged.nch = staged.slots = (int)((n + staged.csz - 1) / staged.csz);
+    staged.base = k->hJ;
+    staged.ld = n;
+    staged.Jc = Jc_host;
+    staged.Jd = Jd_host;
+    std::swap(k->jl, staged);
+    const int rc = do_condense_async(k);
+    std::swap(k->jl, staged);
+    HB_CHECK(rc);
     HB_CHECK(condense_check(k));
   }
   HB_CHECK(hb_lowrank_solve_compressed(k, k->hbuf[8], k->hbuf[9], k->hbuf[10], k->hbuf[11], k->hbuf[12], k->hbuf[13]));
@@ -1195,11 +1158,15 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
 extern "C" int hb_mat_times_vec(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x)
 {
   HB_REQUIRE(c && m >= 0 && n >= 0 && lda >= n, "hb_mat_times_vec: bad arguments");
-  return gemv_rows(c, m, n, A, lda, beta, y, alpha, x);
+  if(m == 0) return HB_OK;
+  const int nchunks = (int)((n + GR_CHUNK - 1) / GR_CHUNK);
+  HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)(nchunks > 0 ? nchunks : 1) * m));
+  HB_CHECK(gemv_rows_partial(c, m, n, A, lda, x, (double*)c->ws));
+  return gemv_rows_final(c, m, n, (const double*)c->ws, beta, y, alpha);
 }
 extern "C" int hb_mat_trans_times_vec(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha,
                                       const double* x)
 {
   HB_REQUIRE(c && m >= 0 && n >= 0 && lda >= n, "hb_mat_trans_times_vec: bad arguments");
-  return gemv_cols(c, m, n, A, lda, beta, y, alpha, x);
+  return gemv_cols_launch(c, gemv_cols_groups(c, m, n), m, n, A, lda, beta, y, alpha, x);
 }

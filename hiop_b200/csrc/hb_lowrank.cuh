@@ -3,7 +3,32 @@
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
 
-constexpr int HB_PANEL_RING = 3; // device panels of a host-resident Jacobian
+constexpr int HB_PANEL_RING = 3; // device slots of a host-resident Jacobian
+
+// Where the columns of J = [Jc; Jd] (m x n) are during a pass over them: nch chunks of csz columns (the last one may be narrower).
+// Chunk q is read from slot q % slots at base + (q % slots) * stride, leading dimension ld. With host rows Jc, Jd (ld n), every pass
+// copies chunk q into its slot first; without, the slots hold J itself.
+//   device J (hb_lowrank_set_jacobian):          one chunk of all n columns, the slot is J, ld n
+//   host J (hb_lowrank_set_jacobian_host):       P columns per chunk, HB_PANEL_RING slots of one allocation, ld P + (n mod 2)
+//   staged upload (hb_lowrank_kkt_system_host): slot q at hJ + q csz, ld n, for its condensation; a device J on hJ after it
+struct hb_jac_layout
+{
+  long long csz = 0, stride = 0, ld = 0;
+  int nch = 1, slots = 1;
+  const double* base = nullptr;
+  const double *Jc = nullptr, *Jd = nullptr;
+  bool from_host() const { return Jc || Jd; }
+  const double* chunk(int q) const { return base + (q % slots) * stride; }
+};
+
+// a device table of row pointers (hb_syrk_rows) and what it was built from
+struct hb_rowtab
+{
+  hb_dev<const double*> dev;
+  hb_pinned<const double*> host;
+  long long key[9] = {0};
+  bool aligned = false; // every row is 16-byte aligned
+};
 
 struct hb_lowrank
 {
@@ -13,14 +38,20 @@ struct hb_lowrank
   double sigma = 1.0;
   // borrowed
   const double *ixl = nullptr, *ixu = nullptr, *idl = nullptr, *idu = nullptr;
-  const double *J = nullptr, *St = nullptr, *Yt = nullptr;
+  const double *St = nullptr, *Yt = nullptr;
   const double *zl = nullptr, *sxl = nullptr, *zu = nullptr, *sxu = nullptr, *vl = nullptr, *sdl = nullptr, *vu = nullptr, *sdu = nullptr;
   // owned
   hb_dev<double> Dx, DhInv, Dd, Dd_inv;
-  hb_dev<double> Jpack;
-  hb_dev<const double*> rowptr_dev;
-  hb_pinned<const double*> rowptr_host;
-  bool rows_aligned = false, rowptr_dirty = true;
+  // the Jacobian: where its columns are, and what the handle holds of it (the packed copy of a device J given as separate Jc and Jd,
+  // the staged upload of hb_lowrank_kkt_system_host, the slots of a host J)
+  hb_jac_layout jl;
+  hb_dev<double> Jpack, hJ, ring;
+  hb_rowtab rows[2]; // the [J; S; Y] tables of the last two layouts, the last one used first (jac_table)
+  hb_rowtab sst_rows; // the l rows of S, for S S^T
+  // a pass that copies J from the host: the copy stream, its events, the partial C_aug (+ partial fused row dots) of one chunk
+  hb_stream copy_stream;
+  hb_event copy_start, chunk_ev[4], slot_free[HB_PANEL_RING];
+  hb_dev<double> Ctmp;
   hb_dev<double> Caug, SSt, Ld, Dd_sec, V, Mdir, U, Z;
   hb_dev<int> ipivV, ipivM, info; // info[0]: V, info[1]: N chol, info[2]: M
   hb_dev<double> Nmat, F, svec, rhs, dy, work, stats;
@@ -37,7 +68,6 @@ struct hb_lowrank
   bool tdot_valid = false;
   // host staging (hb_lowrank_kkt_system_host)
   hb_dev<double> hbuf[14];
-  hb_dev<double> hJ;
   hb_pinned<int> info_host;     // 4 ints
   hb_pinned<double> stats_host; // 4 doubles
   // BiCGStab workspace (hb_krylov.cu), allocated on first use
@@ -46,21 +76,6 @@ struct hb_lowrank
   // secant memory owned by the engine (hb_secant.cu): S_t, Y_t (lmax x n), previous iterate / gradient / Jacobian
   hb_dev<double> sec_S, sec_Y, sec_xprev, sec_gprev, sec_Jprev;
   double sec_L[64 * 64] = {0}, sec_D[64] = {0}; // host copies of L (row-major, stride l) and D; lmax <= 64 in this mode
-  // host-resident Jacobian (hb_lowrank_set_jacobian_host): borrowed page-locked rows of Jc and Jd (ld = n), streamed through a ring of
-  // device panels of panel_cols columns (leading dimension panel_ld); panel_cols == 0: J is on the device (k->J)
-  const double *Jc_host = nullptr, *Jd_host = nullptr;
-  long long panel_cols = 0, panel_ld = 0;
-  hb_dev<double> panel[HB_PANEL_RING];
-  hb_event panel_free[HB_PANEL_RING]; // the context stream is done with a ring slot
-  // column chunks of J copied on a second stream while the context stream consumes earlier ones: the condensation of
-  // hb_lowrank_kkt_system_host and every pass over a host-resident J
-  hb_stream copy_stream;
-  hb_event copy_start, chunk_ev[4];
-  hb_dev<double> Ctmp; // partial C_aug (+ partial fused row dots) of one chunk
-  hb_dev<const double*> chunk_rowptr_dev;
-  hb_pinned<const double*> chunk_rowptr_host; // rows of [J; S; Y] per chunk (chunks x (m + 2 l))
-  long long chunk_key[8] = {0};               // what chunk_rowptr_dev was built for
-  bool chunk_rows_aligned = false;
   hb_dev<double> Finv;  // 16 x 16 inverses of the diagonal of F (cooperative Cholesky / solve)
   hb_big big;           // look-ahead Cholesky of large condensed systems: panel stream, events, scratch
   hb_dev<double> lsq_M; // m x m LSQ matrix / Cholesky factor + 2 m-vectors (hb_lsq.cu)
@@ -68,22 +83,19 @@ struct hb_lowrank
   double sec_sigma0 = 1.0;
 };
 
-// The Jacobian gemvs (hb_lowrank.cu) for an m x n row-major A with leading dimension lda (elements), n = the local columns.
-// y = beta*y + alpha*A x, summed over the ranks (beta*y on rank 0 only)
-int gemv_rows(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
-// y = beta*y + alpha*A^T x over the local columns (no reduction)
-int gemv_cols(hb_ctx* c, int m, long long n, const double* A, long long lda, double beta, double* y, double alpha, const double* x);
-// The registered Jacobian J = [Jc; Jd] of a handle, on the device or streamed from the host in column panels (same results: the J x
-// partials are kept per 2048 columns and summed in one fixed order, each column of J^T y depends on its own column only).
+// The registered Jacobian J = [Jc; Jd] of a handle: every pass runs over the chunks of k->jl, one for a device J (same results for any
+// chunking: the J x partials are kept per 2048 columns and summed in one fixed order, each column of J^T y depends on its own column).
 bool jac_set(const hb_lowrank* k); // a Jacobian is registered (or m == 0)
-// y (m) = beta*y + alpha*J x, all-reduced like gemv_rows
+// y (m) = beta*y + alpha*J x, summed over the ranks (beta*y on rank 0 only)
 int jac_rows(hb_lowrank* k, double beta, double* y, double alpha, const double* x);
-// y (n) = beta*y + alpha*J^T x
+// y (n) = beta*y + alpha*J^T x over the local columns (no reduction)
 int jac_cols(hb_lowrank* k, double beta, double* y, double alpha, const double* x);
 // C (M x M, ldc = M) = R diag(d) R^T over the local columns, R = the first M rows of [J; S; Y]; FP64 DMMA (hb_syrk_rows), with its
 // fused extra row when fuse_rx is given (tdot, M doubles)
 int jac_syrk(hb_lowrank* k, int M, const double* d, double* C, const double* fuse_rx = nullptr, double* tdot = nullptr);
+// The whole J on the device, for the passes that cannot run chunk by chunk: the int8-slice condensation and LSQ matrix (a global
+// row-maximum pass comes first) and the J_prev update of the secant (a device copy of J). *J (m x n, ld n) and *rows (the table of
+// [J rows (m); S rows (l); Y rows (l)]) as asked for; HB_ERR_INVALID, naming `who`, for a J streamed from host memory.
+int jac_whole(hb_lowrank* k, const char* who, const double** J = nullptr, const hb_rowtab** rows = nullptr);
 // k->p2l (device, 2l doubles) = [sigma_s * S (w.*x); Y (w.*x)], all-reduced; w may be NULL
 int multidot(hb_lowrank* k, const double* w, const double* x, double sigma_s);
-// device table of row pointers [J rows (m); S rows (l); Y rows (l)] -> k->rowptr_dev, k->rows_aligned
-int refresh_rowptr(hb_lowrank* k);

@@ -50,11 +50,11 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   double* rhs = M + (size_t)m * m;
   // J J^T: rows 0..m-1 of the row-pointer table are the Jacobian rows
   const int mode = k->condense_mode < 0 ? 0 : k->condense_mode; // AUTO = exact FP64 DMMA, as for the condensation
-  HB_REQUIRE(mode == 0 || !k->panel_cols, "hb_lowrank_lsq_duals: the int8-slice modes 6-8 need the Jacobian on the device");
   if(mode == 0) HB_CHECK(jac_syrk(k, m, nullptr, M));
   else {
-    HB_CHECK(refresh_rowptr(k));
-    HB_CHECK(hb_syrk_rows_ozaki(c, m, n, k->rowptr_dev, k->rows_aligned, nullptr, M, m, mode, nullptr, nullptr));
+    const hb_rowtab* rows;
+    HB_CHECK(jac_whole(k, "hb_lowrank_lsq_duals: the int8-slice modes 6-8", nullptr, &rows));
+    HB_CHECK(hb_syrk_rows_ozaki(c, m, n, rows->dev, rows->aligned, nullptr, M, m, mode, nullptr, nullptr));
   }
   HB_CHECK(hb_allreduce_sum(c, M, (long long)m * m));
   // rhs = -J vecx (all-reduced), then the d-side terms on the replicated part

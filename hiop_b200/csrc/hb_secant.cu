@@ -107,20 +107,19 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
   HB_REQUIRE(k && (k->n == 0 || (x && grad_f)), "hb_lowrank_secant_update: null argument");
   HB_REQUIRE(k->sec_S, "hb_lowrank_secant_update: call hb_lowrank_secant_reset first");
   HB_REQUIRE(jac_set(k), "hb_lowrank_secant_update: register the current Jacobian with hb_lowrank_set_jacobian first");
-  HB_REQUIRE(jacobian_is_constant || k->m == 0 || !k->panel_cols,
-             "hb_lowrank_secant_update: with a host-resident Jacobian only jacobian_is_constant != 0 is supported (J_prev would need a second "
-             "host array)");
   HB_REQUIRE((k->meq == 0 || yc) && (k->mineq == 0 || yd), "hb_lowrank_secant_update: null multiplier block");
   hb_ctx* c = k->ctx;
   const long long n = k->n;
   const int m = k->m, lmax = k->lmax;
   const bool needJ = m > 0 && !jacobian_is_constant;
+  const double* J = nullptr;
+  if(needJ) HB_CHECK(jac_whole(k, "hb_lowrank_secant_update with jacobian_is_constant == 0 (J_prev is a device copy of J)", &J));
   int st = 0;
   if(needJ) HB_CHECK(k->sec_Jprev.reserve(c, (size_t)m * n, "previous Jacobian"));
   if(k->sec_lcurr < 0) {
     // first optimization iterate: only remember it                                     hiopHessianLowRank.cpp:372-381
     k->sec_lcurr = 0;
-    if(needJ) HB_CUDA(cudaMemcpyAsync(k->sec_Jprev, k->J, sizeof(double) * (size_t)m * n, cudaMemcpyDeviceToDevice, c->stream));
+    if(needJ) HB_CUDA(cudaMemcpyAsync(k->sec_Jprev, J, sizeof(double) * (size_t)m * n, cudaMemcpyDeviceToDevice, c->stream));
   } else {
     double* s = k->nv1;
     double* y = k->nv2;
@@ -134,7 +133,7 @@ extern "C" int hb_lowrank_secant_update(hb_lowrank* k, const double* x, const do
       HB_CHECK(hb_stack(c, k->meq, yc, k->mineq, yd, (double*)c->ws));
       if(n > 0) {
         const long long pairs = (n + 1) / 2;
-        k_gemv_cols_diff_store<<<(unsigned)((pairs + ET - 1) / ET), ET, 0, c->stream>>>(m, n, k->J, k->sec_Jprev, (const double*)c->ws, y);
+        k_gemv_cols_diff_store<<<(unsigned)((pairs + ET - 1) / ET), ET, 0, c->stream>>>(m, n, J, k->sec_Jprev, (const double*)c->ws, y);
         HB_LAUNCHED();
       }
     }
