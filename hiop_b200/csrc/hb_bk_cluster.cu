@@ -23,6 +23,7 @@
 //     vector, unit L with zeros below the diagonal of 2x2 blocks, d21 in dsub), which the blocked solves of hb_dense_big.cu consume.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
+#include "hb_ptx.cuh"
 #include <cooperative_groups.h>
 
 namespace cg = cooperative_groups;
@@ -52,18 +53,10 @@ __device__ __forceinline__ ArgMax mailbox_argmax(const double* v, const IT* idx)
   return r;
 }
 
-__device__ __forceinline__ unsigned bk_s2u(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned bk_mapa(unsigned a, unsigned rank)
-{
-  unsigned r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
-  return r;
-}
 // 8 bytes to the same shared-memory location of CTA `rank`, completing 8 bytes of that CTA's mailbox barrier
 __device__ __forceinline__ void bk_post(const void* local_dst, unsigned long long bits, const void* local_bar, unsigned rank)
 {
-  const unsigned ra = bk_mapa(bk_s2u(local_dst), rank), rb = bk_mapa(bk_s2u(local_bar), rank);
-  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b64 [%0], %1, [%2];" ::"r"(ra), "l"(bits), "r"(rb) : "memory");
+  hb_st_async_b64(hb_mapa(local_dst, rank), bits, hb_mapa(local_bar, rank));
 }
 
 // replicated per-step mailbox (one per parity); every CTA of the cluster holds a copy that the others write through DSM
@@ -141,9 +134,9 @@ k_bk_panel(double* __restrict__ A, long long lda, int N, double* __restrict__ W,
   }
   if(tid < NBMAX) sh.dtype[tid] = 0;
   if(tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bk_s2u(&sh.mbar[0])), "r"(1));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bk_s2u(&sh.mbar[1])), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    hb_mbar_init(&sh.mbar[0], 1);
+    hb_mbar_init(&sh.mbar[1], 1);
+    hb_mbar_init_fence();
   }
   __syncthreads();
   cluster.sync();
@@ -166,7 +159,7 @@ k_bk_panel(double* __restrict__ A, long long lda, int N, double* __restrict__ W,
       }
       a = cta_argmax(a, sh.am);
       // this step's mail: 16 candidates (value + index) from the 16 CTAs and the top of column k from CTA 0
-      if(tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bk_s2u(mb)), "r"(CS * 16 + nbp * 8) : "memory");
+      if(tid == 0) hb_mbar_arrive_expect_tx(mb, CS * 16 + nbp * 8);
       if(tid < CS) {
         bk_post(&my->cand_v[rank], (unsigned long long)__double_as_longlong(a.v), mb, tid);
         bk_post(&my->cand_i[rank], (unsigned long long)(long long)a.i, mb, tid);
@@ -178,11 +171,7 @@ k_bk_panel(double* __restrict__ A, long long lda, int N, double* __restrict__ W,
         }
     }
     PP(1);
-    {
-      unsigned ok = 0;
-      while(!ok)
-        asm volatile("{\n.reg .pred q;\nmbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\nselp.u32 %0, 1, 0, q;\n}" : "=r"(ok) : "r"(bk_s2u(mb)), "r"(mphase) : "memory");
-    }
+    while(!hb_mbar_try_wait(mb, mphase)) {}
     PP(2);
     const ArgMax cm = mailbox_argmax(my->cand_v, my->cand_i);
     const double absakk = fabs(my->coltop[kl]);

@@ -244,11 +244,6 @@ __device__ __forceinline__ double hb_warp_max(double v)
   for(int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-// c[0..1] += a * b on the FP64 tensor path (SASS DMMA): one m8n8k4 fragment per thread
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
 __device__ __forceinline__ double hb_warp_min(double v)
 {
 #pragma unroll

@@ -12,6 +12,7 @@
 // Column j of the factor is therefore contiguous in memory -> coalesced along i.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
+#include "hb_ptx.cuh"
 
 namespace {
 
@@ -208,13 +209,12 @@ k_trailing(double* __restrict__ A, int lda, int N, int r0, const double* __restr
     for(int e = tid; e < kpad * TT; e += 128) {
       const int p = e / TT, c = e % TT;
       const bool vp = (p < kb) && (i0 + c < N), vq = (p < kb) && (j0 + c < N);
-      const unsigned sp = (unsigned)__cvta_generic_to_shared(&sP[p][c]), sq = (unsigned)__cvta_generic_to_shared(&sQ[p][c]);
       const double* gp = vp ? P + (size_t)p * ldp + i0 + c : P;
       const double* gq = vq ? Q + (size_t)p * ldq + j0 + c : Q;
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(sp), "l"(gp), "r"(vp ? 8 : 0));
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(sq), "l"(gq), "r"(vq ? 8 : 0));
+      hb_cp_async8(&sP[p][c], gp, vp ? 8 : 0);
+      hb_cp_async8(&sQ[p][c], gq, vq ? 8 : 0);
     }
-    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    hb_cp_async_wait_all();
   }
   __syncthreads();
   const int lane = tid & 31, warp = tid >> 5;
@@ -235,7 +235,7 @@ k_trailing(double* __restrict__ A, int lda, int N, int r0, const double* __restr
 #pragma unroll
     for(int a = 0; a < 4; a++)
 #pragma unroll
-      for(int b = 0; b < 4; b++) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+      for(int b = 0; b < 4; b++) hb_dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
   }
   // epilogue: all loads of the C tile first, then all stores (a load->sub->store chain per element would serialise on
   // L2 latency because the compiler must assume the stores alias the following loads)

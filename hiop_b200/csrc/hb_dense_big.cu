@@ -21,6 +21,7 @@
 // rows below. N = 8192: 2 x 32 launches.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
+#include "hb_ptx.cuh"
 
 namespace {
 
@@ -30,18 +31,6 @@ constexpr int GST = 4;   // pipeline stages
 constexpr int TM = 128;  // tile rows (i)
 constexpr int PLD = TM + 4;
 constexpr int CLD = TM + 2;
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes)
-{
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int NW>
-__device__ __forceinline__ void cp_async_wait()
-{
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(NW));
-}
 
 enum { EPI_SUB = 0, EPI_STORE = 1, EPI_STORE_LDL = 2 };
 
@@ -111,7 +100,7 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
       const int p = idx >> 6, ic = idx & 63;
       const int pp = ch * KC + p, i = i0 + 2 * ic;
       const bool v = pp < kb && i < g.i_end;
-      cp_async16(&sP[p * PLD + 2 * ic], v ? P + (size_t)pp * g.ldp + i : P, v ? 16 : 0);
+      hb_cp_async16(&sP[p * PLD + 2 * ic], v ? P + (size_t)pp * g.ldp + i : P, v ? 16 : 0);
     }
 #pragma unroll
     for(int q = 0; q < (KC * TN / 2) / 256; q++) {
@@ -119,7 +108,7 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
       const int p = idx / (TN / 2), jc = idx % (TN / 2);
       const int pp = ch * KC + p, j = j0 + 2 * jc;
       const bool v = pp < kb && j < g.j_end;
-      cp_async16(&sQ[p * QLD + 2 * jc], v ? Q + (size_t)pp * g.ldq + (j - g.qsub) : Q, v ? 16 : 0);
+      hb_cp_async16(&sQ[p * QLD + 2 * jc], v ? Q + (size_t)pp * g.ldq + (j - g.qsub) : Q, v ? 16 : 0);
     }
   };
 
@@ -135,22 +124,22 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
     for(int e = tid; e < TN * (TM * 8 / 128); e += 256) {
       const int jl = e / (TM * 8 / 128), seg = e % (TM * 8 / 128);
       const int gj = j0 + jl, gi = i0 + seg * 16;
-      if(gj < g.j_end && gi < g.i_end && gi + 15 >= gj) asm volatile("prefetch.global.L2 [%0];" ::"l"(&LC(g.C, g.ldc, gi, gj)));
+      if(gj < g.j_end && gi < g.i_end && gi + 15 >= gj) hb_prefetch_l2(&LC(g.C, g.ldc, gi, gj));
     }
   }
 
 #pragma unroll
   for(int s = 0; s < GST - 1; s++) {
     if(s < nch) load_chunk(s);
-    cp_async_commit();
+    hb_cp_async_commit();
   }
   for(int it = 0; it < nch; it++) {
-    cp_async_wait<GST - 2>();
+    hb_cp_async_wait<GST - 2>();
     __syncthreads();
     {
       const int nx = it + GST - 1;
       if(nx < nch) load_chunk(nx);
-      cp_async_commit();
+      hb_cp_async_commit();
     }
     const double* sP = sm + (size_t)(it % GST) * STAGE_D;
     const double* sQ = sP + KC * PLD;
@@ -164,10 +153,10 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
 #pragma unroll
       for(int a = 0; a < 4; a++)
 #pragma unroll
-        for(int b = 0; b < NJ; b++) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+        for(int b = 0; b < NJ; b++) hb_dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
     }
   }
-  cp_async_wait<0>();
+  hb_cp_async_wait<0>();
   __syncthreads();
   // ---- epilogue: accumulators -> shared (column-major tile, stride CLD) -> global, running down the columns ----
   double* sC = sm;
@@ -351,7 +340,7 @@ __device__ __forceinline__ void subpanel_rows(DiagSmem& S, int kb)
     for(int kk = 0; kk < 4; kk++) {
       const double af = S.D[(c0 + 4 * kk + t4) * DSB + r0 + gq];
 #pragma unroll
-      for(int nt = 0; nt < 2; nt++) dmma884(acc[nt][0], acc[nt][1], af, inv[(nt * 8 + gq) * 17 + 4 * kk + t4]);
+      for(int nt = 0; nt < 2; nt++) hb_dmma884(acc[nt][0], acc[nt][1], af, inv[(nt * 8 + gq) * 17 + 4 * kk + t4]);
     }
     __syncwarp();
 #pragma unroll
@@ -378,7 +367,7 @@ __device__ __forceinline__ void rank16_tile(DiagSmem& S, int c0, int i0, int j0)
     const double af = S.D[(c0 + 4 * kk + t4) * DSB + i0 + gq];
     double bf = S.D[(c0 + 4 * kk + t4) * DSB + j0 + gq];
     if(LDL) bf *= S.dv[c0 + 4 * kk + t4];
-    dmma884(u0, u1, af, bf);
+    hb_dmma884(u0, u1, af, bf);
   }
   const int i = i0 + gq, j = j0 + 2 * t4;
   if(i >= j) S.D[j * DSB + i] -= u0;
@@ -443,7 +432,7 @@ __device__ void invert_block128(DiagSmem& S, double* __restrict__ InvG)
         const int q = q0 + t4, c = n0 + gq;
         const double af = S.D[q * DSB + ncol + 8 * rt + gq];
         const double bf = q > c ? S.D[q * DSB + c] : (q == c ? S.idg[c] : 0.0);
-        dmma884(u0, u1, af, bf);
+        hb_dmma884(u0, u1, af, bf);
       }
       S.Tt[(8 * rt + gq) * TLD + n0 + 2 * t4] = u0;
       S.Tt[(8 * rt + gq) * TLD + n0 + 2 * t4 + 1] = u1;
@@ -454,7 +443,7 @@ __device__ void invert_block128(DiagSmem& S, double* __restrict__ InvG)
       const int rt = t & 1, n0 = (t >> 1) * 8;
       double u0 = 0.0, u1 = 0.0;
 #pragma unroll
-      for(int k4 = 0; k4 < 16; k4 += 4) dmma884(u0, u1, inv[(8 * rt + gq) * 17 + k4 + t4], S.Tt[(k4 + t4) * TLD + n0 + gq]);
+      for(int k4 = 0; k4 < 16; k4 += 4) hb_dmma884(u0, u1, inv[(8 * rt + gq) * 17 + k4 + t4], S.Tt[(k4 + t4) * TLD + n0 + gq]);
       const int ra = ncol + 8 * rt + gq, c = n0 + 2 * t4;
       S.D[ra * DSB + c] = -u0;
       S.D[ra * DSB + c + 1] = -u1;
@@ -535,16 +524,16 @@ k_trsm_panel(double* __restrict__ A, long long lda, int N, int k0, const double*
   //      it lies in memory (never read: the recurrence only touches entries strictly below the 16 x 16 diagonal blocks). ----
   for(int e = tid; e < BB * BB / 2; e += 256) {
     const int j = e / (BB / 2), i = (e % (BB / 2)) * 2;
-    cp_async16(&S.L[j * DSB + i], &LC(A, lda, k0 + i, k0 + j), 16);
+    hb_cp_async16(&S.L[j * DSB + i], &LC(A, lda, k0 + i, k0 + j), 16);
   }
   for(int e = tid; e < BB * XROWS / 2; e += 256) {
     const int c = e / (XROWS / 2), r = (e % (XROWS / 2)) * 2;
     const bool v = i0 + r < N;
-    cp_async16(&S.X[c * XS + r], v ? &LC(A, lda, i0 + r, k0 + c) : A, v ? 16 : 0);
+    hb_cp_async16(&S.X[c * XS + r], v ? &LC(A, lda, i0 + r, k0 + c) : A, v ? 16 : 0);
   }
   for(int e = tid; e < 8 * 16 * 17; e += 256) S.Inv16[e] = inv16G[e];
-  cp_async_commit();
-  cp_async_wait<0>();
+  hb_cp_async_commit();
+  hb_cp_async_wait<0>();
   __syncthreads();
   const int rw = warp * 8; // my 8 rows
   for(int jb = 0; jb < BB / 16; jb++) {
@@ -553,7 +542,7 @@ k_trsm_panel(double* __restrict__ A, long long lda, int N, int k0, const double*
     for(int q0 = 0; q0 < cb; q0 += 4) {
       const double af = S.X[(q0 + t4) * XS + rw + gq];
 #pragma unroll
-      for(int nt = 0; nt < 2; nt++) dmma884(acc[nt][0], acc[nt][1], af, S.L[(q0 + t4) * DSB + cb + 8 * nt + gq]);
+      for(int nt = 0; nt < 2; nt++) hb_dmma884(acc[nt][0], acc[nt][1], af, S.L[(q0 + t4) * DSB + cb + 8 * nt + gq]);
     }
     // Y = A - sum (my C-fragment elements), in place
 #pragma unroll
@@ -570,7 +559,7 @@ k_trsm_panel(double* __restrict__ A, long long lda, int N, int k0, const double*
     for(int kk = 0; kk < 4; kk++) {
       const double af = S.X[(cb + 4 * kk + t4) * XS + rw + gq];
 #pragma unroll
-      for(int nt = 0; nt < 2; nt++) dmma884(ac2[nt][0], ac2[nt][1], af, inv[(nt * 8 + gq) * 17 + 4 * kk + t4]);
+      for(int nt = 0; nt < 2; nt++) hb_dmma884(ac2[nt][0], ac2[nt][1], af, inv[(nt * 8 + gq) * 17 + 4 * kk + t4]);
     }
     __syncwarp();
 #pragma unroll
@@ -706,7 +695,7 @@ k_solve_fwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
   const int r = tid & 127, gsel = tid >> 7; // 8 groups
   // programmatic dependent launch: the next step's grid may start now (its CTAs prefetch the factor / inverse, which no step writes)
   // and blocks in griddepcontrol.wait until this grid has completed before it touches x, the partials or the counter
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  hb_griddep_launch_dependents();
   if(blockIdx.x != 0) {
     // ---- main: partial[b][r] = sum_{j in 64-column chunk b} L(k0 + r, j) x_j ----
     const int b = blockIdx.x - 1;
@@ -717,7 +706,7 @@ k_solve_fwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
       const int j = jb + gsel * 8 + q;
       v[q] = (r < nrows && j < k0) ? LC(F, ldf, k0 + r, j) : 0.0;
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    hb_griddep_wait();
     // x is written by the tail CTA of EARLIER steps (other SMs, overlapping grids under programmatic dependent launch): read it from L2,
     // never from a line this SM's L1 may still hold from before (a vector that is not 128-byte aligned lets a line straddle k0)
     if(tid < 64) S.xs[tid] = (jb + tid < k0) ? __ldcg(x + jb + tid) : 0.0;
@@ -746,7 +735,7 @@ k_solve_fwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
     const int cc = gsel + 8 * q;
     inv[q] = cc <= r ? Inv[cc * BB + r] : 0.0;
   }
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  hb_griddep_wait();
   const double xk = (tid < nrows) ? __ldcg(x + k0 + tid) : 0.0;
   wait_counter(counter, G);
   gather_partials(S, partial, G, nrows, xk);
@@ -773,7 +762,7 @@ k_solve_bwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, G = gridDim.x - 1;
   const int nrows = min(SB, N - k0);
   const int k1 = k0 + nrows;
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  hb_griddep_launch_dependents();
   if(blockIdx.x != 0) {
     // ---- main: partial[b][j] = sum_{i in 64-row chunk b below the step} L(i, k0 + j) x_i ----
     const int b = blockIdx.x - 1;
@@ -785,7 +774,7 @@ k_solve_bwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
       const int jl = cg * 8 + q;
       v[q] = (i < N && jl < nrows) ? LC(F, ldf, i, k0 + jl) : 0.0;
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    hb_griddep_wait();
     const double xi = i < N ? __ldcg(x + i) : 0.0;
 #pragma unroll
     for(int q = 0; q < 8; q++) v[q] = hb_warp_sum(v[q] * xi);
@@ -813,7 +802,7 @@ k_solve_bwd_step(const double* __restrict__ F, long long ldf, int N, int k0, con
       const int cc = warp + 32 * t, rr = lane + 32 * u;
       it[t * 4 + u] = rr >= cc ? Inv[cc * BB + rr] : 0.0;
     }
-  asm volatile("griddepcontrol.wait;" ::: "memory");
+  hb_griddep_wait();
   const double xk = (tid < nrows) ? __ldcg(x + k0 + tid) : 0.0;
   wait_counter(counter, G);
   gather_partials(S, partial, G, nrows, xk);

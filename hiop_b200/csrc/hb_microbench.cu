@@ -4,7 +4,7 @@
 //     (no loads in the loop): the integer tensor-core rate k_oz_gemm draws on.
 // Both are timed with CUDA events on the context stream over a few milliseconds, after a warm-up launch.
 #include "hb_common.cuh"
-#include "hb_wgmma.cuh"
+#include "hb_ptx.cuh"
 
 namespace {
 
@@ -17,7 +17,7 @@ k_peak_dmma(double* __restrict__ out, int iters, double a, double b)
   for(int it = 0; it < iters; it++) {
 #pragma unroll
     for(int i = 0; i < 8; i++)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[i][0]), "+d"(c[i][1]) : "d"(a), "d"(b));
+      hb_dmma884(c[i][0], c[i][1], a, b);
   }
   double s = 0;
 #pragma unroll
@@ -25,23 +25,21 @@ k_peak_dmma(double* __restrict__ out, int iters, double a, double b)
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
-__device__ __forceinline__ uint32_t s2u(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 // one CTA per SM, two warpgroups: 16 KB A tile (128 rows x 128 B, 64 rows per warpgroup) + 32 KB B tile (256 rows x 128 B) in the
 // SWIZZLE_128B K-major layout (contents do not matter for the rate), one m64n256 register accumulator per warpgroup
 __global__ void __launch_bounds__(256, 1)
 k_peak_i8(int iters, int* __restrict__ sink)
 {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024 - (s2u(smem_raw) & 1023)) & 1023);
+  uint8_t* smem = smem_raw + ((1024 - (hb_smem_addr(smem_raw) & 1023)) & 1023);
   const int tid = threadIdx.x, wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
   for(int i = tid; i < (16 + 32) * 1024 / 4; i += 256) reinterpret_cast<uint32_t*>(smem)[i] = 0x01010101u * (i & 3);
-  asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); // generic-proxy writes of the operands -> visible to the tensor core
+  hb_fence_proxy_async_shared(); // generic-proxy writes of the operands -> visible to the tensor core
   __syncthreads();
   uint32_t acc[128];
 #pragma unroll
   for(int i = 0; i < 128; i++) acc[i] = 0u;
-  const uint32_t sa = s2u(smem) + wg * 64 * 128, sb = s2u(smem + 16 * 1024);
+  const uint32_t sa = hb_smem_addr(smem) + wg * 64 * 128, sb = hb_smem_addr(smem + 16 * 1024);
   for(int it = 0; it < iters; it++) {
     hb_wgmma_fence();
 #pragma unroll

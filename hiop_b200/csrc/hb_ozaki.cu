@@ -20,7 +20,7 @@
 // with 232 registers, the producer warpgroup with 40.
 // A last kernel sums the split-K partials in fixed order, applies 2^{e_i+e_j} and mirrors the tile (deterministic).
 #include "hb_common.cuh"
-#include "hb_wgmma.cuh"
+#include "hb_ptx.cuh"
 #include <cuda.h>
 #include <cstdlib>
 
@@ -32,28 +32,7 @@ constexpr int A_TILE = TM * KS;   // 16 KB per slice
 constexpr int B_TILE = TN * KS;   // 4 KB per slice
 constexpr int OZ_CONSUMERS = 256; // two warpgroups
 constexpr int OZ_THREADS = OZ_CONSUMERS + 128; // + the producer warpgroup
-
-__device__ __forceinline__ uint32_t s2u(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* b, unsigned c) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(s2u(b)), "r"(c)); }
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long* b, unsigned bytes)
-{
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(s2u(b)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* b) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(s2u(b)) : "memory"); }
-// the retry loop lives inside the asm: to the compiler the wait is straight-line code, so a warpgroup stays converged for wgmma
-__device__ __forceinline__ void mbar_wait(unsigned long long* b, unsigned parity)
-{
-  asm volatile(
-      "{\n.reg .pred p;\nWAIT_%=:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n@!p bra WAIT_%=;\n}\n" ::"r"(s2u(b)), "r"(parity),
-      "r"(0x989680u)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, unsigned long long* bar)
-{
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n" ::"r"(s2u(dst)),
-               "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(s2u(bar))
-               : "memory");
-}
+constexpr unsigned OZ_SUSPEND_NS = 10000000u;  // suspend-time hint of every mbarrier wait of k_oz_gemm (its SASS differs without it)
 
 // ---------------------------------------------------------------------------------------------------------------------
 // slicing
@@ -280,7 +259,7 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
   constexpr int RING = Cfg::RING;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must start on a 1024-byte boundary
-  uint8_t* smem = smem_raw + ((1024 - (s2u(smem_raw) & 1023)) & 1023);
+  uint8_t* smem = smem_raw + ((1024 - (hb_smem_addr(smem_raw) & 1023)) & 1023);
   uint8_t* bbuf = smem;                       // 2 x B_BLOCK
   uint8_t* aring = smem + 2 * Cfg::B_BLOCK;   // RING x A_TILE
   unsigned long long* bfull = reinterpret_cast<unsigned long long*>(aring + RING * A_TILE);
@@ -290,15 +269,15 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
   // warp index through a shuffle: provably warp-uniform, so the consumer branch is not a divergent path for wgmma
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   if(tid == 0) {
-    for(int s = 0; s < 2; s++) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 2); }
-    for(int s = 0; s < RING; s++) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], 2); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for(int s = 0; s < 2; s++) { hb_mbar_init(&bfull[s], 1); hb_mbar_init(&bempty[s], 2); }
+    for(int s = 0; s < RING; s++) { hb_mbar_init(&afull[s], 1); hb_mbar_init(&aempty[s], 2); }
+    hb_mbar_init_fence();
   }
   __syncthreads();
 
   if(warp >= OZ_CONSUMERS / 32) {
     // ================= TMA producer =================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    hb_setmaxnreg_dec<40>();
     if(warp != OZ_CONSUMERS / 32 || lane != 0) return;
     int bs = 0, as = 0;
     unsigned bph = 0, aph = 0;
@@ -306,15 +285,15 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
       const OzItem itm = items[w];
       for(int it = 0; it < itm.k_count; it++) {
         const int kc = (itm.k_begin + it) * KS;
-        mbar_wait(&bempty[bs], bph ^ 1);
-        mbar_expect_tx(&bfull[bs], Cfg::B_BLOCK);
-        tma_load_3d(bbuf + bs * Cfg::B_BLOCK, &mapB, kc, itm.bj * TN, 0, &bfull[bs]); // box {128 B, 32 rows, S slices}
+        hb_mbar_wait<OZ_SUSPEND_NS>(&bempty[bs], bph ^ 1);
+        hb_mbar_arrive_expect_tx(&bfull[bs], Cfg::B_BLOCK);
+        hb_tma_load_3d(bbuf + bs * Cfg::B_BLOCK, &mapB, kc, itm.bj * TN, 0, &bfull[bs]); // box {128 B, 32 rows, S slices}
         if(++bs == 2) { bs = 0; bph ^= 1; }
 #pragma unroll 1
         for(int p = 0; p < S; p++) {
-          mbar_wait(&aempty[as], aph ^ 1);
-          mbar_expect_tx(&afull[as], A_TILE);
-          tma_load_3d(aring + as * A_TILE, &mapA, kc, itm.bi * TM, p, &afull[as]);    // box {128 B, 128 rows, 1 slice}
+          hb_mbar_wait<OZ_SUSPEND_NS>(&aempty[as], aph ^ 1);
+          hb_mbar_arrive_expect_tx(&afull[as], A_TILE);
+          hb_tma_load_3d(aring + as * A_TILE, &mapA, kc, itm.bi * TM, p, &afull[as]);    // box {128 B, 128 rows, 1 slice}
           if(++as == RING) { as = 0; aph ^= 1; }
         }
       }
@@ -323,7 +302,7 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
   }
 
   // ================= consumer warpgroups: MMA + epilogue =================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  hb_setmaxnreg_inc<232>();
   const int wg = warp >> 2;
   const bool leader = (tid & 127) == 0;
   // accumulator fragment of m64nNk32: register 4j + 2h + c of a 32-column block holds row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
@@ -339,13 +318,13 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
     double* tile = partial + (size_t)itm.slot * (TM * TN);
     int in_chunk = 0, chunk = 0;
     for(int it = 0; it < itm.k_count; it++) {
-      mbar_wait(&bfull[bs], bph);
-      const uint32_t sb = s2u(bbuf + bs * Cfg::B_BLOCK);
+      hb_mbar_wait<OZ_SUSPEND_NS>(&bfull[bs], bph);
+      const uint32_t sb = hb_smem_addr(bbuf + bs * Cfg::B_BLOCK);
       const int chunk_start = in_chunk == 0;
 #pragma unroll
       for(int p = 0; p < S; p++) {
-        mbar_wait(&afull[as], aph);
-        const uint32_t sa = s2u(aring + as * A_TILE) + wg * (64 * KS);
+        hb_mbar_wait<OZ_SUSPEND_NS>(&afull[as], aph);
+        const uint32_t sa = hb_smem_addr(aring + as * A_TILE) + wg * (64 * KS);
 #pragma unroll
         for(int i = 0; i < S * 16; i++) hb_wgmma_fence_operand(acc[i]);
         hb_wgmma_fence();
@@ -358,8 +337,8 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
         hb_wgmma_commit();
         hb_wgmma_wait<1>();
         if(leader) {
-          if(pend_a >= 0) mbar_arrive(&aempty[pend_a]);
-          if(pend_b >= 0) mbar_arrive(&bempty[pend_b]);
+          if(pend_a >= 0) hb_mbar_arrive(&aempty[pend_a]);
+          if(pend_b >= 0) hb_mbar_arrive(&bempty[pend_b]);
         }
         pend_a = as;
         pend_b = p == S - 1 ? bs : -1;
@@ -371,8 +350,8 @@ k_oz_gemm(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUte
 #pragma unroll
         for(int i = 0; i < S * 16; i++) hb_wgmma_fence_operand(acc[i]);
         if(leader) {
-          mbar_arrive(&aempty[pend_a]);
-          mbar_arrive(&bempty[pend_b]);
+          hb_mbar_arrive(&aempty[pend_a]);
+          hb_mbar_arrive(&bempty[pend_b]);
         }
         pend_a = pend_b = -1;
 #pragma unroll

@@ -18,6 +18,7 @@
 // slot; a second kernel sums the slots of each tile in a FIXED order and mirrors the result, so the output is
 // bit-reproducible run to run (no atomics).
 #include "hb_common.cuh"
+#include "hb_ptx.cuh"
 #include <cstdlib>
 
 namespace {
@@ -45,23 +46,6 @@ struct Seg
   int slot;        // workspace slot receiving the partial tile
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes)
-{
-  unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async8(void* smem, const void* gmem, int src_bytes)
-{
-  unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(s), "l"(gmem), "r"(src_bytes));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait()
-{
-  asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
-}
-
 // Loads one K chunk (BK columns starting at column k0) of the row tile(s) into a stage.
 template <bool ALIGN16>
 __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_a, const double* const* srow_b, bool diag,
@@ -79,10 +63,10 @@ __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_
     for(int j = 0; j < 4; j++) {
       const int row = (tid >> 3) + 32 * j;
       const double* pa = srow_a[row];
-      cp_async16(&st.a[row * LDS_ROW + kc * 2], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
+      hb_cp_async16(&st.a[row * LDS_ROW + kc * 2], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
       if(!diag) {
         const double* pb = srow_b[row];
-        cp_async16(&st.b[row * LDS_ROW + kc * 2], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
+        hb_cp_async16(&st.b[row * LDS_ROW + kc * 2], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
       }
     }
     if(tid < 8) {
@@ -90,7 +74,7 @@ __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_
         const long long kd = k0 + tid * 2;
         long long r2 = K - kd;
         const int nbd = r2 >= 2 ? 16 : (r2 == 1 ? 8 : 0);
-        cp_async16(&st.d[tid * 2], nbd ? dvec_or_null + kd : dummy, nbd);
+        hb_cp_async16(&st.d[tid * 2], nbd ? dvec_or_null + kd : dummy, nbd);
       } else {
         st.d[tid * 2] = 1.0;
         st.d[tid * 2 + 1] = 1.0;
@@ -105,17 +89,17 @@ __device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_
     for(int j = 0; j < 8; j++) {
       const int row = (tid >> 4) + 16 * j;
       const double* pa = srow_a[row];
-      cp_async8(&st.a[row * LDS_ROW + kc], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
+      hb_cp_async8(&st.a[row * LDS_ROW + kc], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
       if(!diag) {
         const double* pb = srow_b[row];
-        cp_async8(&st.b[row * LDS_ROW + kc], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
+        hb_cp_async8(&st.b[row * LDS_ROW + kc], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
       }
     }
     if(tid < 16) {
       if(dvec_or_null) {
         const long long kd = k0 + tid;
         const int nbd = kd < K ? 8 : 0;
-        cp_async8(&st.d[tid], nbd ? dvec_or_null + kd : dummy, nbd);
+        hb_cp_async8(&st.d[tid], nbd ? dvec_or_null + kd : dummy, nbd);
       } else {
         st.d[tid] = 1.0;
       }
@@ -163,15 +147,15 @@ k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const 
 #pragma unroll
     for(int s = 0; s < STAGES - 1; s++) {
       if(s < kcount) load_stage<ALIGN16>(stages[s], srow_a, srow_b, diag, dvec, (const double*)rowptr, kbase + (long long)s * BK, K);
-      cp_async_commit();
+      hb_cp_async_commit();
     }
     for(int it = 0; it < kcount; it++) {
-      cp_async_wait<STAGES - 2>();
+      hb_cp_async_wait<STAGES - 2>();
       __syncthreads();
       {
         const int nx = it + STAGES - 1;
         if(nx < kcount) load_stage<ALIGN16>(stages[nx % STAGES], srow_a, srow_b, diag, dvec, (const double*)rowptr, kbase + (long long)nx * BK, K);
-        cp_async_commit();
+        hb_cp_async_commit();
       }
       const Stage& st = stages[it % STAGES];
       const double* sA = st.a + (warp_m * 64 + g) * LDS_ROW + t4;
@@ -187,10 +171,10 @@ k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const 
 #pragma unroll
         for(int i = 0; i < 8; i++)
 #pragma unroll
-          for(int j = 0; j < 4; j++) dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+          for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
       }
     }
-    cp_async_wait<0>();
+    hb_cp_async_wait<0>();
 
     double* slot = ws + (size_t)sg.slot * (BM * BM);
 #pragma unroll
@@ -229,33 +213,6 @@ struct WStage
 };
 constexpr size_t WSMEM_BYTES = sizeof(WStage) * WSTAGES + 2 * BM * sizeof(const double*) + 2 * WSTAGES * sizeof(unsigned long long);
 
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count)
-{
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar)
-{
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_on_cp_async(unsigned long long* bar)
-{
-  // arrives (without incrementing the pending count) once all prior cp.async of this thread have landed
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity)
-{
-  const unsigned addr = (unsigned)__cvta_generic_to_shared(bar);
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra.uni WAIT_DONE;\n"
-      "bra.uni WAIT_LOOP;\n"
-      "WAIT_DONE:\n"
-      "}\n" ::"r"(addr), "r"(parity) : "memory");
-}
-
 __global__ void __launch_bounds__(WTHREADS, 1)
 k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const double* __restrict__ extra_row,
           const Seg* __restrict__ segs, const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
@@ -271,10 +228,10 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
   if(tid == 0) {
 #pragma unroll
     for(int s = 0; s < WSTAGES; s++) {
-      mbar_init(&full[s], WPROD); // every producer thread arrives once its copies of the stage have landed
-      mbar_init(&empty[s], 8);    // one arrival per MMA warp
+      hb_mbar_init(&full[s], WPROD); // every producer thread arrives once its copies of the stage have landed
+      hb_mbar_init(&empty[s], 8);    // one arrival per MMA warp
     }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    hb_mbar_init_fence();
   }
   __syncthreads();
 
@@ -290,35 +247,35 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
     for(int si = sb; si < se; si++) {
       const Seg sg = segs[si];
       const bool diag = sg.ti == sg.tj;
-      asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory"); // all producers done with the previous segment's row table
+      hb_bar_sync<1, WPROD>(); // all producers done with the previous segment's row table
       for(int r = p; r < 2 * BM; r += WPROD) {
         const int grow = (r < BM ? sg.ti * BM + r : sg.tj * BM + (r - BM));
         srow[r] = grow < M ? rowptr[grow] : (grow == M ? extra_row : nullptr);
       }
-      asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory");
+      hb_bar_sync<1, WPROD>();
       for(int it = 0; it < sg.k_count; it++) {
         const long long k = ((long long)sg.k_begin + it) * WBK + kc * 2;
         const long long rem = K - k;
         const int nb = rem >= 2 ? 16 : (rem == 1 ? 8 : 0);
         const long long koff = nb ? k : 0;
-        mbar_wait(&empty[stage], phase ^ 1);
+        hb_mbar_wait(&empty[stage], phase ^ 1);
         WStage& st = stages[stage];
 #pragma unroll 4
         for(int j = 0; j < 16; j++) {
           const int row = r0 + 8 * j;
           const double* pa = srow[row];
-          cp_async16(&st.a[row * WLDS + kc * 2], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
+          hb_cp_async16(&st.a[row * WLDS + kc * 2], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
           if(!diag) {
             const double* pb = srow[BM + row];
-            cp_async16(&st.b[row * WLDS + kc * 2], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
+            hb_cp_async16(&st.b[row * WLDS + kc * 2], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
           }
         }
-        if(p < 16 && dvec) cp_async16(&st.d[kc * 2], nb ? dvec + k : (const double*)rowptr, nb);
-        mbar_arrive_on_cp_async(&full[stage]);
+        if(p < 16 && dvec) hb_cp_async16(&st.d[kc * 2], nb ? dvec + k : (const double*)rowptr, nb);
+        hb_mbar_arrive_cp_async(&full[stage]);
         if(++stage == WSTAGES) { stage = 0; phase ^= 1; }
       }
     }
-    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    hb_cp_async_wait_all();
   } else {
     // ================= 8 MMA warps =================
     const int warp_m = warp & 1, warp_n = warp >> 1;
@@ -333,7 +290,7 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
 #pragma unroll
         for(int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
       for(int it = 0; it < sg.k_count; it++) {
-        mbar_wait(&full[stage], phase);
+        hb_mbar_wait(&full[stage], phase);
         const WStage& st = stages[stage];
         const double* sA = st.a + (warp_m * 64 + g) * WLDS + t4;
         const double* sB = (diag ? st.a : st.b) + (warp_n * 32 + g) * WLDS + t4;
@@ -348,10 +305,10 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
 #pragma unroll
           for(int i = 0; i < 8; i++)
 #pragma unroll
-            for(int j = 0; j < 4; j++) dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+            for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
         }
         __syncwarp();
-        if(lane == 0) mbar_arrive(&empty[stage]);
+        if(lane == 0) hb_mbar_arrive(&empty[stage]);
         if(++stage == WSTAGES) { stage = 0; phase ^= 1; }
       }
       double* slot = ws + (size_t)sg.slot * (BM * BM);

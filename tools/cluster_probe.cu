@@ -2,20 +2,13 @@
 //   (a) st.shared::cluster (generic DSM store) + cluster.sync()  (barrier.cluster.arrive.release / wait.acquire)
 //   (b) st.async ... mbarrier::complete_tx to every CTA + local mbarrier wait (no cluster barrier, no fence)
 //   (c) cluster.sync() alone, and __syncthreads alone, for reference
-// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/cluster_probe tools/cluster_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -Ihiop_b200/csrc -o tools/cluster_probe tools/cluster_probe.cu
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>
+#include "hb_ptx.cuh"
 namespace cg = cooperative_groups;
 constexpr int CS = 16;
-
-__device__ __forceinline__ unsigned s2u(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ unsigned mapa(unsigned a, unsigned rank)
-{
-  unsigned r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
-  return r;
-}
 
 __global__ void __cluster_dims__(CS, 1, 1) k_probe(int iters, int mode, long long* out)
 {
@@ -24,8 +17,8 @@ __global__ void __cluster_dims__(CS, 1, 1) k_probe(int iters, int mode, long lon
   __shared__ double box[2][CS];
   __shared__ unsigned long long bar[2];
   if(tid == 0) {
-    for(int p = 0; p < 2; p++) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(s2u(&bar[p])), "r"(1));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for(int p = 0; p < 2; p++) hb_mbar_init(&bar[p], 1);
+    hb_mbar_init_fence();
   }
   __syncthreads();
   cluster.sync();
@@ -38,14 +31,12 @@ __global__ void __cluster_dims__(CS, 1, 1) k_probe(int iters, int mode, long lon
       if(tid < CS) cluster.map_shared_rank(&box[p][0], tid)[rank] = (double)(it + rank);
       cluster.sync();
     } else if(mode == 1) {
-      if(tid == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(s2u(&bar[p])), "r"(CS * 8) : "memory");
+      if(tid == 0) hb_mbar_arrive_expect_tx(&bar[p], CS * 8);
       if(tid < CS) {
-        const unsigned ra = mapa(s2u(&box[p][rank]), tid), rb = mapa(s2u(&bar[p]), tid);
         const double v = (double)(it + rank);
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.b64 [%0], %1, [%2];" ::"r"(ra), "l"(__double_as_longlong(v)), "r"(rb) : "memory");
+        hb_st_async_b64(hb_mapa(&box[p][rank], tid), __double_as_longlong(v), hb_mapa(&bar[p], tid));
       }
-      unsigned ok = 0;
-      while(!ok) asm volatile("{\n.reg .pred q;\nmbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\nselp.u32 %0, 1, 0, q;\n}" : "=r"(ok) : "r"(s2u(&bar[p])), "r"(phase[p]) : "memory");
+      while(!hb_mbar_try_wait(&bar[p], phase[p])) {}
       phase[p] ^= 1;
     } else if(mode == 2) {
       cluster.sync();

@@ -1,7 +1,8 @@
 // Microbenchmark: FP64 issue rates on H100 (DFMA vs DMMA shapes) -- decides the condensation kernel design.
-// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench_fp64 tools/microbench_fp64.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -Ihiop_b200/csrc -o tools/microbench_fp64 tools/microbench_fp64.cu
 #include <cstdio>
 #include <cuda_runtime.h>
+#include "hb_ptx.cuh"
 
 #define CK(x) do { cudaError_t e = (x); if(e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); return 1; } } while(0)
 
@@ -28,8 +29,7 @@ __global__ void k_dmma884(double* out, int iters, double a, double b)
   for(int it = 0; it < iters; it++) {
 #pragma unroll
     for(int i = 0; i < 8; i++)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-                   : "+d"(c[i][0]), "+d"(c[i][1]) : "d"(a), "d"(b));
+      hb_dmma884(c[i][0], c[i][1], a, b);
   }
   double s = 0;
 #pragma unroll
@@ -40,13 +40,12 @@ __global__ void k_dmma884(double* out, int iters, double a, double b)
 __global__ void k_dmma1688(double* out, int iters, double a, double b)
 {
   double c[8][4];
+  const double fa[4] = {a, b, a, b}, fb[2] = {a, b};
 #pragma unroll
   for(int i = 0; i < 8; i++) { c[i][0] = threadIdx.x; c[i][1] = i; c[i][2] = 1; c[i][3] = 2; }
   for(int it = 0; it < iters; it++) {
 #pragma unroll
-    for(int i = 0; i < 8; i++)
-      asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                   : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3]) : "d"(a), "d"(b), "d"(a), "d"(b), "d"(a), "d"(b));
+    for(int i = 0; i < 8; i++) hb_dmma1688(c[i], fa, fb);
   }
   double s = 0;
 #pragma unroll
@@ -57,14 +56,12 @@ __global__ void k_dmma1688(double* out, int iters, double a, double b)
 __global__ void k_dmma16816(double* out, int iters, double a, double b)
 {
   double c[8][4];
+  const double fa[8] = {a, b, a, b, a, b, a, b}, fb[4] = {a, b, a, b};
 #pragma unroll
   for(int i = 0; i < 8; i++) { c[i][0] = threadIdx.x; c[i][1] = i; c[i][2] = 1; c[i][3] = 2; }
   for(int it = 0; it < iters; it++) {
 #pragma unroll
-    for(int i = 0; i < 8; i++)
-      asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};"
-                   : "+d"(c[i][0]), "+d"(c[i][1]), "+d"(c[i][2]), "+d"(c[i][3])
-                   : "d"(a), "d"(b), "d"(a), "d"(b), "d"(a), "d"(b), "d"(a), "d"(b), "d"(a), "d"(b), "d"(a), "d"(b));
+    for(int i = 0; i < 8; i++) hb_dmma16816(c[i], fa, fb);
   }
   double s = 0;
 #pragma unroll

@@ -10,7 +10,7 @@
 // Reports TFLOP/s executed and bytes/s moved from L2 into shared memory, the SM clock derived from clock64() over the kernel's
 // duration, and the FP64 DMMA peak of the library (hb_microbench_peak(0)) measured in the same process.
 // Build (after make -C hiop_b200/csrc):
-//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Iinclude -o tools/syrk_feed_probe tools/syrk_feed_probe.cu \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Iinclude -Ihiop_b200/csrc -o tools/syrk_feed_probe tools/syrk_feed_probe.cu \
 //        -Lhiop_b200 -lhiopb200 -Xlinker -rpath,'$ORIGIN/../hiop_b200'
 // Run: tools/syrk_feed_probe [M=1012] [K=1000000]
 #include <algorithm>
@@ -19,6 +19,7 @@
 #include <vector>
 #include <cuda_runtime.h>
 #include "hiopb200.h"
+#include "hb_ptx.cuh"
 
 #define CK(x) do { cudaError_t e = (x); if(e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); exit(1); } } while(0)
 
@@ -28,32 +29,6 @@ struct WStage { double a[WTILE_D]; double b[WTILE_D]; double d[WBK]; };
 constexpr size_t WSMEM_BYTES = sizeof(WStage) * WSTAGES + 2 * BM * sizeof(const double*) + 2 * WSTAGES * sizeof(unsigned long long);
 struct Seg { int ti, tj, k_begin, k_count, slot; };
 enum { FULL = 0, MMA_ONLY = 1, FEED_ONLY = 2 };
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes)
-{
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem), "r"(src_bytes));
-}
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
-{
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count)
-{
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar)
-{
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_on_cp_async(unsigned long long* bar)
-{
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity)
-{
-  asm volatile("{\n.reg .pred p;\nWAIT_LOOP:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra.uni WAIT_DONE;\nbra.uni WAIT_LOOP;\nWAIT_DONE:\n}\n"
-               ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(parity) : "memory");
-}
 
 template <int MODE>
 __global__ void __launch_bounds__(WTHREADS, 1)
@@ -70,8 +45,8 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
   if(MODE == MMA_ONLY)
     for(int e = tid; e < (int)(sizeof(WStage) / sizeof(double)); e += WTHREADS) reinterpret_cast<double*>(stages)[e] = 1e-3 * (e & 7);
   if(tid == 0) {
-    for(int s = 0; s < WSTAGES; s++) { mbar_init(&full[s], WPROD); mbar_init(&empty[s], 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    for(int s = 0; s < WSTAGES; s++) { hb_mbar_init(&full[s], WPROD); hb_mbar_init(&empty[s], 8); }
+    hb_mbar_init_fence();
   }
   __syncthreads();
   const int sb = cta_seg_begin[blockIdx.x], se = cta_seg_begin[blockIdx.x + 1];
@@ -83,35 +58,35 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
     for(int si = sb; si < se; si++) {
       const Seg sg = segs[si];
       const bool diag = sg.ti == sg.tj;
-      asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory");
+      hb_bar_sync<1, WPROD>();
       for(int r = p; r < 2 * BM; r += WPROD) {
         const int grow = (r < BM ? sg.ti * BM + r : sg.tj * BM + (r - BM));
         srow[r] = grow < M ? rowptr[grow] : nullptr;
       }
-      asm volatile("bar.sync 1, %0;\n" ::"n"(WPROD) : "memory");
+      hb_bar_sync<1, WPROD>();
       for(int it = 0; it < sg.k_count; it++) {
         const long long k = ((long long)sg.k_begin + it) * WBK + kc * 2;
         const long long rem = K - k;
         const int nb = rem >= 2 ? 16 : (rem == 1 ? 8 : 0);
         const long long koff = nb ? k : 0;
-        mbar_wait(&empty[stage], phase ^ 1);
+        hb_mbar_wait(&empty[stage], phase ^ 1);
         WStage& st = stages[stage];
 #pragma unroll 4
         for(int j = 0; j < 16; j++) {
           const int row = r0 + 8 * j;
           const double* pa = srow[row];
-          cp_async16(&st.a[row * WLDS + kc * 2], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
+          hb_cp_async16(&st.a[row * WLDS + kc * 2], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
           if(!diag) {
             const double* pb = srow[BM + row];
-            cp_async16(&st.b[row * WLDS + kc * 2], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
+            hb_cp_async16(&st.b[row * WLDS + kc * 2], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
           }
         }
-        if(p < 16 && dvec) cp_async16(&st.d[kc * 2], nb ? dvec + k : (const double*)rowptr, nb);
-        mbar_arrive_on_cp_async(&full[stage]);
+        if(p < 16 && dvec) hb_cp_async16(&st.d[kc * 2], nb ? dvec + k : (const double*)rowptr, nb);
+        hb_mbar_arrive_cp_async(&full[stage]);
         if(++stage == WSTAGES) { stage = 0; phase ^= 1; }
       }
     }
-    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    hb_cp_async_wait_all();
   } else {
     const int warp_m = warp & 1, warp_n = warp >> 1, g = lane >> 2, t4 = lane & 3;
     for(int si = sb; si < se; si++) {
@@ -123,7 +98,7 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
 #pragma unroll
         for(int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
       for(int it = 0; it < sg.k_count; it++) {
-        if(MODE != MMA_ONLY) mbar_wait(&full[stage], phase);
+        if(MODE != MMA_ONLY) hb_mbar_wait(&full[stage], phase);
         if(MODE != FEED_ONLY) {
           const WStage& st = stages[MODE == MMA_ONLY ? 0 : stage];
           const double* sA = st.a + (warp_m * 64 + g) * WLDS + t4;
@@ -139,12 +114,12 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
 #pragma unroll
             for(int i = 0; i < 8; i++)
 #pragma unroll
-              for(int j = 0; j < 4; j++) dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+              for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
           }
         }
         if(MODE != MMA_ONLY) {
           __syncwarp();
-          if(lane == 0) mbar_arrive(&empty[stage]);
+          if(lane == 0) hb_mbar_arrive(&empty[stage]);
           if(++stage == WSTAGES) { stage = 0; phase ^= 1; }
         }
       }
