@@ -123,6 +123,7 @@ def lib() -> ctypes.CDLL:
     f("hb_symdense_solve_host", c_i, c_vp, c_vp, c_i)
     f("hb_debug_diag128_profile", c_i, c_vp, c_i, P(c_ll))
     f("hb_debug_bk_profile", c_i, c_vp, c_i, P(c_ll))
+    f("hb_debug_symdense_factor", c_i, c_vp, P(c_i), P(c_i), c_vp, c_vp, c_vp, c_vp)
     f("hb_microbench_peak", c_i, c_vp, c_i, P(c_d))
     # lowrank
     f("hb_lowrank_create", c_i, c_vp, c_ll, c_i, c_i, c_i, P(c_vp))

@@ -618,10 +618,12 @@ bool hb_bkc_supported(int N)
 
 // Bunch-Kaufman factorization P A P^T = L D L^T of the column-major-lower triangle (lda even). Outputs: unit L strictly below the
 // diagonal (zeros below 2x2 blocks), D on the diagonal + dsub, ipiv (sign marks 2x2 blocks), perm (gather order for the right-hand
-// side), info_dev (first exactly-zero pivot column, 1-based). Wp: NB x ldw doubles of scratch (W = L*D of the current panel).
+// side), info_dev (first exactly-zero pivot column, 1-based), widths_host (OR of the panel widths launched, in no order; the last launch
+// may find no column left when the device k0 has already reached N). Wp: NB x ldw doubles of scratch (W = L*D of the current panel).
 int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ipiv_dev, double* dsub_dev, int* perm_dev, double* Wp, long long ldw,
-                  int* state_dev /* 4 ints */, int* swaplog_dev, int* info_dev)
+                  int* state_dev /* 4 ints */, int* swaplog_dev, int* info_dev, int* widths_host)
 {
+  *widths_host = 0;
   double* swap_scratch = Wp + (size_t)NBMAX * ldw; // Wp holds NBMAX columns of W followed by 2*NBMAX rows of staging for the interchanges
   HB_REQUIRE((lda & 1) == 0, "hb_bkc_factor: needs an even leading dimension");
   HB_CHECK(hb_big_init(c, b));
@@ -636,6 +638,7 @@ int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ip
     int S, NB;
     size_t smem;
     bkc_geometry(N - k0_min, &S, &NB, &smem);
+    *widths_host |= NB;
     int threads = S < PT ? S : PT; // one row per thread where possible: fewer idle warps in every barrier / shuffle stage
     if(threads < 128) threads = 128;
     if(c->bkc_prof) k_bk_panel<true><<<CS, threads, smem, st>>>(A, lda, N, Wp, ldw, NB, S, ipiv_dev, dsub_dev, state_dev, swaplog_dev, p, c->bkc_prof);

@@ -128,7 +128,7 @@ int hb_big_solve(hb_ctx* c, hb_big* b, int N, const double* F, long long ldf, in
 int hb_bkc_init_attrs(hb_ctx* c);
 bool hb_bkc_supported(int N);
 int hb_bkc_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int* ipiv_dev, double* dsub_dev, int* perm_dev, double* Wp, long long ldw,
-                  int* state_dev, int* swaplog_dev, int* info_dev);
+                  int* state_dev, int* swaplog_dev, int* info_dev, int* widths_host);
 int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, double* x);
 int hb_bkc_profile(hb_ctx* c, int on, long long* prof_host8);
 #define HB_BKC_SWAPLOG_INTS(N) ((size_t)((N) / 7 + 4) * 132)

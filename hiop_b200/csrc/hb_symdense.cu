@@ -45,6 +45,7 @@ struct Plan
   Factor f;
   Solve s;
   Inertia in;
+  bool pairs; // look-ahead factorization: 128-column blocks in pairs
 };
 
 bool coop_factor(const hb_ctx* c, int N) { return c->coop_ctas > 0 && N >= COOP_MIN_N && N <= COOP_FACTOR_MAX_N; }
@@ -52,13 +53,13 @@ bool coop_factor(const hb_ctx* c, int N) { return c->coop_ctas > 0 && N >= COOP_
 Plan symdense_plan(const hb_ctx* c, int mode, int N)
 {
   if(mode == HB_FACT_BUNCH_KAUFMAN) {
-    if(N >= c->bk_cluster_min && hb_bkc_supported(N)) return {F_BK_CLUSTER, S_BIG, I_BLOCKDIAG};
-    return {N >= BLOCKED_BK_MIN_N ? F_SYTRF_BLOCKED : F_SYTF2, S_SYTRS, I_IPIV};
+    if(N >= c->bk_cluster_min && hb_bkc_supported(N)) return {F_BK_CLUSTER, S_BIG, I_BLOCKDIAG, false};
+    return {N >= BLOCKED_BK_MIN_N ? F_SYTRF_BLOCKED : F_SYTF2, S_SYTRS, I_IPIV, false};
   }
   const bool ldl = mode == HB_FACT_NOPIV;
-  if(N >= (ldl ? c->big_min_ldl : c->big_min_chol)) return {ldl ? F_BIG_LDL : F_BIG_CHOL, S_BIG, I_DIAG};
+  if(N >= (ldl ? c->big_min_ldl : c->big_min_chol)) return {ldl ? F_BIG_LDL : F_BIG_CHOL, S_BIG, I_DIAG, N >= c->pair_min};
   const Factor f = ldl ? F_PANEL_LDL : coop_factor(c, N) ? F_COOP_CHOL : F_PANEL_CHOL;
-  return {f, N >= BIG_SOLVE_MIN_N ? S_BIG : S_ONE_CTA, I_DIAG};
+  return {f, N >= BIG_SOLVE_MIN_N ? S_BIG : S_ONE_CTA, I_DIAG, false};
 }
 
 int bk_sytrs(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, double* B, int ldb, int nrhs)
@@ -149,6 +150,7 @@ struct hb_symdense
   hb_dev<int> info;         // device: [0] info, [1..3] inertia
   hb_pinned<int> info_host;
   int mode = -1;
+  int bk_widths = 0;        // cluster Bunch-Kaufman: OR of the panel widths (8 / 16 / 32 / 64) the last factorization launched (no order)
   bool factored = false;
   int n_neg = 0, n_null = 0, n_pos = 0;
 };
@@ -193,6 +195,7 @@ extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
   s->F = s->M; s->ldf = N; s->big.inv_valid = false;
   const Plan p = symdense_plan(c, mode, N);
   s->plan = p;
+  s->bk_widths = 0;
   const bool big = p.f == F_BIG_CHOL || p.f == F_BIG_LDL;
   if((big || p.f == F_BK_CLUSTER) && (N & 1)) { // even leading dimension for the 16-byte operand copies
     const long long ld = (N + 7) & ~7LL;
@@ -216,13 +219,14 @@ extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
   case F_SYTF2: HB_CHECK(hb_dense_sytf2(c, N, s->M, N, s->ipiv, s->info)); break;
   case F_SYTRF_BLOCKED: HB_CHECK(hb_dense_sytrf_blocked(c, N, s->M, N, s->ipiv, s->W, s->info)); break;
   case F_BK_CLUSTER:
-    HB_CHECK(hb_bkc_factor(c, &s->big, N, s->F, s->ldf, s->ipiv, s->dsub, s->perm, s->Wp, ldw, s->bk_state, s->swaplog, s->info));
+    HB_CHECK(hb_bkc_factor(c, &s->big, N, s->F, s->ldf, s->ipiv, s->dsub, s->perm, s->Wp, ldw, s->bk_state, s->swaplog, s->info,
+                           &s->bk_widths));
     break;
   case F_PANEL_CHOL:
   case F_PANEL_LDL: HB_CHECK(hb_dense_factor_panel(c, N, s->M, N, p.f == F_PANEL_LDL, s->W, s->info)); break;
   case F_COOP_CHOL: HB_CHECK(hb_dense_chol_coop(c, N, s->M, N, s->info, nullptr, nullptr)); break;
   case F_BIG_CHOL:
-  case F_BIG_LDL: HB_CHECK(hb_big_factor(c, &s->big, N, s->F, s->ldf, p.f == F_BIG_LDL, N >= c->pair_min, s->info)); break;
+  case F_BIG_LDL: HB_CHECK(hb_big_factor(c, &s->big, N, s->F, s->ldf, p.f == F_BIG_LDL, p.pairs, s->info)); break;
   }
   // the blocked solve needs the 128 x 128 diagonal inverses; only the look-ahead factorization forms them itself
   if(p.s == S_BIG && !big) HB_CHECK(hb_big_block_inverses(c, &s->big, N, s->F, s->ldf, mode != HB_FACT_CHOLESKY));
@@ -300,6 +304,28 @@ extern "C" int hb_debug_diag128_profile(hb_symdense* s, int ldl, long long* prof
 {
   HB_REQUIRE(s && prof_host8 && s->N >= 128 && (s->N & 1) == 0, "hb_debug_diag128_profile: needs an even N >= 128");
   return hb_big_diag_profile(s->ctx, &s->big, s->N, s->M, s->N, 0, ldl != 0, prof_host8);
+}
+// diagnostics (tests): what the last hb_symdense_matrix_changed chose and computed. Every output pointer may be NULL.
+extern "C" int hb_debug_symdense_factor(hb_symdense* s, int* plan4, int* bk_widths, double* F_host, int* ipiv_host, int* perm_host,
+                                        double* dsub_host)
+{
+  HB_REQUIRE(s && s->N > 0 && s->F, "hb_debug_symdense_factor: no factorization of a non-empty matrix yet");
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  if(plan4) { plan4[0] = s->plan.f; plan4[1] = s->plan.s; plan4[2] = s->plan.in; plan4[3] = s->plan.pairs; }
+  if(bk_widths) *bk_widths = s->bk_widths;
+  HB_CUDA(cudaSetDevice(c->device));
+  if(F_host)
+    HB_CUDA(cudaMemcpy2DAsync(F_host, sizeof(double) * N, s->F, sizeof(double) * s->ldf, sizeof(double) * N, N, cudaMemcpyDeviceToHost, c->stream));
+  const bool bk = s->plan.f == F_SYTF2 || s->plan.f == F_SYTRF_BLOCKED || s->plan.f == F_BK_CLUSTER;
+  HB_REQUIRE(bk || !ipiv_host, "hb_debug_symdense_factor: ipiv exists only for the Bunch-Kaufman factors");
+  if(ipiv_host) HB_CUDA(cudaMemcpyAsync(ipiv_host, s->ipiv, sizeof(int) * N, cudaMemcpyDeviceToHost, c->stream));
+  const bool bkc = s->plan.f == F_BK_CLUSTER;
+  HB_REQUIRE(bkc || (!perm_host && !dsub_host), "hb_debug_symdense_factor: perm / dsub exist only for the cluster Bunch-Kaufman factor");
+  if(perm_host) HB_CUDA(cudaMemcpyAsync(perm_host, s->perm, sizeof(int) * N, cudaMemcpyDeviceToHost, c->stream));
+  if(dsub_host) HB_CUDA(cudaMemcpyAsync(dsub_host, s->dsub, sizeof(double) * N, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return HB_OK;
 }
 extern "C" int hb_debug_bk_profile(hb_ctx* c, int on, long long* prof_host8)
 {

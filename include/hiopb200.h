@@ -189,6 +189,13 @@ int hb_symdense_solve_host(hb_symdense* s, double* x_host, int nrhs);
  * (the 128 x 128 diagonal-block kernel on the leading block of M; the cluster Bunch-Kaufman panel, summed over a factorization) */
 int hb_debug_diag128_profile(hb_symdense* s, int ldl, long long* prof_host8);
 int hb_debug_bk_profile(hb_ctx* ctx, int on, long long* prof_host8);
+/* diagnostics (tests): the last factorization of s, read back (synchronises the stream; every output may be NULL).
+ * plan4: factor, solve and inertia kernels of the dispatch table in hb_symdense.cu (enum order there), 1 if the look-ahead
+ * factorization took its blocks in pairs. bk_widths: OR of the cluster Bunch-Kaufman panel widths {8, 16, 32, 64} launched, in no
+ * order and possibly including a last panel that found no column left (0 for the other paths). F_host: the N x N factor, row-major
+ * with the upper triangle valid as M (unpadded for odd N). ipiv_host: N pivots (LAPACK's convention), Bunch-Kaufman only.
+ * perm_host / dsub_host: N entries each, cluster Bunch-Kaufman only. */
+int hb_debug_symdense_factor(hb_symdense* s, int* plan4, int* bk_widths, double* F_host, int* ipiv_host, int* perm_host, double* dsub_host);
 
 /* ------------------------------------------------------------------------------------------------------------
  * hiopKKTLinSysLowRank + hiopHessianLowRank (B2; src/Optimization/hiopKKTLinSys.cpp:1031-1350,
