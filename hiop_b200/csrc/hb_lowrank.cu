@@ -1091,6 +1091,7 @@ extern "C" const double* hb_lowrank_Dx(hb_lowrank* k) { return k ? k->Dx.get() :
 extern "C" const double* hb_lowrank_DhInv(hb_lowrank* k) { return k ? k->DhInv.get() : nullptr; }
 extern "C" const double* hb_lowrank_Dd_inv(hb_lowrank* k) { return k ? k->Dd_inv.get() : nullptr; }
 extern "C" const double* hb_lowrank_N(hb_lowrank* k) { return k ? k->Nmat.get() : nullptr; }
+extern "C" const double* hb_lowrank_tdot(hb_lowrank* k) { return k ? k->tdot.get() : nullptr; }
 
 // ---- one whole KKT system from host buffers ----------------------------------------------------------------------------
 extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, const double* Jd_host, const double* zl, const double* sxl,

@@ -183,7 +183,10 @@ k_oz_slice(const double* const* __restrict__ rowptr, int M, int Mpad, long long 
   for(int j = 0; j < 8; j++) x[j] = 0.0;
   if(row < M) {
     const double* a = rowptr[row];
-    const double sc = ldexp(1.0, 27 - e[row]);
+    // 2^(27 - e) overflows for e <= -997 (row maximum below 2^-997): such a row is scaled by 2^(27 - e - 512), then by 2^512. Both
+    // products are exact (the first stays below 2^-485, the second below 2^27), so every row gets exactly b * 2^(27 - e).
+    const int es = 27 - e[row];
+    const double sc = ldexp(1.0, es > 1023 ? es - 512 : es);
     if(vec_ok && k0 + 7 < K) {
 #pragma unroll
       for(int j = 0; j < 8; j += 2) {
@@ -197,6 +200,10 @@ k_oz_slice(const double* const* __restrict__ rowptr, int M, int Mpad, long long 
 #pragma unroll
       for(int j = 0; j < 8; j++)
         if(k0 + j < K) x[j] = __dmul_rn(__dmul_rn(a[k0 + j], sd ? sd[k0 + j] : 1.0), sc);
+    }
+    if(es > 1023) {
+#pragma unroll
+      for(int j = 0; j < 8; j++) x[j] = __dmul_rn(x[j], 0x1p512);
     }
   }
   const double MAGIC = 6755399441055744.0; // 1.5 * 2^52

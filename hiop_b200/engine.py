@@ -419,6 +419,10 @@ class KKTLinSysLowRank:
     def N(self):
         m = self.m_eq + self.m_ineq
         return self._readback("hb_lowrank_N", m * m).reshape(m, m)
+    def tdot(self, l: int = 0):
+        """[J; S; Y] (DhInv .* rx) (m + 2l entries, l the current number of secant pairs) of the last solveCompressed that found the
+        condensation pending and fused the row dots into it"""
+        return self._readback("hb_lowrank_tdot", self.m_eq + self.m_ineq + 2 * l)
 
     def last_solve_stats(self):
         a, b = ctypes.c_int(), ctypes.c_double()

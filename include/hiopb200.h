@@ -347,11 +347,14 @@ int hb_lowrank_hess_solve(hb_lowrank* k, const double* rhs, double* x);
 /* y = beta*y + alpha*(B_k [+ D_x]) x in the compact form (same operator as the recursive timesVecCmn :974-1059) */
 int hb_lowrank_hess_times_vec(hb_lowrank* k, double beta, double* y, double alpha, const double* x, int add_log_term);
 /* read-backs (device pointers owned by the engine; valid until destroy): Dx, DhInv (n_local), Dd_inv (m_ineq),
- * N (m x m row-major, full symmetric storage, UNfactorized copy) */
+ * N (m x m row-major, full symmetric storage, UNfactorized copy),
+ * tdot (m + 2l): the row dots [J; S; Y] (DhInv .* rx) that a solveCompressed with a pending condensation took from the condensation's
+ * sweep over the rows (the int8-slice row-maximum pass, or the extra row of the FP64 SYRK when it fits in the last tile); undefined otherwise */
 const double* hb_lowrank_Dx(hb_lowrank* k);
 const double* hb_lowrank_DhInv(hb_lowrank* k);
 const double* hb_lowrank_Dd_inv(hb_lowrank* k);
 const double* hb_lowrank_N(hb_lowrank* k);
+const double* hb_lowrank_tdot(hb_lowrank* k);
 /* statistics of the last solve: refinement steps taken, last residual inf-norm (host) */
 int hb_lowrank_last_solve_stats(hb_lowrank* k, int* n_refine, double* resid_inf);
 /* One whole KKT system from HOST buffers (the e2e path of bench.py and of the C++ adapter when HiOp keeps its data in

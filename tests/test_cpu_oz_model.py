@@ -76,3 +76,96 @@ def test_fused_sweep_identity_for_step_2_of_solveCompressed():
             p = np.concatenate([P.sigma * (P.St @ w), P.Yt @ w])
             got = t_J - Z @ p
         assert np.abs(got - want).max() <= 1e-11 * max(1.0, np.abs(want).max())
+
+
+# ---- the schedule, the bit-exact model and the a-priori bound (oz_model.schedule / condense_bits / truncation_bound) -----------------
+
+@pytest.mark.parametrize("G", [114, 132])
+def test_every_schedule_branch_is_reached(G):
+    """H100 PCIe (114 SMs) and SXM (132 SMs): every branch of hb_syrk_rows_ozaki's schedule has a case, and on 132 SMs the preferred
+    shapes are the ones the kernel's comments and tests name."""
+    got = {}
+    for b, M0, K, S in oz.BRANCH_CASES:
+        M = oz.find_shape(b, M0, K, S, G)
+        got[b] = oz.schedule(M, K, S, G)
+        if G == 132:
+            assert M == M0, (b, M)
+    assert set(got) == set(oz.BRANCHES)
+    if G == 132:
+        assert oz.schedule(100, 20000, 8, 132).splits == 33
+        assert oz.schedule(100, 1000, 8, 132).splits == 8 and oz.schedule(1, 5000, 8, 132).splits == 40
+        s = oz.schedule(1000, 200001, 8, 132)
+        assert (s.splits, len(s.items)) == (11, 1584)
+        assert len(oz.schedule(1000, 12000, 8, 132).items) == 144
+        assert oz.schedule(1260, 140001, 8, 132).max_chunks == 3 and oz.schedule(1260, 140001, 6, 132).max_chunks == 2
+    assert oz.chunk_stages(8) == 511 and oz.chunk_stages(8) * 128 == 65408
+
+
+def test_items_cover_every_tile_and_stage_once():
+    for M, K, S, G in ((1000, 200001, 8, 132), (300, 470001, 8, 114), (33, 4223, 7, 132), (1, 100, 6, 132)):
+        s = oz.schedule(M, K, S, G)
+        cover = {}
+        for bi, bj, kb, kc, slot in s.items:
+            assert kc >= 1 and 0 <= slot < len(s.tiles) * s.splits
+            cover.setdefault((bi, bj), []).append((kb, kc))
+        assert set(cover) == set(s.tiles)
+        for ranges in cover.values():
+            ranges.sort()
+            assert ranges[0][0] == 0 and sum(c for _, c in ranges) == s.kstages
+            assert all(a + c == b for (a, c), (b, _) in zip(ranges, ranges[1:]))
+
+
+def _adversarial(M, K, seed):
+    """rows at 2^-1000 (the row scaling then needs two steps), 1e+-150, an all-zero row, a row with a power-of-two maximum and one whose
+    maximum rounds the first digit word up to 2^27, among rows spanning 6 decades"""
+    B = _B(M, K, seed)
+    B[1] *= 2.0 ** -1000 / np.abs(B[1]).max()
+    B[2] *= 1e150
+    B[3] *= 1e-150
+    B[4] = 0.0
+    B[5, 11] = 2.0 ** np.ceil(np.log2(np.abs(B[5]).max()) + 1)
+    B[6] *= 0.25 / np.abs(B[6]).max()
+    B[6, 7] = 1.0 - 2.0 ** -30
+    return B
+
+
+@pytest.mark.parametrize("S", [6, 7, 8])
+def test_truncation_bound_holds_on_adversarial_rows_and_is_not_vacuous(S):
+    B = _adversarial(12, 3000, 4)
+    e, Q = oz.digits(B, S)
+    assert oz.row_exponents(B)[1] == -999 and Q[0, 6].max() == 64
+    sch = oz.schedule(12, 3000, S, 132)
+    C = oz.condense_bits(B, S, sch, dig=(e, Q))
+    assert np.all(np.isfinite(C)) and np.array_equal(C, C.T)
+    G, err = oz.exact_gram(B)
+    R, _ = oz.truncation_bound(B, S, sch.chain, dig=(e, Q))
+    tol = np.ldexp(R, e[:, None] + e[None, :]) + 2.0 ** -1075 + err
+    ratio = np.abs(C - G) / tol
+    assert ratio.max() <= 1.0, ratio.max()
+    # not vacuous: the bound is within 100x of the error somewhere, and dropping the last anti-diagonal breaks it
+    assert ratio.max() >= 1e-2, ratio.max()
+    Cd = oz.condense_bits(B, S, sch, dig=(e, Q), drop_t=S - 1)
+    assert (np.abs(Cd - G) / tol).max() > 1.0
+    # the row at 2^-1000 is sliced exactly like any other row: its digits are those of the row scaled to 1
+    e1, Q1 = oz.digits(np.ldexp(B[1:2], 1000), S)         # max 2^-1000 = 0.5 2^-999: e = -999 <= -997
+    np.testing.assert_array_equal(Q1[:, 0], Q[:, 1])
+
+
+def test_mutations_change_the_bits():
+    """Dropping anti-diagonal S-1, summing the splits in reverse order or cutting K into 65536-column chunks (instead of the device's
+    65408) each changes condense_bits on seeded inputs: the bit-exact GPU comparison would catch each of these kernels."""
+    B = _B(100, 20000, 5)
+    S = 8
+    sch = oz.schedule(100, 20000, S, 132)
+    assert sch.splits == 33
+    dig = oz.digits(B, S)
+    C = oz.condense_bits(B, S, sch, dig=dig)
+    assert not np.array_equal(C, oz.condense_bits(B, S, sch, dig=dig, drop_t=S - 1))
+    assert not np.array_equal(C, oz.condense_bits(B, S, sch, dig=dig, split_order=range(sch.splits - 1, -1, -1)))
+    B2 = _B(16, 70000, 6)
+    C1, _ = oz.gram(B2, S)
+    C2, _ = oz.gram(B2, S, chunk_cols=65536)
+    assert not np.array_equal(C1, C2)
+    sch2 = oz.schedule(16, 70000, S, 1)                      # one SM: one split, the device's two chunks
+    assert sch2.splits == 1 and sch2.max_chunks == 2
+    np.testing.assert_array_equal(oz.condense_bits(B2, S, sch2), C1)
