@@ -14,6 +14,7 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "hiopb200.h")
 
 HB_OK = 0
 HB_FACT_BUNCH_KAUFMAN, HB_FACT_NOPIV, HB_FACT_CHOLESKY = 0, 1, 2
+HB_CONDENSE_AUTO, HB_CONDENSE_FP64_DMMA, HB_CONDENSE_INT8_CRT = -1, 0, 100
 
 c_dp = ctypes.c_void_p   # device or host pointer to doubles (passed as integer address)
 c_ll = ctypes.c_longlong

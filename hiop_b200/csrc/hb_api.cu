@@ -41,6 +41,7 @@ extern "C" int hb_ctx_create(int device, hb_ctx** out)
   HB_CHECK(c->red_host.reserve(c.get(), 64, "reduction landing slots"));
   HB_CHECK(hb_syrk_init_attrs(c.get()));
   HB_CHECK(hb_ozaki_init_attrs(c.get()));
+  HB_CHECK(hb_crt_init_attrs(c.get()));
   HB_CHECK(hb_microbench_init_attrs(c.get()));
   HB_CHECK(hb_dense_init(c.get()));
   *out = c.release();
@@ -79,7 +80,7 @@ extern "C" int hb_ctx_last_syrk_ms(hb_ctx* c, float* ms)
 
 // Timeline of one quasi-Newton step: with on != 0 the engine records an event after each phase of hb_lowrank_update / condense /
 // solve_compressed; hb_ctx_phase_timeline(ctx, 0, ms) waits for them and returns the phase durations (ms) in the order
-// update, row maxima (+ fused row dots), slicing, GEMM + fix-up [= C_aug; the first two only with the int8-slice kernel, otherwise the whole
+// update, row maxima (+ fused row dots), slicing / residues, GEMM + fix-up [= C_aug; the first two only with the int8 kernels, otherwise the whole
 // condensation is in the third], all-reduce, V/U/N assembly, Cholesky, H^-1 rx, J dx (+ all-reduce), SPD solve, J^T dy, H^-1 rx (second).
 // A mark that was not passed contributes 0 and its time is counted in the next recorded phase.
 extern "C" int hb_ctx_phase_timeline(hb_ctx* c, int on, float* ms_host10)

@@ -123,10 +123,13 @@ private:
 using hb_stream = hb_handle<cudaStream_t>;
 using hb_event = hb_handle<cudaEvent_t>;
 
-// per-context state defined in one kernel file each: the int8-slice condensation (hb_ozaki.cu), the SYRK schedule cache (hb_syrk.cu)
+// per-context state defined in one kernel file each: the int8-slice condensation (hb_ozaki.cu), the Chinese-remainder int8
+// condensation (hb_crt.cu), the SYRK schedule cache (hb_syrk.cu)
 struct OzState;
+struct CrtState;
 struct ScheduleCache;
 void hb_delete(OzState* p);
+void hb_delete(CrtState* p);
 void hb_delete(ScheduleCache* p);
 struct hb_deleter
 {
@@ -157,6 +160,8 @@ struct hb_ctx
   unsigned phase_mask = 0;
   // per-context state of the int8-slice condensation (hb_ozaki.cu): slice buffer, exponents, tensor maps, work list
   hb_state<OzState> oz;
+  // per-context state of the Chinese-remainder condensation (hb_crt.cu): residue planes, exponents, tensor maps, work list
+  hb_state<CrtState> crt;
   // schedule cache of the FP64 condensation (hb_syrk.cu)
   hb_state<ScheduleCache> syrk_sched;
   // dense symmetric solvers: size thresholds (with their environment overrides, set by hb_dense_init in hb_symdense.cu) and the
@@ -215,11 +220,27 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
 bool hb_syrk_extra_row_is_free(int M);
 int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
                        const double* dot_x, double* dot_out);
+// the same contract on the int8 tensor cores by Chinese remaindering (hb_crt.cu): the correctly rounded value of an exact integer Gram
+int hb_syrk_rows_crt(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc,
+                     const double* dot_x, double* dot_out);
+
+// Step 1 of both int8 condensations (hb_ozaki.cu): sd = sqrt(d) (when d is given), the exact row maxima of |a_ik| sd_k and their
+// frexp exponents e_i, and optionally dot_out[i] = sum_k a_ik d_k dot_x_k from the same sweep. Marks HB_PH_OZ_ROWMAX.
+struct hb_rowscale
+{
+  hb_dev<double> sd;
+  hb_dev<unsigned long long> mx;
+  hb_dev<int> e;
+  hb_dev<double> dot_partial; // [chunks][M] partial row dots of the fused row-maximum pass
+};
+int hb_row_exponents(hb_ctx* c, hb_rowscale& rs, int M, int Mpad, long long K, const double* const* rowptr_dev, bool rows_aligned16,
+                     const double* d, const double* dot_x, double* dot_out, const double** sd_out);
 
 // set once by hb_ctx_create: the dynamic-shared-memory / cluster attributes of each kernel file's kernels (function attributes are
 // per device) and the dense solvers' thresholds
 int hb_syrk_init_attrs(hb_ctx* c);
 int hb_ozaki_init_attrs(hb_ctx* c);
+int hb_crt_init_attrs(hb_ctx* c);
 int hb_microbench_init_attrs(hb_ctx* c);
 int hb_dense_init(hb_ctx* c);
 

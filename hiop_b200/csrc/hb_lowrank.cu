@@ -678,10 +678,16 @@ int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
       k->tdot_valid = fuse;
     } else {
       const hb_rowtab* rows;
-      HB_CHECK(jac_whole(k, "hb_lowrank_condense: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)", nullptr, &rows));
+      HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT
+                                ? "hb_lowrank_condense: the int8 Chinese-remainder condensation (mode 100; AUTO and 0 condense in FP64)"
+                                : "hb_lowrank_condense: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)",
+                         nullptr, &rows));
       const bool fuse = fuse_rx && m > 0;
       if(fuse && k->n == 0) HB_CUDA(cudaMemsetAsync(k->tdot, 0, sizeof(double) * Ma, c->stream));
-      HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
+      if(mode == HB_CONDENSE_INT8_CRT)
+        HB_CHECK(hb_syrk_rows_crt(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
+      else
+        HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
       k->tdot_valid = fuse;
     }
     k->condense_used = mode;
@@ -752,8 +758,9 @@ extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_i
   std::unique_ptr<hb_lowrank> k(new hb_lowrank);
   k->ctx = c; k->n = n_local; k->meq = m_eq; k->mineq = m_ineq; k->m = m_eq + m_ineq; k->lmax = l_max;
   k->jl = device_layout(n_local, nullptr);
-  if(const char* e = getenv("HB_CONDENSE")) { // "oz6" | "oz7" | "oz8" | "dmma"
+  if(const char* e = getenv("HB_CONDENSE")) { // "oz6" | "oz7" | "oz8" | "crt" | "dmma"
     if(e[0] == 'o' && e[1] == 'z' && e[2] >= '6' && e[2] <= '8') k->condense_mode = e[2] - '0';
+    else if(strcmp(e, "crt") == 0) k->condense_mode = HB_CONDENSE_INT8_CRT;
     else if(e[0] == 'd') k->condense_mode = 0;
   }
   const int m = k->m, Mamax = m + 2 * l_max, l2 = 2 * l_max;
@@ -929,8 +936,12 @@ extern "C" int hb_lowrank_update(hb_lowrank* k, const double* zl, const double* 
 
 extern "C" int hb_lowrank_set_condense_mode(hb_lowrank* k, int mode)
 {
-  HB_REQUIRE(k && (mode == -1 || mode == 0 || mode == 6 || mode == 7 || mode == 8), "hb_lowrank_set_condense_mode: mode must be -1, 0, 6, 7 or 8");
-  if(mode > 0) HB_CHECK(jac_whole(k, "hb_lowrank_set_condense_mode: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)"));
+  HB_REQUIRE(k && (mode == -1 || mode == 0 || mode == 6 || mode == 7 || mode == 8 || mode == HB_CONDENSE_INT8_CRT),
+             "hb_lowrank_set_condense_mode: mode must be -1, 0, 6, 7, 8 or 100");
+  if(mode > 0)
+    HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT
+                              ? "hb_lowrank_set_condense_mode: the int8 Chinese-remainder condensation (mode 100; AUTO and 0 condense in FP64)"
+                              : "hb_lowrank_set_condense_mode: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)"));
   k->condense_mode = mode;
   k->cond_valid = false;
   return HB_OK;

@@ -60,7 +60,7 @@ struct hb_lowrank
   hb_dev<double> mi1, mi2; // m_ineq scratch
   int md_grid = 0;
   bool have_update = false, cond_valid = false, mdir_valid = false;
-  int condense_mode = -1; // -1 = auto, 0 = FP64 DMMA, 6/7/8 = INT8-slice wgmma
+  int condense_mode = -1; // -1 = auto, 0 = FP64 DMMA, 6/7/8 = INT8-slice wgmma, 100 = INT8 Chinese remaindering
   int condense_used = 0;
   bool check_pending = false; // an asynchronous condensation left its info words unchecked
   hb_dev<double> tri;  // packed upper triangle of C_aug for the all-reduce

@@ -53,8 +53,10 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   if(mode == 0) HB_CHECK(jac_syrk(k, m, nullptr, M));
   else {
     const hb_rowtab* rows;
-    HB_CHECK(jac_whole(k, "hb_lowrank_lsq_duals: the int8-slice modes 6-8", nullptr, &rows));
-    HB_CHECK(hb_syrk_rows_ozaki(c, m, n, rows->dev, rows->aligned, nullptr, M, m, mode, nullptr, nullptr));
+    HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT ? "hb_lowrank_lsq_duals: the int8 Chinese-remainder mode 100" : "hb_lowrank_lsq_duals: the int8-slice modes 6-8",
+                       nullptr, &rows));
+    if(mode == HB_CONDENSE_INT8_CRT) HB_CHECK(hb_syrk_rows_crt(c, m, n, rows->dev, rows->aligned, nullptr, M, m, nullptr, nullptr));
+    else HB_CHECK(hb_syrk_rows_ozaki(c, m, n, rows->dev, rows->aligned, nullptr, M, m, mode, nullptr, nullptr));
   }
   HB_CHECK(hb_allreduce_sum(c, M, (long long)m * m));
   // rhs = -J vecx (all-reduced), then the d-side terms on the replicated part

@@ -422,10 +422,7 @@ struct OzState
   long long K = -1, Kpad = 0;
   int Mpad = 0;
   hb_dev<int8_t> Q;
-  hb_dev<double> sd;
-  hb_dev<unsigned long long> mx;
-  hb_dev<int> e;
-  hb_dev<double> dot_partial; // [chunks][M] partial row dots of the fused row-maximum pass
+  hb_rowscale rs;
   hb_dev<OzItem> d_items;
   hb_dev<int2> d_tiles;
   CUtensorMap mapA, mapB;
@@ -446,6 +443,47 @@ int launch_gemm(hb_ctx* c, OzState& st, int chunk_blocks, double* partial)
 }
 
 } // namespace
+
+// Step 1 of both int8 condensations: the launches and bits are those the slice path has always made
+int hb_row_exponents(hb_ctx* c, hb_rowscale& rs, int M, int Mpad, long long K, const double* const* rowptr_dev, bool rows_aligned16,
+                     const double* d, const double* dot_x, double* dot_out, const double** sd_out)
+{
+  HB_CHECK(rs.sd.reserve(c, K, "sqrt(d)"));
+  HB_CHECK(rs.mx.reserve(c, Mpad, "row maxima"));
+  HB_CHECK(rs.e.reserve(c, Mpad, "row exponents"));
+  const double* sd = nullptr;
+  if(d) {
+    k_sqrt<<<c->num_sms * 8, 256, 0, c->stream>>>(K, d, rs.sd);
+    HB_LAUNCHED();
+    sd = rs.sd;
+  }
+  HB_CUDA(cudaMemsetAsync(rs.mx, 0, sizeof(unsigned long long) * Mpad, c->stream));
+  if(dot_x && dot_out && K > 0) {
+    const int nchunks = (int)((K + RD_COLS - 1) / RD_COLS);
+    HB_CHECK(rs.dot_partial.reserve(c, (size_t)nchunks * M, "fused row-dot partials"));
+    int rsplit = (2 * c->num_sms + nchunks - 1) / nchunks; // short shards: split the rows of a chunk over several CTAs
+    rsplit = rsplit < 1 ? 1 : (rsplit > 8 ? 8 : rsplit);
+    // pairs of columns need 16-byte aligned rows AND an even first column per lane (RD_COLS is even)
+    if(rows_aligned16 && (K & 1) == 0)
+      k_oz_rowmax_dot<true><<<dim3(nchunks, rsplit), RD_THREADS, 0, c->stream>>>(rowptr_dev, M, K, d, dot_x, rs.mx, rs.dot_partial);
+    else
+      k_oz_rowmax_dot<false><<<dim3(nchunks, rsplit), RD_THREADS, 0, c->stream>>>(rowptr_dev, M, K, d, dot_x, rs.mx, rs.dot_partial);
+    HB_LAUNCHED();
+    k_oz_dot_final<<<(M + 31) / 32, 256, 0, c->stream>>>(M, nchunks, rs.dot_partial, dot_out);
+    HB_LAUNCHED();
+  } else {
+    long long gx = (K + 256 * 64 - 1) / (256 * 64);
+    if(gx < 1) gx = 1;
+    if(gx > 64) gx = 64;
+    k_oz_rowmax<<<dim3((unsigned)gx, M), 256, 0, c->stream>>>(rowptr_dev, M, K, sd, rs.mx);
+    HB_LAUNCHED();
+  }
+  k_oz_exponents<<<(Mpad + 127) / 128, 128, 0, c->stream>>>(M, rs.mx, rs.e);
+  HB_LAUNCHED();
+  hb_phase_mark(c, HB_PH_OZ_ROWMAX);
+  *sd_out = sd;
+  return HB_OK;
+}
 
 int hb_ozaki_init_attrs(hb_ctx* c)
 {
@@ -480,9 +518,6 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     st.M = -1; // the tensor maps hold the address of Q
     HB_CHECK(st.Q.reserve(c, qbytes, "the int8 slice buffer"));
   }
-  HB_CHECK(st.sd.reserve(c, K, "sqrt(d)"));
-  HB_CHECK(st.mx.reserve(c, Mpad, "row maxima"));
-  HB_CHECK(st.e.reserve(c, Mpad, "row exponents"));
   if(st.M != M || st.K != K || st.S != S) {
     // schedule: tiles (bi, bj) with bj >= (TM / TN) bi cover the upper triangle; split K so that ~all SMs get one item
     st.M = -1;
@@ -544,45 +579,15 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     st.M = M; st.K = K; st.S = S; st.Mpad = Mpad; st.Kpad = Kpad; st.splits = splits; st.n_tiles = nt; st.n_items = (int)items.size();
   }
   // 1. sqrt(d), row maxima, exponents, slices
-  const double* sd = nullptr;
-  if(d) {
-    k_sqrt<<<c->num_sms * 8, 256, 0, c->stream>>>(K, d, st.sd);
-    HB_LAUNCHED();
-    sd = st.sd;
-  }
-  HB_CUDA(cudaMemsetAsync(st.mx, 0, sizeof(unsigned long long) * Mpad, c->stream));
-  {
-    if(dot_x && dot_out && K > 0) {
-      const int nchunks = (int)((K + RD_COLS - 1) / RD_COLS);
-      HB_CHECK(st.dot_partial.reserve(c, (size_t)nchunks * M, "fused row-dot partials"));
-      int rsplit = (2 * c->num_sms + nchunks - 1) / nchunks; // short shards: split the rows of a chunk over several CTAs
-      rsplit = rsplit < 1 ? 1 : (rsplit > 8 ? 8 : rsplit);
-      // pairs of columns need 16-byte aligned rows AND an even first column per lane (RD_COLS is even)
-      if(rows_aligned16 && (K & 1) == 0)
-        k_oz_rowmax_dot<true><<<dim3(nchunks, rsplit), RD_THREADS, 0, c->stream>>>(rowptr_dev, M, K, d, dot_x, st.mx, st.dot_partial);
-      else
-        k_oz_rowmax_dot<false><<<dim3(nchunks, rsplit), RD_THREADS, 0, c->stream>>>(rowptr_dev, M, K, d, dot_x, st.mx, st.dot_partial);
-      HB_LAUNCHED();
-      k_oz_dot_final<<<(M + 31) / 32, 256, 0, c->stream>>>(M, nchunks, st.dot_partial, dot_out);
-      HB_LAUNCHED();
-    } else {
-      long long gx = (K + 256 * 64 - 1) / (256 * 64);
-      if(gx < 1) gx = 1;
-      if(gx > 64) gx = 64;
-      k_oz_rowmax<<<dim3((unsigned)gx, M), 256, 0, c->stream>>>(rowptr_dev, M, K, sd, st.mx);
-      HB_LAUNCHED();
-    }
-    k_oz_exponents<<<(Mpad + 127) / 128, 128, 0, c->stream>>>(M, st.mx, st.e);
-    HB_LAUNCHED();
-    hb_phase_mark(c, HB_PH_OZ_ROWMAX);
-    const unsigned sx = (unsigned)((Kpad / 8 + 255) / 256);
-    const int vec_ok = rows_aligned16 ? 1 : 0;
-    if(S == 6) k_oz_slice<6><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.e, st.Q, vec_ok);
-    else if(S == 7) k_oz_slice<7><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.e, st.Q, vec_ok);
-    else k_oz_slice<8><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.e, st.Q, vec_ok);
-    HB_LAUNCHED();
-    hb_phase_mark(c, HB_PH_OZ_SLICE);
-  }
+  const double* sd;
+  HB_CHECK(hb_row_exponents(c, st.rs, M, Mpad, K, rowptr_dev, rows_aligned16, d, dot_x, dot_out, &sd));
+  const unsigned sx = (unsigned)((Kpad / 8 + 255) / 256);
+  const int vec_ok = rows_aligned16 ? 1 : 0;
+  if(S == 6) k_oz_slice<6><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
+  else if(S == 7) k_oz_slice<7><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
+  else k_oz_slice<8><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
+  HB_LAUNCHED();
+  hb_phase_mark(c, HB_PH_OZ_SLICE);
   // 2. wgmma GEMM into FP64 partial tiles
   HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)st.n_items * TM * TN));
   // (t+1) * Kc * 2^12 < 2^31 with t+1 <= S  ->  Kc <= 2^19 / S columns
@@ -599,7 +604,7 @@ int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowpt
     c->syrk_timed = true;
   }
   // 3. split-K reduction, row scales, symmetrisation
-  k_oz_fixup<<<st.n_tiles, 256, 0, c->stream>>>(M, st.n_tiles, st.d_tiles, st.splits, (const double*)c->ws, st.e, C, ldc);
+  k_oz_fixup<<<st.n_tiles, 256, 0, c->stream>>>(M, st.n_tiles, st.d_tiles, st.splits, (const double*)c->ws, st.rs.e, C, ldc);
   HB_LAUNCHED();
   return HB_OK;
 }

@@ -347,8 +347,11 @@ class KKTLinSysLowRank:
         check(self.ctx.L.hb_lowrank_update(self.h, *[_ptr(t) for t in (zl, sxl, zu, sxu, vl, sdl, vu, sdu)]), "hb_lowrank_update")
         return True
 
+    CONDENSE_AUTO, CONDENSE_FP64_DMMA, CONDENSE_INT8_CRT = _lib.HB_CONDENSE_AUTO, _lib.HB_CONDENSE_FP64_DMMA, _lib.HB_CONDENSE_INT8_CRT
+
     def set_condense_mode(self, mode: int):
-        """-1 = auto (default: exact FP64 on the DMMA pipe); 0 = exact FP64 on the DMMA pipe; 6/7/8 = INT8-slice emulation on wgmma with that many slices."""
+        """-1 = auto (default: exact FP64 on the DMMA pipe); 0 = exact FP64 on the DMMA pipe; 6/7/8 = INT8-slice emulation on wgmma with that many slices;
+        100 (CONDENSE_INT8_CRT) = int8 Chinese remaindering: the correctly rounded exact Gram of the rows rounded to t(K) bits."""
         check(self.ctx.L.hb_lowrank_set_condense_mode(self.h, int(mode)), "hb_lowrank_set_condense_mode")
 
     def condense_mode_used(self) -> int:

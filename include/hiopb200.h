@@ -60,12 +60,12 @@ void* hb_ctx_stream(hb_ctx* ctx);
 int hb_ctx_device(hb_ctx* ctx);
 
 /* Kernel-level timing for roofline reporting: when enabled, CUDA events bracket the dominant kernel of the condensation -- whichever
- * ran: the FP64 DMMA SYRK (k_syrk_ws) or the int8-slice wgmma GEMM (k_oz_gemm) -- on the context stream; hb_ctx_last_syrk_ms waits
+ * ran: the FP64 DMMA SYRK (k_syrk_ws), the int8-slice wgmma GEMM (k_oz_gemm) or the CRT GEMM (k_crt_gemm) -- on the context stream; hb_ctx_last_syrk_ms waits
  * for it and returns its device duration. */
 int hb_ctx_enable_timing(hb_ctx* ctx, int on);
 /* Per-phase timeline of one quasi-Newton step (per-rank evidence for the multi-GPU runs): hb_ctx_phase_timeline(ctx, 1, NULL) arms the
  * marks, the next hb_lowrank_update + condense + solve_compressed records an event after each phase, hb_ctx_phase_timeline(ctx, 0, ms)
- * returns 12 durations in ms: update, row maxima (+ fused row dots), slicing, GEMM + fix-up (the whole condensation with the FP64 kernel),
+ * returns 12 durations in ms: update, row maxima (+ fused row dots), slicing / residues, GEMM + fix-up (the whole condensation with the FP64 kernel),
  * all-reduce, V/U/N assembly, Cholesky, H^-1 rx, J dx (+ all-reduce), SPD solve, J^T dy, H^-1 rx (second). */
 int hb_ctx_phase_timeline(hb_ctx* ctx, int on, float* ms_host10);
 int hb_ctx_last_syrk_ms(hb_ctx* ctx, float* ms_host);
@@ -303,9 +303,17 @@ int hb_lowrank_condense(hb_lowrank* k);
 /* How the GEMM-shaped part of the condensation is computed:
  *   HB_CONDENSE_FP64_DMMA (0): exact FP64 on the DMMA pipe (mma.sync.m8n8k4.f64);
  *   6, 7, 8: INT8-slice (Ozaki) emulation on the Hopper integer tensor cores (wgmma) with that many 7-bit slices -- exact integer
- *   products/accumulation in registers, truncation of the operands 2^-41 / 2^-48 / 2^-55 relative to each row's largest entry. */
+ *   products/accumulation in registers, truncation of the operands 2^-41 / 2^-48 / 2^-55 relative to each row's largest entry;
+ *   HB_CONDENSE_INT8_CRT (100): Chinese remaindering on the int8 tensor cores. Each row of B = [J;S;Y] sqrt(DhInv) (K = n_local
+ *   columns) is rounded to q_i = rint(b_i 2^(t - e_i)), e_i the frexp exponent of its largest entry, t = min(53, floor((126 -
+ *   ceil(log2 K)) / 2)); X = q q^T is formed exactly from one int8 GEMM per modulus (16 moduli for K <= 340108, 17 up to 2^20) and
+ *   C_ij = ldexp(RN(X_ij), e_i + e_j - 2t), so |C_ij - (B B^T)_ij| <= sum_k (|b_ik| 2^(e_j-t-1) + |b_jk| 2^(e_i-t-1) +
+ *   2^(e_i+e_j-2t-2)) + u |C_ij|. C is a function of (J, DhInv) alone: the same bits for every tile schedule, K split and device.
+ *   The residue planes take N (m + 2l) n_local bytes (about 17 GB at n = 1e6, m + 2l = 1012).
+ *   The int8 modes need the row maxima of a device-resident J: with hb_lowrank_set_jacobian_host they are refused (HB_ERR_INVALID). */
 #define HB_CONDENSE_AUTO (-1)      /* default: exact FP64 DMMA (on H100 faster than the int8-slice emulation at the sizes measured) */
 #define HB_CONDENSE_FP64_DMMA 0
+#define HB_CONDENSE_INT8_CRT 100
 int hb_lowrank_set_condense_mode(hb_lowrank* k, int mode);
 /* hb_lowrank_condense is synchronous: it returns HB_ERR_NUMERIC when V is singular or N is not numerically SPD.
  * hb_lowrank_condense_async only enqueues the work (no host synchronisation; this is also what an implicit condensation
@@ -313,7 +321,7 @@ int hb_lowrank_set_condense_mode(hb_lowrank* k, int mode);
  * calls that synchronise. */
 int hb_lowrank_condense_async(hb_lowrank* k);
 int hb_lowrank_check(hb_lowrank* k);
-/* the mode the last hb_lowrank_condense actually used (0, 6, 7 or 8) */
+/* the mode the last hb_lowrank_condense actually used (0, 6, 7, 8 or 100) */
 int hb_lowrank_get_condense_mode(hb_lowrank* k);
 /* solveCompressed(rx,ryc,ryd -> dx,dyc,dyd) (hiopKKTLinSys.cpp:1110-1190) incl. the residual-driven refinement of
  * solveWithRefin (:1192-1350: ||rhs - N x||_inf < 1e-8, <= 3 corrections). Condenses first if the cache is stale.
