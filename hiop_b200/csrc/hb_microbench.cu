@@ -1,5 +1,7 @@
 // In-run peak measurements for bench.py's roofline denominators:
-//   * FP64 tensor pipe: mma.sync.m8n8k4.f64 (SASS DMMA) issued back to back from registers by every warp of every SM,
+//   * FP64 tensor pipe: mma.sync.m8n8k4.f64 (SASS DMMA.8x8x4, which = 0) or mma.sync.m16n8k16.f64 (SASS DMMA.16x8x16, which = 2)
+//     issued back to back from registers by every warp of every SM. On sm_90a the two are different instructions, and
+//     16x8x16 is the one the condensation kernel k_syrk_ws runs; 0 stays the 8x8x4 rate that bench.py has always reported.
 //   * INT8 wgmma: wgmma.mma_async m64n256k32 s8 issued back to back by two warpgroups per SM on resident shared-memory operands
 //     (no loads in the loop): the integer tensor-core rate k_oz_gemm draws on.
 // Both are timed with CUDA events on the context stream over a few milliseconds, after a warm-up launch.
@@ -8,21 +10,49 @@
 
 namespace {
 
+// 8 independent accumulators per warp; SHAPE 0 = m8n8k4 (2 doubles each), 2 = m16n8k16 (4 doubles each)
+template <int SHAPE>
 __global__ void __launch_bounds__(256)
 k_peak_dmma(double* __restrict__ out, int iters, double a, double b)
 {
-  double c[8][2];
+  double c[8][4];
+  const double fa[8] = {a, b, a, b, a, b, a, b}, fb[4] = {a, b, a, b};
 #pragma unroll
-  for(int i = 0; i < 8; i++) { c[i][0] = threadIdx.x; c[i][1] = i; }
+  for(int i = 0; i < 8; i++) { c[i][0] = threadIdx.x; c[i][1] = i; c[i][2] = 1; c[i][3] = 2; }
   for(int it = 0; it < iters; it++) {
 #pragma unroll
-    for(int i = 0; i < 8; i++)
-      hb_dmma884(c[i][0], c[i][1], a, b);
+    for(int i = 0; i < 8; i++) {
+      if constexpr(SHAPE == 0) hb_dmma884(c[i][0], c[i][1], a, b);
+      else hb_dmma16816(c[i], fa, fb);
+    }
   }
   double s = 0;
 #pragma unroll
-  for(int i = 0; i < 8; i++) s += c[i][0] + c[i][1];
+  for(int i = 0; i < 8; i++) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+
+// best of 3 timed launches of k_peak_dmma<SHAPE> over 4 CTAs of 8 warps per SM, after a warm-up launch
+template <int SHAPE>
+int peak_dmma(hb_ctx* c, hb_event& e0, hb_event& e1, double* best)
+{
+  const int blocks = c->num_sms * 4, iters = 4000;
+  const double mma_flop = SHAPE == 0 ? 2.0 * 8 * 8 * 4 : 2.0 * 16 * 8 * 16;
+  HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)blocks * 256));
+  k_peak_dmma<SHAPE><<<blocks, 256, 0, c->stream>>>((double*)c->ws, 100, 1.0000001, 1e-9);
+  HB_LAUNCHED();
+  float ms = 0.f;
+  for(int rep = 0; rep < 3; rep++) {
+    HB_CUDA(cudaEventRecord(e0, c->stream));
+    k_peak_dmma<SHAPE><<<blocks, 256, 0, c->stream>>>((double*)c->ws, iters, 1.0000001, 1e-9);
+    HB_LAUNCHED();
+    HB_CUDA(cudaEventRecord(e1, c->stream));
+    HB_CUDA(cudaEventSynchronize(e1));
+    HB_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    const double tf = mma_flop * 8 * (double)iters * 8 * blocks / (ms * 1e-3) / 1e12; // 8 MMAs per warp per iteration, 8 warps
+    if(tf > *best) *best = tf;
+  }
+  return HB_OK;
 }
 
 // one CTA per SM, two warpgroups: 16 KB A tile (128 rows x 128 B, 64 rows per warpgroup) + 32 KB B tile (256 rows x 128 B) in the
@@ -65,10 +95,10 @@ int hb_microbench_init_attrs(hb_ctx* c)
   return HB_OK;
 }
 
-// which: 0 = FP64 DMMA (TFLOP/s), 1 = INT8 wgmma (TOP/s, 2 ops per MAC)
+// which: 0 = FP64 DMMA m8n8k4 (TFLOP/s), 1 = INT8 wgmma (TOP/s, 2 ops per MAC), 2 = FP64 DMMA m16n8k16 (TFLOP/s)
 extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
 {
-  HB_REQUIRE(c && result_host && (which == 0 || which == 1), "hb_microbench_peak: bad arguments");
+  HB_REQUIRE(c && result_host && (which == 0 || which == 1 || which == 2), "hb_microbench_peak: bad arguments");
   HB_CUDA(cudaSetDevice(c->device));
   hb_event e0, e1;
   HB_CHECK(e0.create(cudaEventDefault));
@@ -76,20 +106,9 @@ extern "C" int hb_microbench_peak(hb_ctx* c, int which, double* result_host)
   float ms = 0.f;
   double best = 0.0;
   if(which == 0) {
-    const int blocks = c->num_sms * 4, iters = 4000;
-    HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)blocks * 256));
-    k_peak_dmma<<<blocks, 256, 0, c->stream>>>((double*)c->ws, 100, 1.0000001, 1e-9);
-    HB_LAUNCHED();
-    for(int rep = 0; rep < 3; rep++) {
-      HB_CUDA(cudaEventRecord(e0, c->stream));
-      k_peak_dmma<<<blocks, 256, 0, c->stream>>>((double*)c->ws, iters, 1.0000001, 1e-9);
-      HB_LAUNCHED();
-      HB_CUDA(cudaEventRecord(e1, c->stream));
-      HB_CUDA(cudaEventSynchronize(e1));
-      HB_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-      const double tf = 2.0 * 8 * 256 * (double)iters * 8 * blocks / (ms * 1e-3) / 1e12; // 8 DMMAs of 8x8x4 per warp per iteration, 8 warps
-      if(tf > best) best = tf;
-    }
+    HB_CHECK(peak_dmma<0>(c, e0, e1, &best));
+  } else if(which == 2) {
+    HB_CHECK(peak_dmma<2>(c, e0, e1, &best));
   } else {
     const int blocks = c->num_sms, iters = 20000;
     const int smem = PEAK_I8_SMEM;

@@ -108,13 +108,15 @@ template <int N> __device__ __forceinline__ void hb_setmaxnreg_dec() { asm volat
 // named barrier ID over NTHREADS threads (a multiple of 32) of the CTA, ordering their memory accesses as __syncthreads does
 template <int ID, int NTHREADS> __device__ __forceinline__ void hb_bar_sync() { asm volatile("bar.sync %0, %1;\n" ::"n"(ID), "n"(NTHREADS) : "memory"); }
 
-// ---- FP64 MMA (SASS DMMA), registers only
+// ---- FP64 MMA (SASS DMMA), registers only. On sm_90a each shape is its own instruction (DMMA.8x8x4, DMMA.16x8x8, DMMA.16x8x16), and
+// 8x8x4 issues at half the rate of the other two.
 // c[0..1] += a * b: one m8n8k4 fragment per thread
 __device__ __forceinline__ void hb_dmma884(double& c0, double& c1, double a, double b)
 {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
-// the m16n8k8 and m16n8k16 shapes, fragments as in the PTX ISA: no kernel uses them, the FP64 microbenchmark times them
+// the m16n8k8 and m16n8k16 shapes, fragments as in the PTX ISA (k_syrk_ws runs m16n8k16). For m16n8k16 with g = lane / 4, t = lane % 4:
+// a[i] = A(g + 8 (i % 2), t + 4 (i / 2)), b[i] = B(t + 4 i, g), c = C(g, 2t), C(g, 2t + 1), C(g + 8, 2t), C(g + 8, 2t + 1)
 __device__ __forceinline__ void hb_dmma1688(double (&c)[4], const double (&a)[4], const double (&b)[2])
 {
   asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"

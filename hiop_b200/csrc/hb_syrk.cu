@@ -6,12 +6,13 @@
 // table of row pointers) is read ONCE per output tile pair and all of W = J D J^T, S1, Y1 and the three l x l
 // blocks of V come out of the same pass.
 //
-// Why DMMA and not the integer tensor path: wgmma has no f64 kind; mma.sync.m8n8k4.f64 (SASS DMMA) is the FP64
-// tensor path of sm_90a.
+// Why DMMA and not the integer tensor path: wgmma has no f64 kind; mma.sync.*.f64 (SASS DMMA) is the FP64 tensor path of sm_90a. The
+// fast kernel k_syrk_ws issues m16n8k16 (DMMA.16x8x16); m8n8k4 lowers to DMMA.8x8x4, which runs at half that rate on H100.
 //
-// Work decomposition: 128x128 output tiles (upper triangle of the tile grid only), K swept in BK=16 chunks through a
-// 4-stage cp.async pipeline into padded shared memory (row stride 20 doubles = 160 B -> the m8n8k4 fragment reads
-// of a half-warp, 4 rows x 32 B, fall into 4 distinct 32 B bank groups: conflict-free LDS.64).
+// Work decomposition: 128x128 output tiles (upper triangle of the tile grid only). k_syrk_ws sweeps K in 32-column chunks through a
+// 3-stage ring filled by producer warps (see below); the generic kernel k_syrk_diag, for rows that are not 16-byte aligned, sweeps
+// BK=16 chunks through a 4-stage cp.async pipeline (row stride 20 doubles = 160 B -> the m8n8k4 fragment reads of a half-warp,
+// 4 rows x 32 B, fall into 4 distinct 32 B bank groups: conflict-free LDS.64).
 // The (tile, K-range) space is cut into one (tile, K window) per CTA in K lanes, plus stream-K ranges for the CTAs left
 // over (see build_schedule): every SM gets the same number of MMA iterations whatever M is, and the tiles of a lane
 // read the same columns at the same time. Each CTA writes its partial 128x128 tile to a workspace
@@ -195,13 +196,16 @@ k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const 
 // The producers issue 16-byte cp.async copies (zero-filling rows beyond M and the K tail through the src-size operand)
 // and signal the stage's mbarrier with cp.async.mbarrier.arrive.noinc; the MMA warps never execute a CTA-wide barrier
 // and never compute a global address, so they drift out of phase and keep the FP64 tensor pipe busy during refills.
+// Each MMA warp owns a 64x32 block of the tile: 4 x 4 m16n8k16 accumulators, 64 doubles per thread. With one A and four B fragments
+// that does not fit the 168 registers of 384 threads, so the producer warpgroup gives its registers to the MMA warpgroups (setmaxnreg
+// 40 / 232). d scales the B fragment in registers: each product is rounded twice, as in k_syrk_diag.
 // (A first version staged rows with 256-byte cp.async.bulk copies from one producer warp: 288 bulk copies per stage
 // made the producer the bottleneck.)
 // Needs 16-byte aligned rows (else k_syrk_diag<false> runs).
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int WBK = 32;                 // doubles per K chunk
 constexpr int WSTAGES = 3;
-constexpr int WLDS = WBK + 4;           // 36 doubles = 288 B row stride (288 mod 128 = 32 -> conflict-free fragment reads)
+constexpr int WLDS = WBK + 4;           // 36 doubles = 288 B row stride (288 mod 128 = 32 -> conflict-free LDS.64 fragment reads)
 constexpr int WTILE_D = BM * WLDS;
 constexpr int WPROD = 128;              // producer threads (4 warps)
 constexpr int WTHREADS = 256 + WPROD;
@@ -241,6 +245,7 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
 
   if(warp >= 8) {
     // ================= producer warps =================
+    hb_setmaxnreg_dec<40>();
     const int p = tid - 256;          // 0..127
     const int kc = p & 15;            // 16-byte chunk within the 256-byte row segment
     const int r0 = p >> 4;            // rows r0 + 8*j
@@ -278,34 +283,43 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
     hb_cp_async_wait_all();
   } else {
     // ================= 8 MMA warps =================
+    hb_setmaxnreg_inc<232>(); // 64 accumulators + one A and four B fragments of m16n8k16 per thread
     const int warp_m = warp & 1, warp_n = warp >> 1;
     const int g = lane >> 2, t4 = lane & 3;
     const bool unit_d = (dvec == nullptr);
     for(int si = sb; si < se; si++) {
       const Seg sg = segs[si];
       const bool diag = sg.ti == sg.tj;
-      double acc[8][4][2];
+      double acc[4][4][4]; // [16-row block i][8-column block j]: rows g, g, g+8, g+8; columns 2*t4, 2*t4+1, 2*t4, 2*t4+1
 #pragma unroll
-      for(int i = 0; i < 8; i++)
+      for(int i = 0; i < 4; i++)
 #pragma unroll
-        for(int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
+        for(int j = 0; j < 4; j++)
+#pragma unroll
+          for(int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
       for(int it = 0; it < sg.k_count; it++) {
         hb_mbar_wait(&full[stage], phase);
         const WStage& st = stages[stage];
         const double* sA = st.a + (warp_m * 64 + g) * WLDS + t4;
         const double* sB = (diag ? st.a : st.b) + (warp_n * 32 + g) * WLDS + t4;
 #pragma unroll
-        for(int kk = 0; kk < WBK / 4; kk++) {
-          const double dv = unit_d ? 1.0 : st.d[kk * 4 + t4];
-          double af[8], bf[4];
+        for(int kk = 0; kk < WBK; kk += 16) {
+          // m16n8k16 fragments: B element q at (k = t4 + 4q, column g), A element q at (row g + 8*(q&1), k = t4 + 4*(q>>1))
+          double bf[4][4];
 #pragma unroll
-          for(int i = 0; i < 8; i++) af[i] = sA[i * 8 * WLDS + kk * 4];
+          for(int q = 0; q < 4; q++) {
+            const double dv = unit_d ? 1.0 : st.d[kk + 4 * q + t4];
 #pragma unroll
-          for(int j = 0; j < 4; j++) bf[j] = sB[j * 8 * WLDS + kk * 4] * dv;
+            for(int j = 0; j < 4; j++) bf[j][q] = sB[j * 8 * WLDS + kk + 4 * q] * dv;
+          }
 #pragma unroll
-          for(int i = 0; i < 8; i++)
+          for(int i = 0; i < 4; i++) {
+            double af[8];
 #pragma unroll
-            for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+            for(int q = 0; q < 8; q++) af[q] = sA[(i * 16 + 8 * (q & 1)) * WLDS + kk + 4 * (q >> 1)];
+#pragma unroll
+            for(int j = 0; j < 4; j++) hb_dmma16816(acc[i][j], af, bf[j]);
+          }
         }
         __syncwarp();
         if(lane == 0) hb_mbar_arrive(&empty[stage]);
@@ -313,12 +327,15 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
       }
       double* slot = ws + (size_t)sg.slot * (BM * BM);
 #pragma unroll
-      for(int i = 0; i < 8; i++) {
-        const int row = warp_m * 64 + i * 8 + g;
+      for(int i = 0; i < 4; i++) {
 #pragma unroll
-        for(int j = 0; j < 4; j++) {
-          const int col = warp_n * 32 + j * 8 + t4 * 2;
-          *reinterpret_cast<double2*>(slot + row * BM + col) = make_double2(acc[i][j][0], acc[i][j][1]);
+        for(int h = 0; h < 2; h++) {
+          const int row = warp_m * 64 + i * 16 + 8 * h + g;
+#pragma unroll
+          for(int j = 0; j < 4; j++) {
+            const int col = warp_n * 32 + j * 8 + t4 * 2;
+            *reinterpret_cast<double2*>(slot + row * BM + col) = make_double2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
+          }
         }
       }
     }

@@ -75,7 +75,8 @@ class Context:
         return {name: float(ms[i]) for i, name in enumerate(self.PHASES)}
 
     def microbench_peak(self, which: int) -> float:
-        """0: FP64 DMMA TFLOP/s, 1: int8 wgmma TOP/s -- measured on this device, now (hb_microbench_peak)"""
+        """0: FP64 DMMA m8n8k4 TFLOP/s, 1: int8 wgmma TOP/s, 2: FP64 DMMA m16n8k16 TFLOP/s (the shape k_syrk_ws runs) -- measured on
+        this device, now (hb_microbench_peak)"""
         v = ctypes.c_double()
         check(self.L.hb_microbench_peak(self.h, which, ctypes.byref(v)), "hb_microbench_peak")
         return v.value

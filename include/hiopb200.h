@@ -71,8 +71,9 @@ int hb_ctx_phase_timeline(hb_ctx* ctx, int on, float* ms_host10);
 int hb_ctx_last_syrk_ms(hb_ctx* ctx, float* ms_host);
 
 /* Measured roofline denominators of this device (a few milliseconds each, CUDA events on the context stream):
- * which = 0: FP64 tensor pipe, mma.sync.m8n8k4.f64 issued back to back from registers (TFLOP/s);
- * which = 1: wgmma.mma_async m64n256k32 s8 issued back to back by two warpgroups per SM on resident operands (TOP/s, 2 ops per MAC). */
+ * which = 0: FP64 tensor pipe, mma.sync.m8n8k4.f64 issued back to back from registers (TFLOP/s; SASS DMMA.8x8x4, half the rate of 2);
+ * which = 1: wgmma.mma_async m64n256k32 s8 issued back to back by two warpgroups per SM on resident operands (TOP/s, 2 ops per MAC);
+ * which = 2: FP64 tensor pipe, mma.sync.m16n8k16.f64 issued back to back from registers (TFLOP/s; SASS DMMA.16x8x16, what k_syrk_ws runs). */
 int hb_microbench_peak(hb_ctx* ctx, int which, double* result_host);
 
 int hb_malloc(hb_ctx* ctx, size_t bytes, void** dptr);

@@ -8,7 +8,8 @@
 // for both K schedules: "streamk" (one contiguous range of the tile-major (tile, k) space per CTA) and "lanes" (CTAs grouped in
 // K lanes so that all tiles of a lane read the same K window at the same time; the stream-K remainder as in hb_syrk.cu).
 // Reports TFLOP/s executed and bytes/s moved from L2 into shared memory, the SM clock derived from clock64() over the kernel's
-// duration, and the FP64 DMMA peak of the library (hb_microbench_peak(0)) measured in the same process.
+// duration, and the FP64 DMMA peaks of the library measured in the same process: m16n8k16 (hb_microbench_peak(2), the shape the
+// kernel runs, against which "% of peak" is given) and m8n8k4 (hb_microbench_peak(0)).
 // Build (after make -C hiop_b200/csrc):
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -Iinclude -Ihiop_b200/csrc -o tools/syrk_feed_probe tools/syrk_feed_probe.cu \
 //        -Lhiop_b200 -lhiopb200 -Xlinker -rpath,'$ORIGIN/../hiop_b200'
@@ -53,6 +54,7 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
   int stage = 0;
   unsigned phase = 0;
   if(warp >= 8) {
+    hb_setmaxnreg_dec<40>();
     if(MODE == MMA_ONLY) return;
     const int p = tid - 256, kc = p & 15, r0 = p >> 4;
     for(int si = sb; si < se; si++) {
@@ -88,15 +90,18 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
     }
     hb_cp_async_wait_all();
   } else {
+    hb_setmaxnreg_inc<232>();
     const int warp_m = warp & 1, warp_n = warp >> 1, g = lane >> 2, t4 = lane & 3;
     for(int si = sb; si < se; si++) {
       const Seg sg = segs[si];
       const bool diag = sg.ti == sg.tj;
-      double acc[8][4][2];
+      double acc[4][4][4];
 #pragma unroll
-      for(int i = 0; i < 8; i++)
+      for(int i = 0; i < 4; i++)
 #pragma unroll
-        for(int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
+        for(int j = 0; j < 4; j++)
+#pragma unroll
+          for(int e = 0; e < 4; e++) acc[i][j][e] = 0.0;
       for(int it = 0; it < sg.k_count; it++) {
         if(MODE != MMA_ONLY) hb_mbar_wait(&full[stage], phase);
         if(MODE != FEED_ONLY) {
@@ -104,17 +109,22 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
           const double* sA = st.a + (warp_m * 64 + g) * WLDS + t4;
           const double* sB = (diag ? st.a : st.b) + (warp_n * 32 + g) * WLDS + t4;
 #pragma unroll
-          for(int kk = 0; kk < WBK / 4; kk++) {
-            const double dv = st.d[kk * 4 + t4];
-            double af[8], bf[4];
+          for(int kk = 0; kk < WBK; kk += 16) {
+            double bf[4][4];
 #pragma unroll
-            for(int i = 0; i < 8; i++) af[i] = sA[i * 8 * WLDS + kk * 4];
+            for(int q = 0; q < 4; q++) {
+              const double dv = st.d[kk + 4 * q + t4];
 #pragma unroll
-            for(int j = 0; j < 4; j++) bf[j] = sB[j * 8 * WLDS + kk * 4] * dv;
+              for(int j = 0; j < 4; j++) bf[j][q] = sB[j * 8 * WLDS + kk + 4 * q] * dv;
+            }
 #pragma unroll
-            for(int i = 0; i < 8; i++)
+            for(int i = 0; i < 4; i++) {
+              double af[8];
 #pragma unroll
-              for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+              for(int q = 0; q < 8; q++) af[q] = sA[(i * 16 + 8 * (q & 1)) * WLDS + kk + 4 * (q >> 1)];
+#pragma unroll
+              for(int j = 0; j < 4; j++) hb_dmma16816(acc[i][j], af, bf[j]);
+            }
           }
         }
         if(MODE != MMA_ONLY) {
@@ -125,10 +135,13 @@ k_probe(const double* const* __restrict__ rowptr, int M, long long K, const doub
       }
       double* slot = ws + (size_t)sg.slot * (BM * BM);
 #pragma unroll
-      for(int i = 0; i < 8; i++)
+      for(int i = 0; i < 4; i++)
 #pragma unroll
-        for(int j = 0; j < 4; j++)
-          *reinterpret_cast<double2*>(slot + (warp_m * 64 + i * 8 + g) * BM + warp_n * 32 + j * 8 + t4 * 2) = make_double2(acc[i][j][0], acc[i][j][1]);
+        for(int h = 0; h < 2; h++)
+#pragma unroll
+          for(int j = 0; j < 4; j++)
+            *reinterpret_cast<double2*>(slot + (warp_m * 64 + i * 16 + 8 * h + g) * BM + warp_n * 32 + j * 8 + t4 * 2) =
+                make_double2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
     }
   }
   if(blockIdx.x == 0 && tid == 0) *cycles = clock64() - t0;
@@ -213,8 +226,12 @@ int main(int argc, char** argv)
   printf("device %s, %d SMs, M = %d, K = %lld\n", prop.name, G, M, K);
   hb_ctx* hc = nullptr;
   double peak = 0;
-  if(hb_ctx_create(0, &hc) != HB_OK || hb_microbench_peak(hc, 0, &peak) != HB_OK) { printf("hb_microbench_peak: %s\n", hb_last_error()); return 1; }
-  printf("FP64 DMMA peak (hb_microbench_peak(0)): %.1f TFLOP/s\n", peak);
+  double peak884 = 0;
+  if(hb_ctx_create(0, &hc) != HB_OK || hb_microbench_peak(hc, 0, &peak884) != HB_OK || hb_microbench_peak(hc, 2, &peak) != HB_OK) {
+    printf("hb_microbench_peak: %s\n", hb_last_error());
+    return 1;
+  }
+  printf("FP64 DMMA peaks: m16n8k16 (hb_microbench_peak(2)) %.1f TFLOP/s, m8n8k4 (hb_microbench_peak(0)) %.1f TFLOP/s\n", peak, peak884);
 
   double *J, *d;
   CK(cudaMalloc(&J, sizeof(double) * (size_t)M * K));
