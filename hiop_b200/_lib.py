@@ -160,6 +160,7 @@ def lib() -> ctypes.CDLL:
     f("hb_lowrank_Dd_inv", c_vp, c_vp)
     f("hb_lowrank_N", c_vp, c_vp)
     f("hb_lowrank_tdot", c_vp, c_vp)
+    f("hb_debug_lowrank_state", c_i, c_vp, *([c_vp] * 14))
     f("hb_lowrank_last_solve_stats", c_i, c_vp, P(c_i), P(c_d))
     f("hb_lowrank_kkt_system_host", c_i, c_vp, *([c_vp] * 16))
     # mds

@@ -41,6 +41,8 @@ __global__ void k_update_d(int mi, const double* __restrict__ vl, const double* 
 }
 
 // ---- a8: V from the blocks of C_aug = [J;S;Y] DhInv [J;S;Y]^T (updateInternalBFGSRepresentation, :400-485) ----------------
+// V, M and U are written with explicit roundings (no FMA contraction), so each entry is a fixed function of its inputs that
+// oracle/lowrank_model.py restates bit for bit.
 __global__ void k_build_V(int m, int l, double sigma, const double* __restrict__ C, int ldc, const double* __restrict__ SSt,
                           const double* __restrict__ L, const double* __restrict__ D, double* __restrict__ V)
 {
@@ -48,10 +50,10 @@ __global__ void k_build_V(int m, int l, double sigma, const double* __restrict__
   for(int e = blockIdx.x * blockDim.x + threadIdx.x; e < n2 * n2; e += gridDim.x * blockDim.x) {
     const int a = e / n2, b = e % n2;
     double v;
-    if(a < l && b < l) v = sigma * sigma * C[(size_t)(m + a) * ldc + m + b] - sigma * SSt[a * l + b];
-    else if(a < l && b >= l) v = sigma * C[(size_t)(m + a) * ldc + m + b] - L[a * l + (b - l)];
-    else if(a >= l && b < l) v = sigma * C[(size_t)(m + b) * ldc + m + a] - L[b * l + (a - l)];
-    else v = C[(size_t)(m + a) * ldc + m + b] + (a == b ? D[a - l] : 0.0);
+    if(a < l && b < l) v = __dsub_rn(__dmul_rn(__dmul_rn(sigma, sigma), C[(size_t)(m + a) * ldc + m + b]), __dmul_rn(sigma, SSt[a * l + b]));
+    else if(a < l && b >= l) v = __dsub_rn(__dmul_rn(sigma, C[(size_t)(m + a) * ldc + m + b]), L[a * l + (b - l)]);
+    else if(a >= l && b < l) v = __dsub_rn(__dmul_rn(sigma, C[(size_t)(m + b) * ldc + m + a]), L[b * l + (a - l)]);
+    else v = __dadd_rn(C[(size_t)(m + a) * ldc + m + b], a == b ? D[a - l] : 0.0);
     V[a * n2 + b] = v;
   }
 }
@@ -63,7 +65,7 @@ __global__ void k_build_Mdirect(int l, double sigma, const double* __restrict__ 
   for(int e = blockIdx.x * blockDim.x + threadIdx.x; e < n2 * n2; e += gridDim.x * blockDim.x) {
     const int a = e / n2, b = e % n2;
     double v;
-    if(a < l && b < l) v = sigma * SSt[a * l + b];
+    if(a < l && b < l) v = __dmul_rn(sigma, SSt[a * l + b]);
     else if(a < l && b >= l) v = L[a * l + (b - l)];
     else if(a >= l && b < l) v = L[b * l + (a - l)];
     else v = (a == b ? -D[a - l] : 0.0);
@@ -77,7 +79,7 @@ __global__ void k_build_U(int m, int l, double sigma, const double* __restrict__
   for(int e = blockIdx.x * blockDim.x + threadIdx.x; e < m * n2; e += gridDim.x * blockDim.x) {
     const int i = e / n2, q = e % n2;
     double v = C[(size_t)i * ldc + m + q];
-    if(q < l) v *= sigma;
+    if(q < l) v = __dmul_rn(sigma, v);
     U[e] = v;
     Z[e] = v;
   }
@@ -990,6 +992,7 @@ extern "C" int hb_lowrank_solve_compressed(hb_lowrank* k, double* rx, const doub
     fused = k->tdot_valid;
     k->tdot_valid = false; // tied to this rx
   }
+  k->rhs_fused = fused;
   if(fused) {
     hb_phase_mark(c, HB_PH_HSOLVE1);
     k_fused_rhs<<<(m + 127) / 128, 128, 0, c->stream>>>(m, k->meq, k->l, k->sigma, k->tdot, k->Z, ryc, ryd, k->rhs);
@@ -1103,6 +1106,50 @@ extern "C" const double* hb_lowrank_DhInv(hb_lowrank* k) { return k ? k->DhInv.g
 extern "C" const double* hb_lowrank_Dd_inv(hb_lowrank* k) { return k ? k->Dd_inv.get() : nullptr; }
 extern "C" const double* hb_lowrank_N(hb_lowrank* k) { return k ? k->Nmat.get() : nullptr; }
 extern "C" const double* hb_lowrank_tdot(hb_lowrank* k) { return k ? k->tdot.get() : nullptr; }
+
+extern "C" int hb_debug_lowrank_state(hb_lowrank* k, double* Caug, double* SSt, double* V_built, double* V_factor, int* ipivV, double* U, double* Z,
+                                      double* M_built, double* M_factor, int* ipivM, double* p2l, double* rhs, double* tdot, int* info4)
+{
+  HB_REQUIRE(k, "null handle");
+  hb_ctx* c = k->ctx;
+  const int m = k->m, l = k->l, n2 = 2 * l, Ma = m + n2;
+  auto get = [&](void* dst, const void* src, size_t bytes) -> int {
+    if(dst && bytes) HB_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream));
+    return HB_OK;
+  };
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  if((V_built || M_built) && l > 0) {
+    // rebuilt from the handle's current inputs into scratch: the production path keeps no unfactored copy
+    HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)n2 * n2));
+    double* W = (double*)c->ws;
+    if(V_built) {
+      k_build_V<<<(4 * l * l + 127) / 128, 128, 0, c->stream>>>(m, l, k->sigma, k->Caug, Ma, k->SSt, k->Ld, k->Dd_sec, W);
+      HB_LAUNCHED();
+      HB_CHECK(get(V_built, W, sizeof(double) * n2 * n2));
+      HB_CUDA(cudaStreamSynchronize(c->stream));
+    }
+    if(M_built) {
+      k_build_Mdirect<<<(4 * l * l + 127) / 128, 128, 0, c->stream>>>(l, k->sigma, k->SSt, k->Ld, k->Dd_sec, W);
+      HB_LAUNCHED();
+      HB_CHECK(get(M_built, W, sizeof(double) * n2 * n2));
+    }
+  }
+  HB_CHECK(get(Caug, k->Caug, sizeof(double) * Ma * Ma));
+  HB_CHECK(get(SSt, k->SSt, sizeof(double) * l * l));
+  HB_CHECK(get(V_factor, k->V, sizeof(double) * n2 * n2));
+  HB_CHECK(get(ipivV, k->ipivV, sizeof(int) * n2));
+  HB_CHECK(get(U, k->U, sizeof(double) * m * n2));
+  HB_CHECK(get(Z, k->Z, sizeof(double) * m * n2));
+  HB_CHECK(get(M_factor, k->Mdir, sizeof(double) * n2 * n2));
+  HB_CHECK(get(ipivM, k->ipivM, sizeof(int) * n2));
+  HB_CHECK(get(p2l, k->p2l, sizeof(double) * n2));
+  HB_CHECK(get(rhs, k->rhs, sizeof(double) * m));
+  HB_CHECK(get(tdot, k->tdot, sizeof(double) * Ma));
+  HB_CHECK(get(info4, k->info, sizeof(int) * 3));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  if(info4) info4[3] = k->rhs_fused ? 1 : 0;
+  return HB_OK;
+}
 
 // ---- one whole KKT system from host buffers ----------------------------------------------------------------------------
 extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, const double* Jd_host, const double* zl, const double* sxl,

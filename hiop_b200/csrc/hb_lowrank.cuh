@@ -66,6 +66,7 @@ struct hb_lowrank
   hb_dev<double> tri;  // packed upper triangle of C_aug for the all-reduce
   hb_dev<double> tdot; // [J; S; Y] (DhInv .* rx) from the fused row-maximum sweep of an int8-slice condensation (m + 2 lmax)
   bool tdot_valid = false;
+  bool rhs_fused = false; // the last solve_compressed formed rhs from tdot (k_fused_rhs)
   // host staging (hb_lowrank_kkt_system_host)
   hb_dev<double> hbuf[14];
   hb_pinned<int> info_host;     // 4 ints

@@ -428,6 +428,22 @@ class KKTLinSysLowRank:
         condensation pending and fused the row dots into it"""
         return self._readback("hb_lowrank_tdot", self.m_eq + self.m_ineq + 2 * l)
 
+    def debug_state(self, l: int) -> dict:
+        """The compact-BFGS state of the last condensation / solve (hb_debug_lowrank_state), l the current memory length: C_aug, SSt,
+        V / M as built (rebuilt from the current inputs) and as factored (column-major lower, LAPACK's layout) with their pivots, U, Z,
+        p2l, the condensed rhs and tdot of the last solveCompressed, and info = (V, N, M, rhs formed from tdot)."""
+        m, n2 = self.m_eq + self.m_ineq, 2 * l
+        Ma = m + n2
+        out = dict(Caug=np.zeros((Ma, Ma)), SSt=np.zeros((l, l)), V_built=np.zeros((n2, n2)), V_factor=np.zeros((n2, n2)),
+                   ipivV=np.zeros(n2, dtype=np.int32), U=np.zeros((m, n2)), Z=np.zeros((m, n2)), M_built=np.zeros((n2, n2)),
+                   M_factor=np.zeros((n2, n2)), ipivM=np.zeros(n2, dtype=np.int32), p2l=np.zeros(n2), rhs=np.zeros(m), tdot=np.zeros(Ma),
+                   info=np.zeros(4, dtype=np.int32))
+        order = ("Caug", "SSt", "V_built", "V_factor", "ipivV", "U", "Z", "M_built", "M_factor", "ipivM", "p2l", "rhs", "tdot", "info")
+        check(self.ctx.L.hb_debug_lowrank_state(self.h, *[out[kk].ctypes.data_as(ctypes.c_void_p) for kk in order]), "hb_debug_lowrank_state")
+        for kk in ("V_factor", "M_factor"):          # column-major lower: the row-major read is its transpose
+            out[kk] = np.ascontiguousarray(out[kk].T)
+        return out
+
     def last_solve_stats(self):
         a, b = ctypes.c_int(), ctypes.c_double()
         check(self.ctx.L.hb_lowrank_last_solve_stats(self.h, ctypes.byref(a), ctypes.byref(b)), "hb_lowrank_last_solve_stats")

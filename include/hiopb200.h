@@ -364,6 +364,15 @@ const double* hb_lowrank_DhInv(hb_lowrank* k);
 const double* hb_lowrank_Dd_inv(hb_lowrank* k);
 const double* hb_lowrank_N(hb_lowrank* k);
 const double* hb_lowrank_tdot(hb_lowrank* k);
+/* diagnostics (tests): the compact-BFGS state of the last condensation / solve, read back (synchronises the stream; every output may
+ * be NULL). Row-major unless noted, l the current memory length, m = m_eq + m_ineq, Ma = m + 2l.
+ * Caug: Ma x Ma. SSt: l x l. V_built / M_built: the 2l x 2l V and M rebuilt now from the current C_aug, S S^T, L, D and sigma.
+ * V_factor / M_factor: their Bunch-Kaufman factors as left by the condensation / the last hess_times_vec, column-major lower
+ * (LAPACK's dsytrf layout), ipivV / ipivM: 2l pivots. U, Z: m x 2l (Z = U V^-1). p2l: the 2l-vector of the last low-rank solve.
+ * rhs: the m condensed right-hand side of the last solve_compressed; tdot: its Ma fused row dots.
+ * info4: the info words of V, N and M, then 1 if that rhs was formed from the fused row dots. */
+int hb_debug_lowrank_state(hb_lowrank* k, double* Caug, double* SSt, double* V_built, double* V_factor, int* ipivV, double* U, double* Z,
+                           double* M_built, double* M_factor, int* ipivM, double* p2l, double* rhs, double* tdot, int* info4);
 /* statistics of the last solve: refinement steps taken, last residual inf-norm (host) */
 int hb_lowrank_last_solve_stats(hb_lowrank* k, int* n_refine, double* resid_inf);
 /* One whole KKT system from HOST buffers (the e2e path of bench.py and of the C++ adapter when HiOp keeps its data in

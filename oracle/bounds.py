@@ -277,7 +277,7 @@ def factor_backward_ratio(PAP, L, d, dsub=None, theta=1.0):
 EXACT_RESIDUAL_MAX_N = 320    # above: the residual in FP64 with its evaluation bound (exact_rows takes ~1 s per rhs at N = 4000)
 
 
-def solve_backward_ratio(A, x, b, L, d, dsub=None, theta=1.0):
+def solve_backward_ratio(A, x, b, L, d, dsub=None, theta=1.0, extra=0.0):
     """Backward error of a solve A x = b through the factor P A P^T = L D L^T (one rhs per column of x, b), against its bound:
     returns (ratio, omega). omega is the Oettli-Prager backward error max_i |b - A x|_i / (|A||x| + |b|)_i (Higham Thm 7.3); ratio is
     max_i |b - A x|_i / tol_i with
@@ -288,7 +288,8 @@ def solve_backward_ratio(A, x, b, L, d, dsub=None, theta=1.0):
     factor_backward_ratio (theta gamma(3N + 3)) plus one triangular solve per factor of L (gamma(N) each, Thm 8.5), each doubled by the
     explicit diagonal-block inverses of the blocked solves (theta gamma(2N) each): theta gamma(7N + 3). A, L: full arrays in the permuted
     order given by perm on the caller's side; pass A = P A P^T, x, b permuted alike. eval = 0 when the residual is evaluated exactly
-    (numpy arrays, N <= EXACT_RESIDUAL_MAX_N), else gamma(N + 1)(|A||x| + |b|) for the FP64 evaluation."""
+    (numpy arrays, N <= EXACT_RESIDUAL_MAX_N), else gamma(N + 1)(|A||x| + |b|) for the FP64 evaluation. extra (>= 0, broadcast to b):
+    a bound on how far the right-hand side the kernel solved with is from b, added to tol (a b formed by a reduction)."""
     xp = _xp(A)
     N = A.shape[0]
     x = x.reshape(N, -1)
@@ -304,7 +305,7 @@ def solve_backward_ratio(A, x, b, L, d, dsub=None, theta=1.0):
     op = aA @ ax + xp.abs(b)
     aL = xp.abs(L)
     ldl = ld_product(aL, xp.abs(d), None if dsub is None else xp.abs(dsub)) @ (aL.T @ ax)
-    tol = theta * gamma(SOLVE_C * N + 3) * (op + ldl) + ev * gamma(N + 1) * op
+    tol = theta * gamma(SOLVE_C * N + 3) * (op + ldl) + ev * gamma(N + 1) * op + extra
     tiny = np.finfo(np.float64).tiny
     ratio = float((xp.abs(r) / xp.clip(tol, tiny, None)).max())
     omega = float((xp.abs(r) / xp.clip(op, tiny, None)).max())
