@@ -1,6 +1,7 @@
 // Shared internals of libhiopb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <cudaTypedefs.h>
 #include <atomic>
 #include <cmath>
 #include <cstdint>
@@ -123,13 +124,10 @@ private:
 using hb_stream = hb_handle<cudaStream_t>;
 using hb_event = hb_handle<cudaEvent_t>;
 
-// per-context state defined in one kernel file each: the int8-slice condensation (hb_ozaki.cu), the Chinese-remainder int8
-// condensation (hb_crt.cu), the SYRK schedule cache (hb_syrk.cu)
-struct OzState;
-struct CrtState;
+// per-context state: of each int8 condensation (hb_int8_state, below; released in hb_ozaki.cu), the SYRK schedule cache (hb_syrk.cu)
+struct hb_int8_state;
 struct ScheduleCache;
-void hb_delete(OzState* p);
-void hb_delete(CrtState* p);
+void hb_delete(hb_int8_state* p);
 void hb_delete(ScheduleCache* p);
 struct hb_deleter
 {
@@ -158,10 +156,9 @@ struct hb_ctx
   bool phases = false;
   hb_event ev_phase[HB_PH_COUNT];
   unsigned phase_mask = 0;
-  // per-context state of the int8-slice condensation (hb_ozaki.cu): slice buffer, exponents, tensor maps, work list
-  hb_state<OzState> oz;
-  // per-context state of the Chinese-remainder condensation (hb_crt.cu): residue planes, exponents, tensor maps, work list
-  hb_state<CrtState> crt;
+  // per-context state of the int8-slice condensation (hb_ozaki.cu: the slice buffer) and of the Chinese-remainder condensation
+  // (hb_crt.cu: the residue planes), side by side
+  hb_state<hb_int8_state> oz, crt;
   // schedule cache of the FP64 condensation (hb_syrk.cu)
   hb_state<ScheduleCache> syrk_sched;
   // dense symmetric solvers: size thresholds (with their environment overrides, set by hb_dense_init in hb_symdense.cu) and the
@@ -214,18 +211,32 @@ int hb_reduce_slots(hb_ctx* c, int nblocks, const double* partial, double* out, 
 // out = [a (na doubles); b (nb doubles)]
 int hb_stack(hb_ctx* c, int na, const double* a, int nb, const double* b, double* out);
 
-// C = A diag(d) A^T over the rows of a device row-pointer table: FP64 DMMA (hb_syrk.cu) and int8 slices (hb_ozaki.cu)
+// C = A diag(d) A^T over the rows of a device row-pointer table: FP64 DMMA (hb_syrk.cu), int8 slices (hb_ozaki.cu), int8 Chinese
+// remaindering (hb_crt.cu). Optional dot_out[i] = sum_k row_i[k] d[k] dot_x[k] from the int8 row-maximum pass (none when K == 0).
 int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
                  const double* fuse_rx = nullptr, double* tdot = nullptr);
 bool hb_syrk_extra_row_is_free(int M);
 int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
                        const double* dot_x, double* dot_out);
-// the same contract on the int8 tensor cores by Chinese remaindering (hb_crt.cu): the correctly rounded value of an exact integer Gram
+// the correctly rounded value of an exact integer Gram
 int hb_syrk_rows_crt(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc,
                      const double* dot_x, double* dot_out);
 
-// Step 1 of both int8 condensations (hb_ozaki.cu): sd = sqrt(d) (when d is given), the exact row maxima of |a_ik| sd_k and their
-// frexp exponents e_i, and optionally dot_out[i] = sum_k a_ik d_k dot_x_k from the same sweep. Marks HB_PH_OZ_ROWMAX.
+// Runs launch(), which launches the GEMM kernel of a condensation, between the two events hb_ctx_last_syrk_ms reads when timing is on
+template <typename F>
+int hb_timed_syrk(hb_ctx* c, F&& launch)
+{
+  if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
+  HB_CHECK(launch());
+  if(c->timing) {
+    HB_CUDA(cudaEventRecord(c->ev_syrk1, c->stream));
+    c->syrk_timed = true;
+  }
+  return HB_OK;
+}
+
+// The host driver of both int8 condensations (hb_ozaki.cu). Step 1: sd = sqrt(d) (when d is given), the exact row maxima of |a_ik| sd_k and their frexp exponents e_i, and optionally
+// dot_out[i] = sum_k a_ik d_k dot_x_k from the same sweep. Marks HB_PH_OZ_ROWMAX.
 struct hb_rowscale
 {
   hb_dev<double> sd;
@@ -235,6 +246,45 @@ struct hb_rowscale
 };
 int hb_row_exponents(hb_ctx* c, hb_rowscale& rs, int M, int Mpad, long long K, const double* const* rowptr_dev, bool rows_aligned16,
                      const double* d, const double* dot_x, double* dot_out, const double** sd_out);
+
+// How a scheme lays out its work. Rows are padded to tm, K to 128-byte stages; plane p of the int8 buffer holds row r at
+// Q + (p Mpad + r) Kpad. The tiles (bi, bj) with bj >= (tm / tn) bi and bj tn < M cover the upper triangle. Work items are listed
+// split-major, then by group, then by tile; the item of tile t, group g and split s owns workspace tile (t groups + g) splits + s.
+struct hb_int8_layout
+{
+  int planes;         // int8 planes of every row: S slices, or N(K) moduli
+  int tm, tn;         // output tile
+  int groups;         // work items per tile and K range: 1 (each item runs all planes) or one per plane
+  size_t tile_bytes;  // workspace of one item
+  size_t item_bytes;  // the work item the GEMM kernel reads, written by put_item
+  void (*put_item)(void* dst, int bi, int bj, int group, int k_begin, int k_count, int slot);
+  // K splits for `units` items per split, max_splits read from the environment variable split_env (default 16) on every call
+  int (*splits)(const hb_ctx* c, long long units, long long kstages, int max_splits, size_t tile_bytes);
+  const char* split_env;
+  int n_maps;
+  cuuint32_t box[2][3]; // TMA box of each tensor map over (k bytes, row, plane)
+};
+// per-context state of one scheme: its planes, row scales, work list, tile list and tensor maps
+struct hb_int8_state
+{
+  int M = -1, planes = 0, max_splits = 0; // (M, K, planes, max_splits): what the work list and tensor maps were built for
+  long long K = -1, Kpad = 0;
+  int Mpad = 0, splits = 0, n_tiles = 0, n_items = 0;
+  hb_dev<int8_t> Q;
+  hb_rowscale rs;
+  hb_dev<unsigned char> items;
+  hb_dev<int2> tiles;
+  CUtensorMap maps[2];
+  PFN_cuTensorMapEncodeTiled encode = nullptr; // resolved on first use
+};
+// Clears C for K == 0; nothing to do for M == 0
+int hb_int8_empty(hb_ctx* c, int M, double* C, int ldc);
+// The state of `slot` ready for M rows of K columns (M, K > 0): plane buffer, work list and tensor maps (rebuilt when the key changed),
+// and a context workspace of one tile per item
+int hb_int8_prepare(hb_ctx* c, hb_state<hb_int8_state>& slot, const hb_int8_layout& L, int M, long long K, hb_int8_state** st);
+// The K-split search of both schemes: of at most max_splits splits (>= 64 stages and <= 1 GB of workspace, not asked of one split), the
+// count with the shortest makespan ceil(units splits / SMs) / splits that beats `best`, the cost of `splits`, by 0.1 %; ties go lower
+int hb_split_search(const hb_ctx* c, long long units, long long kstages, int max_splits, size_t tile_bytes, int splits, double best);
 
 // set once by hb_ctx_create: the dynamic-shared-memory / cluster attributes of each kernel file's kernels (function attributes are
 // per device) and the dense solvers' thresholds

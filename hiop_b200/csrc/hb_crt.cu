@@ -27,7 +27,6 @@
 #include "hb_common.cuh"
 #include "hb_ptx.cuh"
 #include <cuda.h>
-#include <cstdlib>
 
 namespace {
 
@@ -320,9 +319,6 @@ k_crt_fixup(int M, const int2* __restrict__ tile_ij, int splits, const int* __re
   }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // t(K) = min(53, floor((126 - ceil(log2 K)) / 2)): K 2^(2t) <= 2^126
 int crt_bits(long long K)
 {
@@ -344,21 +340,20 @@ int crt_moduli(long long K, int t)
   return n;
 }
 
-} // namespace
-
-struct CrtState
+void put_item(void* dst, int bi, int bj, int plane, int k_begin, int k_count, int slot)
 {
-  int M = -1, nmod = 0, t = 0, splits = 0, n_tiles = 0, n_items = 0, max_splits = 0; // (M, K, max_splits): what the work list was built for
-  long long K = -1, Kpad = 0;
-  int Mpad = 0;
-  hb_dev<int8_t> R; // residue planes
-  hb_rowscale rs;
-  hb_dev<CrtItem> d_items;
-  hb_dev<int2> d_tiles;
-  CUtensorMap map;
-  PFN_encodeTiled encode = nullptr;
-};
-void hb_delete(CrtState* p) { delete p; }
+  const CrtItem it = {bi, bj, plane, k_begin, k_count, slot};
+  memcpy(dst, &it, sizeof(it));
+}
+
+// K splits: the count of at most 16 (HB_CRT_MAX_SPLITS) with the shortest makespan, searched from one split (hb_split_search). The
+// bits do not depend on it.
+int crt_splits(const hb_ctx* c, long long pairs, long long kstages, int max_splits, size_t tile_bytes)
+{
+  return hb_split_search(c, pairs, kstages, max_splits, tile_bytes, 1, (double)((pairs + c->num_sms - 1) / c->num_sms));
+}
+
+} // namespace
 
 int hb_crt_init_attrs(hb_ctx* c)
 {
@@ -368,101 +363,43 @@ int hb_crt_init_attrs(hb_ctx* c)
 }
 
 // Same contract as hb_syrk_rows (C = A diag(d) A^T, both triangles), as the correctly rounded value of the exact integer Gram of the
-// rows rounded to t(K) bits. dot_x/dot_out as in hb_syrk_rows_ozaki.
+// rows rounded to t(K) bits
 int hb_syrk_rows_crt(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc,
                      const double* dot_x, double* dot_out)
 {
   HB_REQUIRE(c && M >= 0 && K >= 0 && K < (1LL << 31) && ldc >= M, "hb_syrk_rows_crt: bad arguments");
-  if(M == 0) return HB_OK;
-  if(K == 0) {
-    HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
-    return HB_OK;
-  }
-  if(!c->crt) c->crt.reset(new CrtState);
-  CrtState& st = *c->crt;
-  if(!st.encode) {
-    cudaDriverEntryPointQueryResult qres;
-    HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&st.encode, cudaEnableDefault, &qres));
-    if(!st.encode) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver%s", "");
-  }
-  const int Mpad = ((M + CT - 1) / CT) * CT;
-  const long long Kpad = ((K + KS - 1) / KS) * KS;
+  if(M == 0 || K == 0) return hb_int8_empty(c, M, C, ldc);
   const int t = crt_bits(K), nmod = crt_moduli(K, t);
   HB_REQUIRE(nmod >= 14 && nmod <= CRT_MAX, "hb_syrk_rows_crt: the reconstruction covers 14 to 17 moduli");
-  const size_t rbytes = (size_t)nmod * Mpad * Kpad;
-  if(!st.R || st.R.capacity() < rbytes) {
-    st.M = -1; // the tensor map holds the address of R
-    HB_CHECK(st.R.reserve(c, rbytes, "the int8 residue planes"));
-  }
-  const int max_splits = getenv("HB_CRT_MAX_SPLITS") ? atoi(getenv("HB_CRT_MAX_SPLITS")) : 16;
-  if(st.M != M || st.K != K || st.max_splits != max_splits) {
-    st.M = -1;
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    const int nb = Mpad / CT;
-    std::vector<int2> tiles;
-    for(int bi = 0; bi < nb; bi++)
-      for(int bj = bi; bj < nb; bj++) tiles.push_back(make_int2(bi, bj));
-    const int nt = (int)tiles.size();
-    const long long kstages = Kpad / KS, pairs = (long long)nt * nmod;
-    // K splits: the count of at most 16 (HB_CRT_MAX_SPLITS; >= 64 stages each, residue workspace <= 1 GB) with the shortest makespan
-    // ceil(pairs * splits / SMs) / splits; ties go to the smaller count. The bits do not depend on it.
-    int splits = 1;
-    double best = (double)((pairs + c->num_sms - 1) / c->num_sms);
-    for(int sp = 2; sp <= max_splits; sp++) {
-      if(kstages / sp < 64 || (size_t)pairs * sp * CT * CT * sizeof(int) > ((size_t)1 << 30)) break;
-      const double cost = (double)((pairs * sp + c->num_sms - 1) / c->num_sms) / sp;
-      if(cost < best * (1.0 - 1e-3)) { best = cost; splits = sp; }
-    }
-    // split-major, then modulus: the CTAs running at once sweep the same K window of the same residue plane (operand reuse in L2)
-    std::vector<CrtItem> items;
-    for(int s = 0; s < splits; s++)
-      for(int m = 0; m < nmod; m++)
-        for(int tt = 0; tt < nt; tt++) {
-          CrtItem it;
-          it.bi = tiles[tt].x; it.bj = tiles[tt].y; it.plane = m;
-          const long long b = hb_part_begin(kstages, splits, s), e2 = hb_part_begin(kstages, splits, s + 1);
-          it.k_begin = (int)b; it.k_count = (int)(e2 - b);
-          it.slot = (tt * nmod + m) * splits + s;
-          items.push_back(it);
-        }
-    HB_CHECK(st.d_items.reserve(c, items.size(), "the CRT work list"));
-    HB_CHECK(st.d_tiles.reserve(c, nt, "the CRT tile list"));
-    HB_CUDA(cudaMemcpy(st.d_items, items.data(), sizeof(CrtItem) * items.size(), cudaMemcpyHostToDevice));
-    HB_CUDA(cudaMemcpy(st.d_tiles, tiles.data(), sizeof(int2) * nt, cudaMemcpyHostToDevice));
-    cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Mpad, (cuuint64_t)nmod};
-    cuuint64_t strides[2] = {(cuuint64_t)Kpad, (cuuint64_t)Kpad * Mpad};
-    cuuint32_t box[3] = {KS, CT, 1}, es[3] = {1, 1, 1};
-    if(st.encode(&st.map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.R, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled failed%s", "");
-    st.M = M; st.K = K; st.Mpad = Mpad; st.Kpad = Kpad; st.t = t; st.nmod = nmod; st.splits = splits; st.n_tiles = nt;
-    st.n_items = (int)items.size(); st.max_splits = max_splits;
-  }
+  // 128 x 128 tiles, one item per (tile, modulus, K range): per K stage one box of each operand from the same map
+  const hb_int8_layout L = {nmod, CT, CT, nmod, sizeof(int) * CT * CT, sizeof(CrtItem), put_item, crt_splits, "HB_CRT_MAX_SPLITS",
+                            1, {{KS, CT, 1}}};
+  hb_int8_state* st;
+  HB_CHECK(hb_int8_prepare(c, c->crt, L, M, K, &st));
+  const int Mpad = st->Mpad;
+  const long long Kpad = st->Kpad;
   // 1. sqrt(d), row maxima, exponents (shared with the slice path), residues
   const double* sd;
-  HB_CHECK(hb_row_exponents(c, st.rs, M, Mpad, K, rowptr_dev, rows_aligned16, d, dot_x, dot_out, &sd));
-  k_crt_residues<<<dim3((unsigned)((Kpad / 8 + 255) / 256), Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, t, nmod, st.R,
+  HB_CHECK(hb_row_exponents(c, st->rs, M, Mpad, K, rowptr_dev, rows_aligned16, d, dot_x, dot_out, &sd));
+  k_crt_residues<<<dim3((unsigned)((Kpad / 8 + 255) / 256), Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st->rs.e, t, nmod, st->Q,
                                                                                        rows_aligned16 ? 1 : 0);
   HB_LAUNCHED();
   hb_phase_mark(c, HB_PH_OZ_SLICE);
   // 2. one exact int8 GEMM per modulus into int32 residue tiles
-  HB_CHECK(hb_ws_reserve(c, sizeof(int) * (size_t)st.n_items * CT * CT));
-  if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
-  const int G = st.n_items < c->num_sms ? st.n_items : c->num_sms;
-  k_crt_gemm<<<G, CRT_THREADS, CRT_SMEM, c->stream>>>(st.map, st.d_items, st.n_items, (int*)c->ws.get());
-  HB_LAUNCHED();
-  if(c->timing) {
-    HB_CUDA(cudaEventRecord(c->ev_syrk1, c->stream));
-    c->syrk_timed = true;
-  }
+  int* ws = (int*)c->ws.get();
+  HB_CHECK(hb_timed_syrk(c, [&] {
+    const int G = st->n_items < c->num_sms ? st->n_items : c->num_sms;
+    k_crt_gemm<<<G, CRT_THREADS, CRT_SMEM, c->stream>>>(st->maps[0], (const CrtItem*)st->items.get(), st->n_items, ws);
+    HB_LAUNCHED();
+    return HB_OK;
+  }));
   // 3. split residues, reconstruction, rounding, row scales, symmetrisation
-  const int* ws = (const int*)c->ws.get();
-  const dim3 fg(st.n_tiles, CRT_FIXUP_PARTS);
+  const dim3 fg(st->n_tiles, CRT_FIXUP_PARTS);
   switch(nmod) {
-  case 14: k_crt_fixup<14><<<fg, 256, 0, c->stream>>>(M, st.d_tiles, st.splits, ws, st.rs.e, t, C, ldc); break; // K <= 8
-  case 15: k_crt_fixup<15><<<fg, 256, 0, c->stream>>>(M, st.d_tiles, st.splits, ws, st.rs.e, t, C, ldc); break;
-  case 16: k_crt_fixup<16><<<fg, 256, 0, c->stream>>>(M, st.d_tiles, st.splits, ws, st.rs.e, t, C, ldc); break;
-  case 17: k_crt_fixup<17><<<fg, 256, 0, c->stream>>>(M, st.d_tiles, st.splits, ws, st.rs.e, t, C, ldc); break;
+  case 14: k_crt_fixup<14><<<fg, 256, 0, c->stream>>>(M, st->tiles, st->splits, ws, st->rs.e, t, C, ldc); break; // K <= 8
+  case 15: k_crt_fixup<15><<<fg, 256, 0, c->stream>>>(M, st->tiles, st->splits, ws, st->rs.e, t, C, ldc); break;
+  case 16: k_crt_fixup<16><<<fg, 256, 0, c->stream>>>(M, st->tiles, st->splits, ws, st->rs.e, t, C, ldc); break;
+  case 17: k_crt_fixup<17><<<fg, 256, 0, c->stream>>>(M, st->tiles, st->splits, ws, st->rs.e, t, C, ldc); break;
   }
   HB_LAUNCHED();
   return HB_OK;

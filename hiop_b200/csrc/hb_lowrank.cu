@@ -537,6 +537,31 @@ int jac_table(hb_lowrank* k, const hb_rowtab** out)
   return HB_OK;
 }
 
+// ---- the condensation modes: HB_CONDENSE_AUTO (-1), HB_CONDENSE_FP64_DMMA (0), int8 slices (6, 7, 8), HB_CONDENSE_INT8_CRT ----
+// AUTO runs the FP64 kernel: on H100 it is faster than either int8 mode at the sizes measured (DESIGN.md section 3). The int8 modes
+// need the row maxima of the whole J before their first GEMM, so they need J whole on the device.
+bool mode_valid(int mode) { return mode == HB_CONDENSE_AUTO || mode == HB_CONDENSE_FP64_DMMA || (mode >= 6 && mode <= 8) || mode == HB_CONDENSE_INT8_CRT; }
+int mode_resolved(int mode) { return mode == HB_CONDENSE_AUTO ? HB_CONDENSE_FP64_DMMA : mode; }
+bool mode_needs_whole_J(int mode) { return mode_resolved(mode) != HB_CONDENSE_FP64_DMMA; }
+// HB_CONDENSE = oz6 | oz7 | oz8 | crt | dmma (anything starting with 'd'): the mode of a new handle; other values leave `mode`
+int mode_from_env(int mode)
+{
+  if(const char* e = getenv("HB_CONDENSE")) {
+    if(e[0] == 'o' && e[1] == 'z' && e[2] >= '6' && e[2] <= '8') return e[2] - '0';
+    if(strcmp(e, "crt") == 0) return HB_CONDENSE_INT8_CRT;
+    if(e[0] == 'd') return HB_CONDENSE_FP64_DMMA;
+  }
+  return mode;
+}
+// jac_whole for an int8 mode, the refusal naming the entry point `who` and the mode
+int mode_whole_J(hb_lowrank* k, const char* who, int mode, const hb_rowtab** rows)
+{
+  char what[256];
+  snprintf(what, sizeof(what), "%s: the %s (AUTO and 0 condense in FP64)", who,
+           mode == HB_CONDENSE_INT8_CRT ? "int8 Chinese-remainder condensation of mode 100" : "int8-slice condensation of modes 6-8");
+  return jac_whole(k, what, nullptr, rows);
+}
+
 } // namespace
 
 bool jac_set(const hb_lowrank* k) { return k->m == 0 || k->jl.base; }
@@ -602,6 +627,27 @@ int jac_syrk(hb_lowrank* k, int M, const double* d, double* C, const double* fus
   });
 }
 
+int jac_gram(hb_lowrank* k, const char* who, int M, const double* d, double* C, const double* fuse_rx, double* tdot, bool* fused)
+{
+  const int mode = mode_resolved(k->condense_mode);
+  const bool fuse = fuse_rx && k->m > 0 &&
+                    (mode != HB_CONDENSE_FP64_DMMA || (hb_syrk_extra_row_is_free(M) && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0));
+  if(!fuse) {
+    fuse_rx = nullptr;
+    tdot = nullptr;
+  }
+  if(mode == HB_CONDENSE_FP64_DMMA) HB_CHECK(jac_syrk(k, M, d, C, fuse_rx, tdot));
+  else {
+    const hb_rowtab* rows;
+    HB_CHECK(mode_whole_J(k, who, mode, &rows));
+    if(tdot && k->n == 0) HB_CUDA(cudaMemsetAsync(tdot, 0, sizeof(double) * M, k->ctx->stream)); // no row-maximum pass then
+    if(mode == HB_CONDENSE_INT8_CRT) HB_CHECK(hb_syrk_rows_crt(k->ctx, M, k->n, rows->dev, rows->aligned, d, C, M, fuse_rx, tdot));
+    else HB_CHECK(hb_syrk_rows_ozaki(k->ctx, M, k->n, rows->dev, rows->aligned, d, C, M, mode, fuse_rx, tdot));
+  }
+  if(fused) *fused = fuse;
+  return HB_OK;
+}
+
 namespace {
 
 // x = (B_k + D_x)^{-1} rhs
@@ -619,7 +665,7 @@ int hess_solve(hb_lowrank* k, const double* rhs, double* x)
   return HB_OK;
 }
 
-int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx = nullptr);
+int condense_enqueue(hb_lowrank* k, const double* fuse_rx = nullptr);
 int condense_finish(hb_lowrank* k);
 
 
@@ -629,10 +675,7 @@ int do_condense_async(hb_lowrank* k, const double* fuse_rx = nullptr)
 {
   HB_REQUIRE(k->have_update, "hb_lowrank_condense: call hb_lowrank_update first");
   HB_REQUIRE(jac_set(k), "hb_lowrank_condense: Jacobian not set");
-  // AUTO = exact FP64 DMMA: on H100 (700 W) at n = 1e6, m = 1000 the int8-slice GEMM takes as long as the DMMA kernel (37.4 against
-  // 38.1 ms) and the row-maximum and slicing passes over J come on top (step 49.9 against 44.4 ms), so the emulation runs only on request
-  const int mode = k->condense_mode < 0 ? 0 : k->condense_mode;
-  HB_CHECK(condense_enqueue(k, mode, fuse_rx));
+  HB_CHECK(condense_enqueue(k, fuse_rx));
   k->check_pending = true;
   k->cond_valid = true; // optimistic: a failure is reported by the next synchronous call (hb_lowrank_check / hb_lowrank_condense)
   return HB_OK;
@@ -663,36 +706,15 @@ int do_condense(hb_lowrank* k)
   return condense_check(k);
 }
 
-// fuse_rx (optional): the x-block of the right-hand side the caller is about to solve for. The int8-slice condensation has to sweep all
-// rows for their maxima anyway; the same sweep then leaves tdot = [J; S; Y] (DhInv .* rx), from which step 2 of solveCompressed follows
-// without reading J again (see solve_compressed). The FP64 kernel computes the same dots as one more row of its SYRK, which is free
-// when it fits in the padding of the last 128-row tile (otherwise a whole tile row would cost more than the sweep it saves); rx must be
-// 16-byte aligned to keep the fast kernel.
-int condense_enqueue(hb_lowrank* k, int mode, const double* fuse_rx)
+// fuse_rx (optional): the x-block of the right-hand side the caller is about to solve for; jac_gram leaves tdot = [J; S; Y] (DhInv .* rx)
+// where that costs no extra pass over J, from which step 2 of solveCompressed follows without reading J again (see solve_compressed)
+int condense_enqueue(hb_lowrank* k, const double* fuse_rx)
 {
-  hb_ctx* c = k->ctx;
-  const int m = k->m, l = k->l, Ma = m + 2 * l;
+  const int Ma = k->m + 2 * k->l;
   k->tdot_valid = false;
   if(Ma > 0) {
-    if(mode == 0) {
-      const bool fuse = fuse_rx && m > 0 && hb_syrk_extra_row_is_free(Ma) && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
-      HB_CHECK(jac_syrk(k, Ma, k->DhInv, k->Caug, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
-      k->tdot_valid = fuse;
-    } else {
-      const hb_rowtab* rows;
-      HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT
-                                ? "hb_lowrank_condense: the int8 Chinese-remainder condensation (mode 100; AUTO and 0 condense in FP64)"
-                                : "hb_lowrank_condense: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)",
-                         nullptr, &rows));
-      const bool fuse = fuse_rx && m > 0;
-      if(fuse && k->n == 0) HB_CUDA(cudaMemsetAsync(k->tdot, 0, sizeof(double) * Ma, c->stream));
-      if(mode == HB_CONDENSE_INT8_CRT)
-        HB_CHECK(hb_syrk_rows_crt(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
-      else
-        HB_CHECK(hb_syrk_rows_ozaki(c, Ma, k->n, rows->dev, rows->aligned, k->DhInv, k->Caug, Ma, mode, fuse ? fuse_rx : nullptr, fuse ? k->tdot.get() : nullptr));
-      k->tdot_valid = fuse;
-    }
-    k->condense_used = mode;
+    HB_CHECK(jac_gram(k, "hb_lowrank_condense", Ma, k->DhInv, k->Caug, fuse_rx, k->tdot, &k->tdot_valid));
+    k->condense_used = mode_resolved(k->condense_mode);
   }
   return condense_finish(k);
 }
@@ -760,11 +782,7 @@ extern "C" int hb_lowrank_create(hb_ctx* c, long long n_local, int m_eq, int m_i
   std::unique_ptr<hb_lowrank> k(new hb_lowrank);
   k->ctx = c; k->n = n_local; k->meq = m_eq; k->mineq = m_ineq; k->m = m_eq + m_ineq; k->lmax = l_max;
   k->jl = device_layout(n_local, nullptr);
-  if(const char* e = getenv("HB_CONDENSE")) { // "oz6" | "oz7" | "oz8" | "crt" | "dmma"
-    if(e[0] == 'o' && e[1] == 'z' && e[2] >= '6' && e[2] <= '8') k->condense_mode = e[2] - '0';
-    else if(strcmp(e, "crt") == 0) k->condense_mode = HB_CONDENSE_INT8_CRT;
-    else if(e[0] == 'd') k->condense_mode = 0;
-  }
+  k->condense_mode = mode_from_env(k->condense_mode);
   const int m = k->m, Mamax = m + 2 * l_max, l2 = 2 * l_max;
   HB_CHECK(k->Dx.reserve(c, n_local, "Dx")); HB_CHECK(k->DhInv.reserve(c, n_local, "DhInv"));
   HB_CHECK(k->Dd.reserve(c, m_ineq, "Dd")); HB_CHECK(k->Dd_inv.reserve(c, m_ineq, "Dd_inv"));
@@ -938,12 +956,8 @@ extern "C" int hb_lowrank_update(hb_lowrank* k, const double* zl, const double* 
 
 extern "C" int hb_lowrank_set_condense_mode(hb_lowrank* k, int mode)
 {
-  HB_REQUIRE(k && (mode == -1 || mode == 0 || mode == 6 || mode == 7 || mode == 8 || mode == HB_CONDENSE_INT8_CRT),
-             "hb_lowrank_set_condense_mode: mode must be -1, 0, 6, 7, 8 or 100");
-  if(mode > 0)
-    HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT
-                              ? "hb_lowrank_set_condense_mode: the int8 Chinese-remainder condensation (mode 100; AUTO and 0 condense in FP64)"
-                              : "hb_lowrank_set_condense_mode: the int8-slice condensation (modes 6-8; AUTO and 0 condense in FP64)"));
+  HB_REQUIRE(k && mode_valid(mode), "hb_lowrank_set_condense_mode: mode must be -1, 0, 6, 7, 8 or 100");
+  if(mode_needs_whole_J(mode)) HB_CHECK(mode_whole_J(k, "hb_lowrank_set_condense_mode", mode, nullptr));
   k->condense_mode = mode;
   k->cond_valid = false;
   return HB_OK;
@@ -1177,7 +1191,7 @@ extern "C" int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, 
   // is condensed (exact FP64 DMMA kernel, which needs no global row scaling) while the next one is in flight; the partial C_aug are
   // added in chunk order, so the result does not depend on timing.
   constexpr size_t chunk_min_bytes = (size_t)256 << 20;
-  const bool chunked = have_J && Ma > 0 && (k->condense_mode <= 0) && (size_t)m * n * sizeof(double) >= chunk_min_bytes && n >= 2048;
+  const bool chunked = have_J && Ma > 0 && !mode_needs_whole_J(k->condense_mode) && (size_t)m * n * sizeof(double) >= chunk_min_bytes && n >= 2048;
   if(have_J) HB_CHECK(k->hJ.reserve(c, (size_t)k->m * n, "the staged Jacobian"));
   if(have_J && !chunked) {
     if(meq) HB_CUDA(cudaMemcpyAsync(k->hJ, Jc_host, sizeof(double) * (size_t)meq * n, cudaMemcpyHostToDevice, c->stream));

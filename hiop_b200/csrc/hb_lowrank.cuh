@@ -94,6 +94,13 @@ int jac_cols(hb_lowrank* k, double beta, double* y, double alpha, const double* 
 // C (M x M, ldc = M) = R diag(d) R^T over the local columns, R = the first M rows of [J; S; Y]; FP64 DMMA (hb_syrk_rows), with its
 // fused extra row when fuse_rx is given (tdot, M doubles)
 int jac_syrk(hb_lowrank* k, int M, const double* d, double* C, const double* fuse_rx = nullptr, double* tdot = nullptr);
+// The same C by the handle's condensation mode (hb_lowrank_set_condense_mode): jac_syrk, or an int8 kernel over the whole J (refused
+// for a J streamed from host memory, the error naming the entry point `who`). With fuse_rx, tdot (M doubles) = R (d .* fuse_rx) where
+// that costs no extra pass over J, and *fused tells whether it did: always for the int8 modes, which sweep all rows for their maxima
+// anyway; in FP64 only when the extra SYRK row fits in the padding of the last 128-row tile (a whole tile row would cost more than the
+// sweep it saves) and fuse_rx is 16-byte aligned (the fast kernel needs it). Never fused for a handle without Jacobian rows (m == 0).
+int jac_gram(hb_lowrank* k, const char* who, int M, const double* d, double* C, const double* fuse_rx = nullptr, double* tdot = nullptr,
+             bool* fused = nullptr);
 // The whole J on the device, for the passes that cannot run chunk by chunk: the int8-slice condensation and LSQ matrix (a global
 // row-maximum pass comes first) and the J_prev update of the secant (a device copy of J). *J (m x n, ld n) and *rows (the table of
 // [J rows (m); S rows (l); Y rows (l)]) as asked for; HB_ERR_INVALID, naming `who`, for a J streamed from host memory.

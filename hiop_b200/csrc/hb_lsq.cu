@@ -48,16 +48,8 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   HB_CHECK(k->lsq_M.reserve(c, (size_t)m * m + 2 * m, "the LSQ workspace"));
   double* M = k->lsq_M;
   double* rhs = M + (size_t)m * m;
-  // J J^T: rows 0..m-1 of the row-pointer table are the Jacobian rows
-  const int mode = k->condense_mode < 0 ? 0 : k->condense_mode; // AUTO = exact FP64 DMMA, as for the condensation
-  if(mode == 0) HB_CHECK(jac_syrk(k, m, nullptr, M));
-  else {
-    const hb_rowtab* rows;
-    HB_CHECK(jac_whole(k, mode == HB_CONDENSE_INT8_CRT ? "hb_lowrank_lsq_duals: the int8 Chinese-remainder mode 100" : "hb_lowrank_lsq_duals: the int8-slice modes 6-8",
-                       nullptr, &rows));
-    if(mode == HB_CONDENSE_INT8_CRT) HB_CHECK(hb_syrk_rows_crt(c, m, n, rows->dev, rows->aligned, nullptr, M, m, nullptr, nullptr));
-    else HB_CHECK(hb_syrk_rows_ozaki(c, m, n, rows->dev, rows->aligned, nullptr, M, m, mode, nullptr, nullptr));
-  }
+  // J J^T by the condensation's kernel: rows 0..m-1 of the row-pointer table are the Jacobian rows
+  HB_CHECK(jac_gram(k, "hb_lowrank_lsq_duals", m, nullptr, M));
   HB_CHECK(hb_allreduce_sum(c, M, (long long)m * m));
   // rhs = -J vecx (all-reduced), then the d-side terms on the replicated part
   if(n > 0) {

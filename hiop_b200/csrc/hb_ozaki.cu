@@ -410,36 +410,26 @@ k_oz_fixup(int M, int n_tiles, const int2* __restrict__ tile_ij, int splits, con
   }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-} // namespace
-
-// one state per CONTEXT (it used to be per device: two contexts on one GPU would have shared the slice buffer across their streams)
-struct OzState
+void put_item(void* dst, int bi, int bj, int, int k_begin, int k_count, int slot)
 {
-  int M = -1, S = 0, splits = 0, n_tiles = 0, n_items = 0; // (M, K, S): the shape the work list and tensor maps were built for
-  long long K = -1, Kpad = 0;
-  int Mpad = 0;
-  hb_dev<int8_t> Q;
-  hb_rowscale rs;
-  hb_dev<OzItem> d_items;
-  hb_dev<int2> d_tiles;
-  CUtensorMap mapA, mapB;
-  PFN_encodeTiled encode = nullptr; // cuTensorMapEncodeTiled, resolved on first use
-};
-void hb_delete(OzState* p) { delete p; }
+  const OzItem it = {bi, bj, k_begin, k_count, slot};
+  memcpy(dst, &it, sizeof(it));
+}
 
-namespace {
-
-template <int S>
-int launch_gemm(hb_ctx* c, OzState& st, int chunk_blocks, double* partial)
+// Default: one wave, splits = SMs / tiles (every CTA gets one item). Where that leaves the machine badly filled (144 tiles at m = 1000
+// or 1024 on 132 SMs: two waves, 55 % busy) several waves of the persistent CTAs are searched (hb_split_search): e.g. 11 splits = 1584
+// items = 12 full waves -> 1.091 of one tile's full-K time, the ideal 144/132.
+int oz_splits(const hb_ctx* c, long long nt, long long kstages, int max_splits, size_t tile_bytes)
 {
-  const size_t smem = OzCfg<S>::SMEM;
-  const int G = st.n_items < c->num_sms ? st.n_items : c->num_sms;
-  k_oz_gemm<S><<<G, OZ_THREADS, smem, c->stream>>>(st.mapA, st.mapB, st.d_items, st.n_items, chunk_blocks, partial);
-  HB_LAUNCHED();
-  return HB_OK;
+  int splits = (int)(c->num_sms / (nt > 0 ? nt : 1));
+  if(splits < 1) splits = 1;
+  if(splits > kstages) splits = (int)(kstages > 0 ? kstages : 1);
+  const long long items0 = nt * splits;
+  const long long waves0 = (items0 + c->num_sms - 1) / c->num_sms;
+  const double util0 = nt > 0 ? (double)items0 / (double)(waves0 * c->num_sms) : 1.0;
+  if(util0 < 0.7) splits = hb_split_search(c, nt, kstages, max_splits, tile_bytes, splits, (double)waves0 / splits);
+  if(splits > kstages) splits = (int)(kstages > 0 ? kstages : 1);
+  return splits;
 }
 
 } // namespace
@@ -485,6 +475,82 @@ int hb_row_exponents(hb_ctx* c, hb_rowscale& rs, int M, int Mpad, long long K, c
   return HB_OK;
 }
 
+void hb_delete(hb_int8_state* p) { delete p; }
+
+int hb_int8_empty(hb_ctx* c, int M, double* C, int ldc)
+{
+  if(M > 0) HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
+  return HB_OK;
+}
+
+int hb_split_search(const hb_ctx* c, long long units, long long kstages, int max_splits, size_t tile_bytes, int splits, double best)
+{
+  for(int sp = 1; sp <= max_splits; sp++) {
+    if(sp > 1 && (kstages / sp < 64 || (size_t)units * sp * tile_bytes > ((size_t)1 << 30))) break;
+    const double cost = (double)((units * sp + c->num_sms - 1) / c->num_sms) / sp;
+    if(cost < best * (1.0 - 1e-3)) { best = cost; splits = sp; }
+  }
+  return splits;
+}
+
+int hb_int8_prepare(hb_ctx* c, hb_state<hb_int8_state>& slot, const hb_int8_layout& L, int M, long long K, hb_int8_state** out)
+{
+  if(!slot) slot.reset(new hb_int8_state);
+  hb_int8_state& st = *slot;
+  if(!st.encode) {
+    cudaDriverEntryPointQueryResult qres;
+    HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&st.encode, cudaEnableDefault, &qres));
+    if(!st.encode) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver%s", "");
+  }
+  const int Mpad = ((M + L.tm - 1) / L.tm) * L.tm;
+  const long long Kpad = ((K + KS - 1) / KS) * KS;
+  const size_t qbytes = (size_t)L.planes * Mpad * Kpad;
+  if(!st.Q || st.Q.capacity() < qbytes) {
+    st.M = -1; // the tensor maps hold the address of Q
+    HB_CHECK(st.Q.reserve(c, qbytes, "the int8 planes"));
+  }
+  const char* env = getenv(L.split_env);
+  const int max_splits = env ? atoi(env) : 16;
+  if(st.M != M || st.K != K || st.planes != L.planes || st.max_splits != max_splits) {
+    st.M = -1;
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    const int nbi = Mpad / L.tm, nbj = Mpad / L.tn;
+    std::vector<int2> tiles;
+    for(int bi = 0; bi < nbi; bi++)
+      for(int bj = (L.tm / L.tn) * bi; bj < nbj; bj++)
+        if(bj * L.tn < M) tiles.push_back(make_int2(bi, bj));
+    const int nt = (int)tiles.size();
+    const long long kstages = Kpad / KS;
+    const int splits = L.splits(c, (long long)nt * L.groups, kstages, max_splits, L.tile_bytes);
+    // split-major: the CTAs running at once sweep the same K window (of the same plane) -> operand reuse in L2
+    const int n_items = splits * L.groups * nt;
+    std::vector<unsigned char> items((size_t)n_items * L.item_bytes);
+    unsigned char* it = items.data();
+    for(int s = 0; s < splits; s++)
+      for(int g = 0; g < L.groups; g++)
+        for(int t = 0; t < nt; t++, it += L.item_bytes) {
+          const long long b = hb_part_begin(kstages, splits, s), e = hb_part_begin(kstages, splits, s + 1);
+          L.put_item(it, tiles[t].x, tiles[t].y, g, (int)b, (int)(e - b), (t * L.groups + g) * splits + s);
+        }
+    HB_CHECK(st.items.reserve(c, items.size(), "the int8 work list"));
+    HB_CHECK(st.tiles.reserve(c, nt, "the int8 tile list"));
+    HB_CUDA(cudaMemcpy(st.items, items.data(), items.size(), cudaMemcpyHostToDevice));
+    HB_CUDA(cudaMemcpy(st.tiles, tiles.data(), sizeof(int2) * nt, cudaMemcpyHostToDevice));
+    const cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Mpad, (cuuint64_t)L.planes};
+    const cuuint64_t strides[2] = {(cuuint64_t)Kpad, (cuuint64_t)Kpad * Mpad};
+    const cuuint32_t es[3] = {1, 1, 1};
+    for(int i = 0; i < L.n_maps; i++)
+      if(st.encode(&st.maps[i], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, L.box[i], es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled failed%s", "");
+    st.M = M; st.K = K; st.planes = L.planes; st.max_splits = max_splits;
+    st.Mpad = Mpad; st.Kpad = Kpad; st.splits = splits; st.n_tiles = nt; st.n_items = n_items;
+  }
+  HB_CHECK(hb_ws_reserve(c, L.tile_bytes * st.n_items));
+  *out = &st;
+  return HB_OK;
+}
+
 int hb_ozaki_init_attrs(hb_ctx* c)
 {
   HB_CUDA(cudaFuncSetAttribute(k_oz_gemm<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)OzCfg<6>::SMEM));
@@ -493,118 +559,46 @@ int hb_ozaki_init_attrs(hb_ctx* c)
   return HB_OK;
 }
 
-// Same contract as hb_syrk_rows (C = A diag(d) A^T, both triangles), computed with S int8 slices on the integer tensor cores.
-// dot_x/dot_out (optional, device): dot_out[i] = sum_k row_i[k] d[k] dot_x[k] over the local columns, produced by the row-maximum pass
+// Same contract as hb_syrk_rows (C = A diag(d) A^T, both triangles), computed with S int8 slices on the integer tensor cores
 int hb_syrk_rows_ozaki(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool rows_aligned16, const double* d, double* C, int ldc, int S,
                        const double* dot_x, double* dot_out)
 {
   HB_REQUIRE(c && M >= 0 && K >= 0 && ldc >= M && (S == 6 || S == 7 || S == 8), "hb_syrk_rows_ozaki: bad arguments");
-  if(M == 0) return HB_OK;
-  if(K == 0) {
-    HB_CUDA(cudaMemset2DAsync(C, sizeof(double) * ldc, 0, sizeof(double) * M, M, c->stream));
-    return HB_OK;
-  }
-  if(!c->oz) c->oz.reset(new OzState);
-  OzState& st = *c->oz;
-  if(!st.encode) {
-    cudaDriverEntryPointQueryResult qres;
-    HB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&st.encode, cudaEnableDefault, &qres));
-    if(!st.encode) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled is not available in this driver%s", "");
-  }
-  const int Mpad = ((M + TM - 1) / TM) * TM;
-  const long long Kpad = ((K + KS - 1) / KS) * KS;
-  const size_t qbytes = (size_t)S * Mpad * Kpad;
-  if(!st.Q || st.Q.capacity() < qbytes) {
-    st.M = -1; // the tensor maps hold the address of Q
-    HB_CHECK(st.Q.reserve(c, qbytes, "the int8 slice buffer"));
-  }
-  if(st.M != M || st.K != K || st.S != S) {
-    // schedule: tiles (bi, bj) with bj >= (TM / TN) bi cover the upper triangle; split K so that ~all SMs get one item
-    st.M = -1;
-    HB_CUDA(cudaStreamSynchronize(c->stream));
-    const int nbi = Mpad / TM, nbj = Mpad / TN;
-    std::vector<int2> tiles;
-    for(int bi = 0; bi < nbi; bi++)
-      for(int bj = (TM / TN) * bi; bj < nbj; bj++)
-        if(bj * TN < M) tiles.push_back(make_int2(bi, bj));
-    const int nt = (int)tiles.size();
-    const long long kstages = Kpad / KS;
-    // K splits. Default: one wave, splits = SMs / tiles (every CTA gets one item).
-    // Where that leaves the machine badly filled (144 tiles at m = 1000 or 1024 on 132 SMs: two waves, 55 % busy) several waves of the
-    // persistent CTAs are considered: the makespan is ceil(tiles * splits / SMs) / splits of one tile's full-K time, e.g. 11 splits =
-    // 1584 items = 12 full waves -> 1.091, the ideal 144/132. Bounds there: >= 64 K stages per split, partial-tile workspace <= 1 GB,
-    // <= 16 splits; ties go to the smaller count.
-    int splits = c->num_sms / (nt > 0 ? nt : 1);
-    if(splits < 1) splits = 1;
-    if(splits > kstages) splits = (int)(kstages > 0 ? kstages : 1);
-    {
-      const long long items0 = (long long)nt * splits;
-      const long long waves0 = (items0 + c->num_sms - 1) / c->num_sms;
-      const double util0 = nt > 0 ? (double)items0 / (double)(waves0 * c->num_sms) : 1.0;
-      if(util0 < 0.7) {
-        double best = (double)waves0 / splits;
-        const int smax = getenv("HB_OZ_MAX_SPLITS") ? atoi(getenv("HB_OZ_MAX_SPLITS")) : 16;
-        for(int sp = 1; sp <= smax; sp++) {
-          if(sp > 1 && (kstages / sp < 64 || (size_t)nt * sp * TM * TN * sizeof(double) > ((size_t)1 << 30))) break;
-          const long long waves = ((long long)nt * sp + c->num_sms - 1) / c->num_sms;
-          const double cost = (double)waves / sp;
-          if(cost < best * (1.0 - 1e-3)) { best = cost; splits = sp; }
-        }
-      }
-    }
-    if(splits > kstages) splits = (int)(kstages > 0 ? kstages : 1);
-    std::vector<OzItem> items;
-    // split-major order: the CTAs of one split sweep the same K range concurrently (operand reuse in L2)
-    for(int s = 0; s < splits; s++)
-      for(int t = 0; t < nt; t++) {
-        OzItem it;
-        it.bi = tiles[t].x; it.bj = tiles[t].y;
-        const long long b = hb_part_begin(kstages, splits, s), e2 = hb_part_begin(kstages, splits, s + 1);
-        it.k_begin = (int)b; it.k_count = (int)(e2 - b);
-        it.slot = t * splits + s;
-        items.push_back(it);
-      }
-    HB_CHECK(st.d_items.reserve(c, items.size(), "the int8-slice work list"));
-    HB_CHECK(st.d_tiles.reserve(c, nt, "the int8-slice tile list"));
-    HB_CUDA(cudaMemcpy(st.d_items, items.data(), sizeof(OzItem) * items.size(), cudaMemcpyHostToDevice));
-    HB_CUDA(cudaMemcpy(st.d_tiles, tiles.data(), sizeof(int2) * nt, cudaMemcpyHostToDevice));
-    cuuint64_t dims[3] = {(cuuint64_t)Kpad, (cuuint64_t)Mpad, (cuuint64_t)S};
-    cuuint64_t strides[2] = {(cuuint64_t)Kpad, (cuuint64_t)Kpad * Mpad};
-    cuuint32_t boxA[3] = {KS, TM, 1}, boxB[3] = {KS, TN, (cuuint32_t)S}, es[3] = {1, 1, 1};
-    CUresult r1 = st.encode(&st.mapA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxA, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    CUresult r2 = st.encode(&st.mapB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, st.Q, dims, strides, boxB, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if(r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS) return hb_fail(HB_ERR_CUDA, "cuTensorMapEncodeTiled failed%s", "");
-    st.M = M; st.K = K; st.S = S; st.Mpad = Mpad; st.Kpad = Kpad; st.splits = splits; st.n_tiles = nt; st.n_items = (int)items.size();
-  }
+  if(M == 0 || K == 0) return hb_int8_empty(c, M, C, ldc);
+  // 128 x 32 tiles; one item per (tile, K range) multiplies all S slices: per K stage one box of A per slice, one of B with all S
+  const hb_int8_layout L = {S, TM, TN, 1, sizeof(double) * TM * TN, sizeof(OzItem), put_item, oz_splits, "HB_OZ_MAX_SPLITS",
+                            2, {{KS, TM, 1}, {KS, TN, (cuuint32_t)S}}};
+  hb_int8_state* st;
+  HB_CHECK(hb_int8_prepare(c, c->oz, L, M, K, &st));
+  const int Mpad = st->Mpad;
+  const long long Kpad = st->Kpad;
   // 1. sqrt(d), row maxima, exponents, slices
   const double* sd;
-  HB_CHECK(hb_row_exponents(c, st.rs, M, Mpad, K, rowptr_dev, rows_aligned16, d, dot_x, dot_out, &sd));
+  HB_CHECK(hb_row_exponents(c, st->rs, M, Mpad, K, rowptr_dev, rows_aligned16, d, dot_x, dot_out, &sd));
   const unsigned sx = (unsigned)((Kpad / 8 + 255) / 256);
   const int vec_ok = rows_aligned16 ? 1 : 0;
-  if(S == 6) k_oz_slice<6><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
-  else if(S == 7) k_oz_slice<7><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
-  else k_oz_slice<8><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st.rs.e, st.Q, vec_ok);
+  if(S == 6) k_oz_slice<6><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st->rs.e, st->Q, vec_ok);
+  else if(S == 7) k_oz_slice<7><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st->rs.e, st->Q, vec_ok);
+  else k_oz_slice<8><<<dim3(sx, Mpad), 256, 0, c->stream>>>(rowptr_dev, M, Mpad, K, Kpad, sd, st->rs.e, st->Q, vec_ok);
   HB_LAUNCHED();
   hb_phase_mark(c, HB_PH_OZ_SLICE);
   // 2. wgmma GEMM into FP64 partial tiles
-  HB_CHECK(hb_ws_reserve(c, sizeof(double) * (size_t)st.n_items * TM * TN));
   // (t+1) * Kc * 2^12 < 2^31 with t+1 <= S  ->  Kc <= 2^19 / S columns
   int chunk_stages = (int)((524288 / S) / KS);
   // strict: S products of |q q'| <= 2^12 per column must stay BELOW 2^31 (S = 8 gives exactly 2^31 with 512 stages of 128 columns when
   // every digit is -64, see tests/test_cpu_oz_model.py)
   while((long long)S * chunk_stages * KS * 4096 >= (1LL << 31)) chunk_stages--;
-  if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
-  if(S == 6) HB_CHECK(launch_gemm<6>(c, st, chunk_stages, (double*)c->ws));
-  else if(S == 7) HB_CHECK(launch_gemm<7>(c, st, chunk_stages, (double*)c->ws));
-  else HB_CHECK(launch_gemm<8>(c, st, chunk_stages, (double*)c->ws));
-  if(c->timing) {
-    HB_CUDA(cudaEventRecord(c->ev_syrk1, c->stream));
-    c->syrk_timed = true;
-  }
+  const int G = st->n_items < c->num_sms ? st->n_items : c->num_sms;
+  const OzItem* items = (const OzItem*)st->items.get();
+  HB_CHECK(hb_timed_syrk(c, [&] {
+    if(S == 6) k_oz_gemm<6><<<G, OZ_THREADS, OzCfg<6>::SMEM, c->stream>>>(st->maps[0], st->maps[1], items, st->n_items, chunk_stages, (double*)c->ws);
+    else if(S == 7) k_oz_gemm<7><<<G, OZ_THREADS, OzCfg<7>::SMEM, c->stream>>>(st->maps[0], st->maps[1], items, st->n_items, chunk_stages, (double*)c->ws);
+    else k_oz_gemm<8><<<G, OZ_THREADS, OzCfg<8>::SMEM, c->stream>>>(st->maps[0], st->maps[1], items, st->n_items, chunk_stages, (double*)c->ws);
+    HB_LAUNCHED();
+    return HB_OK;
+  }));
   // 3. split-K reduction, row scales, symmetrisation
-  k_oz_fixup<<<st.n_tiles, 256, 0, c->stream>>>(M, st.n_tiles, st.d_tiles, st.splits, (const double*)c->ws, st.rs.e, C, ldc);
+  k_oz_fixup<<<st->n_tiles, 256, 0, c->stream>>>(M, st->n_tiles, st->tiles, st->splits, (const double*)c->ws, st->rs.e, C, ldc);
   HB_LAUNCHED();
   return HB_OK;
 }

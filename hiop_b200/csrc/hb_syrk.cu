@@ -526,18 +526,16 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
   Schedule& S = *Sp;
   HB_CHECK(hb_ws_reserve(c, (size_t)S.nslots * BM * BM * sizeof(double)));
   const int G = S.Gl;
-  if(c->timing) HB_CUDA(cudaEventRecord(c->ev_syrk0, c->stream));
-  if(use_ws)
-    k_syrk_ws<<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
-  else if(aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0))
-    k_syrk_diag<true><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
-  else
-    k_syrk_diag<false><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
-  HB_LAUNCHED();
-  if(c->timing) {
-    HB_CUDA(cudaEventRecord(c->ev_syrk1, c->stream));
-    c->syrk_timed = true;
-  }
+  HB_CHECK(hb_timed_syrk(c, [&] {
+    if(use_ws)
+      k_syrk_ws<<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    else if(aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0))
+      k_syrk_diag<true><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    else
+      k_syrk_diag<false><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    HB_LAUNCHED();
+    return HB_OK;
+  }));
   k_syrk_fixup<<<dim3(S.ntiles, BM / 16), 256, 0, c->stream>>>(M, S.d_tile_ij, S.d_tile_slot_begin, S.d_tile_slots, (const double*)c->ws, C, ldc, tdot);
   HB_LAUNCHED();
   return HB_OK;

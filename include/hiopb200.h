@@ -302,7 +302,7 @@ int hb_lowrank_update(hb_lowrank* k, const double* zl, const double* sxl, const 
  * Returns HB_ERR_NUMERIC if N is not numerically SPD. */
 int hb_lowrank_condense(hb_lowrank* k);
 /* How the GEMM-shaped part of the condensation is computed:
- *   HB_CONDENSE_FP64_DMMA (0): exact FP64 on the DMMA pipe (mma.sync.m8n8k4.f64);
+ *   HB_CONDENSE_FP64_DMMA (0): exact FP64 on the DMMA pipe (mma.sync.m16n8k16.f64);
  *   6, 7, 8: INT8-slice (Ozaki) emulation on the Hopper integer tensor cores (wgmma) with that many 7-bit slices -- exact integer
  *   products/accumulation in registers, truncation of the operands 2^-41 / 2^-48 / 2^-55 relative to each row's largest entry;
  *   HB_CONDENSE_INT8_CRT (100): Chinese remaindering on the int8 tensor cores. Each row of B = [J;S;Y] sqrt(DhInv) (K = n_local

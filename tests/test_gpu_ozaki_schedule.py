@@ -283,7 +283,7 @@ def test_schedule_revisit_and_fresh_context_are_bit_identical(ctx):
 
 
 def test_max_splits_override_in_a_fresh_context():
-    """HB_OZ_MAX_SPLITS bounds the multi-wave split search; it is read when the schedule is built, so it takes a fresh context. With 1
+    """HB_OZ_MAX_SPLITS bounds the multi-wave split search (read on every call, like HB_CRT_MAX_SPLITS), here in a fresh context. With 1
     the search keeps one split where it would pick more, and N equals the model of that schedule (and differs from the default's)."""
     from hiop_b200.engine import Context
     G, S = _G(), 8
