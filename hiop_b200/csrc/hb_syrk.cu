@@ -7,12 +7,11 @@
 // blocks of V come out of the same pass.
 //
 // Why DMMA and not the integer tensor path: wgmma has no f64 kind; mma.sync.*.f64 (SASS DMMA) is the FP64 tensor path of sm_90a. The
-// fast kernel k_syrk_ws issues m16n8k16 (DMMA.16x8x16); m8n8k4 lowers to DMMA.8x8x4, which runs at half that rate on H100.
+// kernel k_syrk_ws issues m16n8k16 (DMMA.16x8x16); m8n8k4 lowers to DMMA.8x8x4, which runs at half that rate on H100.
 //
 // Work decomposition: 128x128 output tiles (upper triangle of the tile grid only). k_syrk_ws sweeps K in 32-column chunks through a
-// 3-stage ring filled by producer warps (see below); the generic kernel k_syrk_diag, for rows that are not 16-byte aligned, sweeps
-// BK=16 chunks through a 4-stage cp.async pipeline (row stride 20 doubles = 160 B -> the m8n8k4 fragment reads of a half-warp,
-// 4 rows x 32 B, fall into 4 distinct 32 B bank groups: conflict-free LDS.64).
+// 3-stage ring filled by producer warps (see below), for every row alignment: rows that are only 8-byte aligned (every odd n_local)
+// differ from 16-byte aligned ones in the producers' copy width alone.
 // The (tile, K-range) space is cut into one (tile, K window) per CTA in K lanes, plus stream-K ranges for the CTAs left
 // over (see build_schedule): every SM gets the same number of MMA iterations whatever M is, and the tiles of a lane
 // read the same columns at the same time. Each CTA writes its partial 128x128 tile to a workspace
@@ -20,188 +19,32 @@
 // bit-reproducible run to run (no atomics).
 #include "hb_common.cuh"
 #include "hb_ptx.cuh"
-#include <cstdlib>
 
 namespace {
 
 constexpr int BM = 128;          // tile rows = tile cols
-constexpr int BK = 16;           // doubles per K chunk
-constexpr int STAGES = 4;
-constexpr int THREADS = 256;     // 8 warps: 2 (rows) x 4 (cols), warp tile 64 x 32
-constexpr int LDS_ROW = BK + 4;  // padded row stride in doubles (160 B)
-constexpr int TILE_D = BM * LDS_ROW;
-
-struct Stage
-{
-  double a[TILE_D];
-  double b[TILE_D];
-  double d[BK];
-};
-constexpr size_t SMEM_BYTES = sizeof(Stage) * STAGES + 2 * BM * sizeof(const double*);
 
 struct Seg
 {
   int ti, tj;      // tile coordinates, ti <= tj
-  int k_begin;     // first K iteration (units of BK columns)
+  int k_begin;     // first K iteration (units of WBK columns)
   int k_count;     // number of K iterations
   int slot;        // workspace slot receiving the partial tile
 };
 
-// Loads one K chunk (BK columns starting at column k0) of the row tile(s) into a stage.
-template <bool ALIGN16>
-__device__ __forceinline__ void load_stage(Stage& st, const double* const* srow_a, const double* const* srow_b, bool diag,
-                                           const double* __restrict__ dvec_or_null, const double* __restrict__ dummy, long long k0, long long K)
-{
-  const int tid = threadIdx.x;
-  const double* dvec = dummy; // only used as a valid address for zero-byte copies
-  if(ALIGN16) {
-    const int kc = tid & 7;            // 16-byte chunk within the row
-    const long long k = k0 + kc * 2;
-    long long rem = K - k;
-    const int nb = rem >= 2 ? 16 : (rem == 1 ? 8 : 0);
-    const long long koff = nb ? k : 0; // keep the address valid when nothing is read
-#pragma unroll
-    for(int j = 0; j < 4; j++) {
-      const int row = (tid >> 3) + 32 * j;
-      const double* pa = srow_a[row];
-      hb_cp_async16(&st.a[row * LDS_ROW + kc * 2], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
-      if(!diag) {
-        const double* pb = srow_b[row];
-        hb_cp_async16(&st.b[row * LDS_ROW + kc * 2], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
-      }
-    }
-    if(tid < 8) {
-      if(dvec_or_null) {
-        const long long kd = k0 + tid * 2;
-        long long r2 = K - kd;
-        const int nbd = r2 >= 2 ? 16 : (r2 == 1 ? 8 : 0);
-        hb_cp_async16(&st.d[tid * 2], nbd ? dvec_or_null + kd : dummy, nbd);
-      } else {
-        st.d[tid * 2] = 1.0;
-        st.d[tid * 2 + 1] = 1.0;
-      }
-    }
-  } else {
-    const int kc = tid & 15;           // 8-byte chunk within the row
-    const long long k = k0 + kc;
-    const int nb = k < K ? 8 : 0;
-    const long long koff = nb ? k : 0;
-#pragma unroll
-    for(int j = 0; j < 8; j++) {
-      const int row = (tid >> 4) + 16 * j;
-      const double* pa = srow_a[row];
-      hb_cp_async8(&st.a[row * LDS_ROW + kc], pa ? pa + koff : (const double*)dvec, pa ? nb : 0);
-      if(!diag) {
-        const double* pb = srow_b[row];
-        hb_cp_async8(&st.b[row * LDS_ROW + kc], pb ? pb + koff : (const double*)dvec, pb ? nb : 0);
-      }
-    }
-    if(tid < 16) {
-      if(dvec_or_null) {
-        const long long kd = k0 + tid;
-        const int nbd = kd < K ? 8 : 0;
-        hb_cp_async8(&st.d[tid], nbd ? dvec_or_null + kd : dummy, nbd);
-      } else {
-        st.d[tid] = 1.0;
-      }
-    }
-  }
-}
-
-template <bool ALIGN16>
-__global__ void __launch_bounds__(THREADS, 1)
-k_syrk_diag(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const double* __restrict__ extra_row,
-            const Seg* __restrict__ segs, const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
-{
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  Stage* stages = reinterpret_cast<Stage*>(smem_raw);
-  const double** srow_a = reinterpret_cast<const double**>(smem_raw + sizeof(Stage) * STAGES);
-  const double** srow_b = srow_a + BM;
-
-  const int tid = threadIdx.x;
-  const int lane = tid & 31, warp = tid >> 5;
-  const int warp_m = warp & 1, warp_n = warp >> 1;
-  const int g = lane >> 2, t4 = lane & 3;
-
-  const int sb = cta_seg_begin[blockIdx.x], se = cta_seg_begin[blockIdx.x + 1];
-  for(int si = sb; si < se; si++) {
-    const Seg sg = segs[si];
-    const bool diag = sg.ti == sg.tj;
-    __syncthreads(); // previous segment fully consumed before the row tables / stages are reused
-    if(tid < BM) {
-      const int ra = sg.ti * BM + tid;
-      srow_a[tid] = ra < M ? rowptr[ra] : (ra == M ? extra_row : nullptr);
-    } else {
-      const int rb = sg.tj * BM + (tid - BM);
-      srow_b[tid - BM] = rb < M ? rowptr[rb] : (rb == M ? extra_row : nullptr);
-    }
-    __syncthreads();
-
-    double acc[8][4][2];
-#pragma unroll
-    for(int i = 0; i < 8; i++)
-#pragma unroll
-      for(int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
-
-    const int kcount = sg.k_count;
-    const long long kbase = (long long)sg.k_begin * BK;
-#pragma unroll
-    for(int s = 0; s < STAGES - 1; s++) {
-      if(s < kcount) load_stage<ALIGN16>(stages[s], srow_a, srow_b, diag, dvec, (const double*)rowptr, kbase + (long long)s * BK, K);
-      hb_cp_async_commit();
-    }
-    for(int it = 0; it < kcount; it++) {
-      hb_cp_async_wait<STAGES - 2>();
-      __syncthreads();
-      {
-        const int nx = it + STAGES - 1;
-        if(nx < kcount) load_stage<ALIGN16>(stages[nx % STAGES], srow_a, srow_b, diag, dvec, (const double*)rowptr, kbase + (long long)nx * BK, K);
-        hb_cp_async_commit();
-      }
-      const Stage& st = stages[it % STAGES];
-      const double* sA = st.a + (warp_m * 64 + g) * LDS_ROW + t4;
-      const double* sB = (diag ? st.a : st.b) + (warp_n * 32 + g) * LDS_ROW + t4;
-#pragma unroll
-      for(int kk = 0; kk < BK / 4; kk++) {
-        const double dv = st.d[kk * 4 + t4];
-        double af[8], bf[4];
-#pragma unroll
-        for(int i = 0; i < 8; i++) af[i] = sA[i * 8 * LDS_ROW + kk * 4];
-#pragma unroll
-        for(int j = 0; j < 4; j++) bf[j] = sB[j * 8 * LDS_ROW + kk * 4] * dv;
-#pragma unroll
-        for(int i = 0; i < 8; i++)
-#pragma unroll
-          for(int j = 0; j < 4; j++) hb_dmma884(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
-      }
-    }
-    hb_cp_async_wait<0>();
-
-    double* slot = ws + (size_t)sg.slot * (BM * BM);
-#pragma unroll
-    for(int i = 0; i < 8; i++) {
-      const int row = warp_m * 64 + i * 8 + g;
-#pragma unroll
-      for(int j = 0; j < 4; j++) {
-        const int col = warp_n * 32 + j * 8 + t4 * 2;
-        *reinterpret_cast<double2*>(slot + row * BM + col) = make_double2(acc[i][j][0], acc[i][j][1]);
-      }
-    }
-  }
-}
-
-
 // ---------------------------------------------------------------------------------------------------------------------
-// Warp-specialised variant (the fast path): 8 MMA warps + 4 producer warps, mbarrier full/empty ring.
-// The producers issue 16-byte cp.async copies (zero-filling rows beyond M and the K tail through the src-size operand)
+// Warp-specialised kernel: 8 MMA warps + 4 producer warps, mbarrier full/empty ring.
+// The producers issue cp.async copies (zero-filling rows beyond M and the K tail through the src-size operand)
 // and signal the stage's mbarrier with cp.async.mbarrier.arrive.noinc; the MMA warps never execute a CTA-wide barrier
 // and never compute a global address, so they drift out of phase and keep the FP64 tensor pipe busy during refills.
 // Each MMA warp owns a 64x32 block of the tile: 4 x 4 m16n8k16 accumulators, 64 doubles per thread. With one A and four B fragments
 // that does not fit the 168 registers of 384 threads, so the producer warpgroup gives its registers to the MMA warpgroups (setmaxnreg
-// 40 / 232). d scales the B fragment in registers: each product is rounded twice, as in k_syrk_diag.
+// 40 / 232). d scales the B fragment in registers: each product is rounded twice.
+// ALIGN16 (rows, d, the extra row and the row table 16-byte aligned): 16 producer threads per row, 16 bytes per copy. Otherwise
+// (every odd n_local: the packed rows of J then start on alternating 8-byte boundaries) 32 threads per row, 8 bytes per copy. The
+// copy width is the only difference: the shared layout, the MMA warps and so the summation order are the same.
 // (A first version staged rows with 256-byte cp.async.bulk copies from one producer warp: 288 bulk copies per stage
 // made the producer the bottleneck.)
-// Needs 16-byte aligned rows (else k_syrk_diag<false> runs).
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int WBK = 32;                 // doubles per K chunk
 constexpr int WSTAGES = 3;
@@ -217,6 +60,15 @@ struct WStage
 };
 constexpr size_t WSMEM_BYTES = sizeof(WStage) * WSTAGES + 2 * BM * sizeof(const double*) + 2 * WSTAGES * sizeof(unsigned long long);
 
+// a cp.async of 16 (ALIGN16) or 8 bytes, of which the first src_bytes are read and the rest zero-filled
+template <bool ALIGN16>
+__device__ __forceinline__ void cp_async_chunk(double* smem, const double* gmem, int src_bytes)
+{
+  if constexpr(ALIGN16) hb_cp_async16(smem, gmem, src_bytes);
+  else hb_cp_async8(smem, gmem, src_bytes);
+}
+
+template <bool ALIGN16>
 __global__ void __launch_bounds__(WTHREADS, 1)
 k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const double* __restrict__ dvec, const double* __restrict__ extra_row,
           const Seg* __restrict__ segs, const int* __restrict__ cta_seg_begin, double* __restrict__ ws)
@@ -246,9 +98,12 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
   if(warp >= 8) {
     // ================= producer warps =================
     hb_setmaxnreg_dec<40>();
+    constexpr int CW = ALIGN16 ? 2 : 1;     // doubles per copy
+    constexpr int LOG_LPR = ALIGN16 ? 4 : 5; // producer threads per row: WBK / CW
+    constexpr int RSTEP = WPROD >> LOG_LPR;  // rows per pass: 8 or 4
     const int p = tid - 256;          // 0..127
-    const int kc = p & 15;            // 16-byte chunk within the 256-byte row segment
-    const int r0 = p >> 4;            // rows r0 + 8*j
+    const int kc = p & ((1 << LOG_LPR) - 1); // copy within the 256-byte row segment
+    const int r0 = p >> LOG_LPR;      // rows r0 + RSTEP*j
     for(int si = sb; si < se; si++) {
       const Seg sg = segs[si];
       const bool diag = sg.ti == sg.tj;
@@ -259,23 +114,24 @@ k_syrk_ws(const double* const* __restrict__ rowptr, int M, long long K, const do
       }
       hb_bar_sync<1, WPROD>();
       for(int it = 0; it < sg.k_count; it++) {
-        const long long k = ((long long)sg.k_begin + it) * WBK + kc * 2;
+        const long long k = ((long long)sg.k_begin + it) * WBK + kc * CW;
         const long long rem = K - k;
-        const int nb = rem >= 2 ? 16 : (rem == 1 ? 8 : 0);
+        const int nb = rem >= CW ? 8 * CW : (rem == 1 ? 8 : 0); // bytes read: the K tail fills half of a 16-byte copy
         const long long koff = nb ? k : 0;
         hb_mbar_wait(&empty[stage], phase ^ 1);
         WStage& st = stages[stage];
+        // the zero-byte copies read from rowptr: a valid address aligned to the copy width (hb_syrk_rows checks 16 bytes for ALIGN16)
 #pragma unroll 4
-        for(int j = 0; j < 16; j++) {
-          const int row = r0 + 8 * j;
+        for(int j = 0; j < BM / RSTEP; j++) {
+          const int row = r0 + RSTEP * j;
           const double* pa = srow[row];
-          hb_cp_async16(&st.a[row * WLDS + kc * 2], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
+          cp_async_chunk<ALIGN16>(&st.a[row * WLDS + kc * CW], pa ? pa + koff : (const double*)rowptr, pa ? nb : 0);
           if(!diag) {
             const double* pb = srow[BM + row];
-            hb_cp_async16(&st.b[row * WLDS + kc * 2], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
+            cp_async_chunk<ALIGN16>(&st.b[row * WLDS + kc * CW], pb ? pb + koff : (const double*)rowptr, pb ? nb : 0);
           }
         }
-        if(p < 16 && dvec) hb_cp_async16(&st.d[kc * 2], nb ? dvec + k : (const double*)rowptr, nb);
+        if(p < (1 << LOG_LPR) && dvec) cp_async_chunk<ALIGN16>(&st.d[kc * CW], nb ? dvec + k : (const double*)rowptr, nb);
         hb_mbar_arrive_cp_async(&full[stage]);
         if(++stage == WSTAGES) { stage = 0; phase ^= 1; }
       }
@@ -370,9 +226,8 @@ k_syrk_fixup(int M, const int2* __restrict__ tile_ij, const int* __restrict__ ti
 
 struct Schedule
 {
-  int M = -1;      // (M, K, bk, G): the key this way was built for, M = -1 while it holds none
+  int M = -1;      // (M, K, G): the key this way was built for, M = -1 while it holds none
   long long K = -1;
-  int bk = 0;      // K-chunk (columns per iteration) the schedule counts in
   int G = 0;       // SM count the schedule was built for
   int Gl = 0;      // CTAs to launch
   long long stamp = 0;
@@ -394,14 +249,14 @@ void hb_delete(ScheduleCache* p) { delete p; }
 
 namespace {
 
-int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
+int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K)
 {
   if(!c->syrk_sched) c->syrk_sched.reset(new ScheduleCache);
   ScheduleCache& sc = *c->syrk_sched;
   Schedule* ways = sc.ways;
   int victim = 0;
   for(int w = 0; w < SCHED_WAYS; w++) {
-    if(ways[w].M == M && ways[w].K == K && ways[w].bk == bk && ways[w].G == c->num_sms) {
+    if(ways[w].M == M && ways[w].K == K && ways[w].G == c->num_sms) {
       ways[w].stamp = ++sc.clock;
       Sout = &ways[w];
       return HB_OK;
@@ -415,7 +270,7 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   HB_CUDA(cudaStreamSynchronize(c->stream));
   const int T = (M + BM - 1) / BM;
   const int ntiles = T * (T + 1) / 2;
-  const long long kiters = (K + bk - 1) / bk;
+  const long long kiters = (K + WBK - 1) / WBK;
   const long long total = (long long)ntiles * kiters;
   int G = c->num_sms;
   if(total < G) G = (int)(total > 0 ? total : 1);
@@ -487,7 +342,7 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
   HB_CUDA(cudaMemcpy(S.d_tile_slots, tsl.data(), sizeof(int) * tsl.size(), cudaMemcpyHostToDevice));
   HB_CUDA(cudaMemcpy(S.d_tile_ij, tij.data(), sizeof(int2) * ntiles, cudaMemcpyHostToDevice));
   HB_CUDA(cudaMemcpy(S.d_segs, segs.data(), sizeof(Seg) * segs.size(), cudaMemcpyHostToDevice));
-  S.M = M; S.K = K; S.bk = bk; S.G = c->num_sms; S.Gl = G; S.ntiles = ntiles; S.nslots = (int)cta_begin[G];
+  S.M = M; S.K = K; S.G = c->num_sms; S.Gl = G; S.ntiles = ntiles; S.nslots = (int)cta_begin[G];
   return HB_OK;
 }
 
@@ -495,9 +350,8 @@ int build_schedule(hb_ctx* c, Schedule*& Sout, int M, long long K, int bk)
 
 int hb_syrk_init_attrs(hb_ctx* c)
 {
-  HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  HB_CUDA(cudaFuncSetAttribute(k_syrk_diag<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-  HB_CUDA(cudaFuncSetAttribute(k_syrk_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WSMEM_BYTES));
+  HB_CUDA(cudaFuncSetAttribute(k_syrk_ws<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WSMEM_BYTES));
+  HB_CUDA(cudaFuncSetAttribute(k_syrk_ws<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WSMEM_BYTES));
   return HB_OK;
 }
 
@@ -505,7 +359,8 @@ int hb_syrk_init_attrs(hb_ctx* c)
 bool hb_syrk_extra_row_is_free(int M) { return (M + BM) / BM == (M + BM - 1) / BM; }
 
 // rowptr: DEVICE table of M row pointers (each row K doubles, K-contiguous). d: length K (device) or NULL (= ones).
-// C: M x M (ldc), both triangles written. `aligned16`: every row pointer and d are 16-byte aligned.
+// C: M x M (ldc), both triangles written. `aligned16`: every row pointer is 16-byte aligned; with d, fuse_rx and the table itself
+// also 16-byte aligned, k_syrk_ws copies 16 bytes at a time, else 8.
 // fuse_rx (optional, device, length K): swept as row M of the same pass; tdot[i] = sum_k row_i[k] d[k] fuse_rx[k] for i < M. It costs
 // no extra MMA when M + 1 rows need no more 128-row tiles than M.
 int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev, bool aligned16, const double* d, double* C, int ldc,
@@ -518,21 +373,17 @@ int hb_syrk_rows(hb_ctx* c, int M, long long K, const double* const* rowptr_dev,
     if(tdot) HB_CUDA(cudaMemsetAsync(tdot, 0, sizeof(double) * M, c->stream));
     return HB_OK;
   }
-  const bool d_aligned = (reinterpret_cast<uintptr_t>(d) & 15u) == 0 && (reinterpret_cast<uintptr_t>(fuse_rx) & 15u) == 0;
-  const char* force_generic = getenv("HB_SYRK_GENERIC");
-  const bool use_ws = aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0) && !(force_generic && force_generic[0] == '1');
+  const bool align16 = aligned16 && ((reinterpret_cast<uintptr_t>(d) | reinterpret_cast<uintptr_t>(fuse_rx) | reinterpret_cast<uintptr_t>(rowptr_dev)) & 15u) == 0;
   Schedule* Sp = nullptr;
-  HB_CHECK(build_schedule(c, Sp, M + (fuse_rx ? 1 : 0), K, use_ws ? WBK : BK));
+  HB_CHECK(build_schedule(c, Sp, M + (fuse_rx ? 1 : 0), K));
   Schedule& S = *Sp;
   HB_CHECK(hb_ws_reserve(c, (size_t)S.nslots * BM * BM * sizeof(double)));
   const int G = S.Gl;
   HB_CHECK(hb_timed_syrk(c, [&] {
-    if(use_ws)
-      k_syrk_ws<<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
-    else if(aligned16 && d_aligned && ((reinterpret_cast<uintptr_t>(rowptr_dev) & 15u) == 0))
-      k_syrk_diag<true><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+    if(align16)
+      k_syrk_ws<true><<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
     else
-      k_syrk_diag<false><<<G, THREADS, SMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
+      k_syrk_ws<false><<<G, WTHREADS, WSMEM_BYTES, c->stream>>>(rowptr_dev, M, K, d, fuse_rx, S.d_segs, S.d_cta_seg_begin, (double*)c->ws);
     HB_LAUNCHED();
     return HB_OK;
   }));

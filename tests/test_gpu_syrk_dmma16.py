@@ -5,11 +5,13 @@ K < 2^14, every product J_ik DhInv_k J_jk is a multiple of 2^-3 of magnitude at 
 multiple of 2^-3 below 2^27 and exact. So N and
 the fused row dots tdot = J (DhInv .* rx) (integer rx) must equal the exact result bit for bit, whatever order the tensor core sums in:
 an A or B fragment element read from the wrong row, column or K slot, a missed K tail or a lost accumulator shows up as a wrong entry
-that a tolerance would hide. The cases reach every branch of build_schedule on the running device, K mod 32 in {0, 2, 16, 30}, diagonal
-and off-diagonal tiles, and the fused rhs row at M = 1012.
+that a tolerance would hide. The cases reach every branch of build_schedule on the running device with both producers of k_syrk_ws: even
+K (16-byte copies, K mod 32 in {0, 2, 16, 30}) and odd K with several rows (8-byte copies, K mod 32 in {1, 15, 17, 31}), diagonal and
+off-diagonal tiles, and the fused rhs row at M = 1012.
 
-The SASS check runs without a GPU: k_syrk_ws in the built library issues DMMA.16x8x16 only (DMMA.8x8x4 is the half-rate shape on
-sm_90a) and has no local-memory traffic (a register spill would show as LDL / STL)."""
+The SASS check runs without a GPU: both instantiations of k_syrk_ws in the built library issue DMMA.16x8x16 only (DMMA.8x8x4 is the
+half-rate shape on sm_90a) and have no local-memory traffic (a register spill would show as LDL / STL); no kernel of hb_syrk.cu
+issues DMMA.8x8x4."""
 import os
 import re
 import shutil
@@ -24,13 +26,15 @@ from test_gpu_syrk_schedule import _G, _setup, case_shape, ctx, schedule_branch 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # (branch, K, rows short of a full last tile, preferred tile-row count T); the T is moved to the nearest one whose schedule is the
-# named branch on this device, as in test_gpu_syrk_schedule.py
+# named branch on this device, as in test_gpu_syrk_schedule.py. Odd K (every M here is > 1) runs the 8-byte producer.
 CASES = [
     ("lanes, R = 0", 4126, 0, 2), ("lanes, R = 0", 12288, 8, 11),
     ("lanes, R > 0", 8194, 12, 4), ("lanes, R > 0", 12016, 24, 8),
     ("L = 1", 12030, 36, 12), ("L = 1", 12000, 20, 15),
     ("stream-K", 12288, 48, 16), ("stream-K", 12018, 0, 17),
     ("reduced G", 1600, 28, 1), ("reduced G", 1040, 56, 2),
+    ("lanes, R = 0", 12001, 0, 2), ("lanes, R > 0", 12015, 24, 8), ("L = 1", 12017, 36, 12),
+    ("stream-K", 12031, 0, 17), ("reduced G", 1041, 56, 2), ("reduced G", 1583, 28, 1),
 ]
 
 
@@ -82,8 +86,8 @@ def _run(ctx, P, fused):
 def test_ws_condensation_is_exact(ctx, case):
     G = _G()
     branch, K, short, T0 = case
-    M, K, bk = case_shape((branch, "ws", K, short, T0), G)
-    assert schedule_branch(M, K, bk, G)[0] == branch and K % 2 == 0
+    M, K = case_shape((branch, "ws" if K % 2 == 0 else "odd", K, short, T0), G)
+    assert schedule_branch(M, K, G)[0] == branch and M > 1
     P = _exact_problem(M, K, seed=M + K)
     N, _, DhInv, Dd_inv = _run(ctx, P, fused=False)
     Nref, _ = _exact_reference(P, DhInv, Dd_inv)
@@ -92,9 +96,9 @@ def test_ws_condensation_is_exact(ctx, case):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("K", [12000, 12002, 12016, 12030])
+@pytest.mark.parametrize("K", [12000, 12002, 12016, 12030, 12001, 12031])
 def test_ws_fused_row_is_exact(ctx, K):
-    """M = 1012: the rhs row is row 1012 of the eighth tile row (no extra tile), its dots go to tdot"""
+    """M = 1012: the rhs row is row 1012 of the eighth tile row (no extra tile), its dots go to tdot; odd K runs the 8-byte producer"""
     M = 1012
     P = _exact_problem(M, K, seed=K)
     N, tdot, DhInv, Dd_inv = _run(ctx, P, fused=True)
@@ -103,21 +107,26 @@ def test_ws_fused_row_is_exact(ctx, K):
     assert np.array_equal(tdot[:M], tref), int((tdot[:M] != tref).sum())
 
 
-def _kernel_sass(name):
-    """SASS of the kernel whose mangled name contains `name`, from hiop_b200/libhiopb200.so"""
+def _library_sass():
+    """{mangled kernel name: SASS} of hiop_b200/libhiopb200.so"""
     lib = os.path.join(ROOT, "hiop_b200", "libhiopb200.so")
     out = subprocess.run(["cuobjdump", "-sass", lib], check=True, capture_output=True, text=True).stdout
     blocks = re.split(r"\n\s*Function : ", out)
-    found = [b for b in blocks[1:] if name in b.split("\n", 1)[0]]
-    assert len(found) == 1, f"{len(found)} SASS functions named like {name}"
-    return found[0]
+    return {b.split("\n", 1)[0].strip(): b for b in blocks[1:]}
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_ws_sass_is_dmma16x8x16_without_spills():
+def test_syrk_sass_is_dmma16x8x16_without_spills():
     if not os.path.exists(os.path.join(ROOT, "hiop_b200", "libhiopb200.so")):
         pytest.skip("libhiopb200.so not built")
-    sass = _kernel_sass("k_syrk_ws")
-    shapes = set(re.findall(r"\bDMMA\.(\w+)", sass))
-    assert shapes == {"16x8x16"}, shapes
-    assert not re.search(r"\b(LDL|STL)\b", sass)
+    sass = _library_sass()
+    ws = {name: body for name, body in sass.items() if "k_syrk_wsILb" in name}
+    assert sorted(re.search(r"k_syrk_wsILb(\d)", name).group(1) for name in ws) == ["0", "1"], sorted(ws)
+    for name, body in ws.items():
+        shapes = set(re.findall(r"\bDMMA\.(\w+)", body))
+        assert shapes == {"16x8x16"}, (name, shapes)
+        assert not re.search(r"\b(LDL|STL)\b", body), name
+    assert not [name for name in sass if "k_syrk_diag" in name]
+    syrk = {name: body for name, body in sass.items() if "_hb_syrk_cu_" in name}
+    assert len(syrk) == 3, sorted(syrk)  # the two k_syrk_ws instantiations and k_syrk_fixup
+    assert not [name for name, body in syrk.items() if "DMMA.8x8x4" in body]

@@ -6,13 +6,11 @@ problems max|N| is the all-ones row's N_00 ~ 0.3 n, so the old check was an FP32
 
 build_schedule cuts the upper triangle of 128 x 128 output tiles (T tile rows, ntiles = T(T+1)/2) and the K iterations over the G
 streaming multiprocessors. Its branches are restated below (schedule_branch) and every case asserts the branch it is named after; the
-shapes are derived from the device's SM count, so a 114-SM H100 PCIe reaches the same branches as a 132-SM SXM part. The three kernels:
-k_syrk_ws (16-byte aligned rows, K chunks of WBK = 32), k_syrk_diag<true> (HB_SYRK_GENERIC=1, BK = 16) and k_syrk_diag<false> (odd K:
-the packed rows of J are then only 8-byte aligned). With two or more packed rows an odd K leaves k_syrk_ws, so its tails there are
-K mod 32 in {0, 2, 30}; a single row (M = 1) keeps k_syrk_ws at odd K, which reaches its 8-byte tail (K mod 32 in {1, 31}). The tails
-of k_syrk_diag are K mod 16 in {0, 1, 2, 14, 15}."""
-import os
-
+shapes are derived from the device's SM count, so a 114-SM H100 PCIe reaches the same branches as a 132-SM SXM part. One kernel,
+k_syrk_ws, sweeps K in chunks of WBK = 32 columns with two producers: 16-byte copies when the rows are 16-byte aligned ("ws": even K,
+or a single row, M = 1, whose row pointer is J itself) and 8-byte copies otherwise ("odd": odd K with two or more packed rows, which
+then start on alternating 8-byte boundaries). The "ws" K tails are K mod 32 in {0, 2, 30} and, at M = 1, the 16-byte producer's
+8-byte tail {1, 31}; the "odd" cases reach every branch with K mod 32 in {1, 15, 17, 31}."""
 import numpy as np
 import pytest
 import torch
@@ -22,14 +20,14 @@ from oracle import bounds
 
 pytestmark = pytest.mark.gpu
 
-BM, BK, WBK = 128, 16, 32
+BM, WBK = 128, 32
 
 
-def schedule_branch(M, K, bk, G):
+def schedule_branch(M, K, G):
     """build_schedule's decision (hb_syrk.cu), restated: returns (branch, launched CTAs)."""
     T = -(-M // BM)
     ntiles = T * (T + 1) // 2
-    kiters = -(-K // bk)
+    kiters = -(-K // WBK)
     total = ntiles * kiters
     Gl = G if total >= G else max(total, 1)
     L = Gl // ntiles
@@ -54,18 +52,6 @@ def ctx():
     c = Context(0)
     yield c
     c.close()
-
-
-@pytest.fixture
-def generic_kernel():
-    """HB_SYRK_GENERIC=1 (read on every call) selects k_syrk_diag<true> for aligned rows; restored afterwards."""
-    old = os.environ.get("HB_SYRK_GENERIC")
-    os.environ["HB_SYRK_GENERIC"] = "1"
-    yield
-    if old is None:
-        del os.environ["HB_SYRK_GENERIC"]
-    else:
-        os.environ["HB_SYRK_GENERIC"] = old
 
 
 def _setup(ctx, P):
@@ -99,10 +85,10 @@ def _check_N(N, Nref, B, K, G):
     return 1.0 / max(ratio, 1e-300)
 
 
-# (branch, kernel, K, rows short of a full last tile, preferred T). The tile-row count T is chosen on the running device: the preferred T
-# when it lands in the branch, else the nearest T that does (on 132 SMs every preferred T lands). K tails: K mod 32 in {0, 2, 30} for
-# k_syrk_ws with packed rows, {1, 31} for its 8-byte cp.async tail with a single row (M = 1: the row pointer is J itself, 16-byte
-# aligned, whatever K), K mod 16 in {0, 1, 2, 14, 15} for the k_syrk_diag kernels.
+# (branch, producer, K, rows short of a full last tile, preferred T). The tile-row count T is chosen on the running device: the preferred
+# T when it lands in the branch, else the nearest T that does (on 132 SMs every preferred T lands). K tails: K mod 32 in {0, 2, 30} for
+# the 16-byte producer with packed rows, {1, 31} for its 8-byte cp.async tail with a single row (M = 1: the row pointer is J itself,
+# 16-byte aligned, whatever K), {1, 15, 17, 31} for the 8-byte producer.
 CASES = [
     ("lanes, R = 0", "ws", 4126, 0, 2), ("lanes, R = 0", "ws", 6002, 84, 3), ("lanes, R = 0", "ws", 12288, 8, 11),
     ("lanes, R > 0", "ws", 8194, 12, 4), ("lanes, R > 0", "ws", 9214, 0, 6), ("lanes, R > 0", "ws", 12000, 24, 8),
@@ -111,47 +97,50 @@ CASES = [
     ("stream-K", "ws", 12288, 48, 16), ("stream-K", "ws", 12002, 0, 17),
     ("reduced G", "ws", 1600, 28, 1), ("reduced G", "ws", 1000, 56, 2),
     ("reduced G", "ws", 2017, 127, 1), ("reduced G", "ws", 2015, 127, 1),
-    ("lanes, R > 0", "generic", 8194, 12, 4), ("lanes, R > 0", "generic", 12014, 1, 9), ("stream-K", "generic", 12000, 0, 16),
-    ("lanes, R = 0", "odd", 8193, 1, 3), ("L = 1", "odd", 12015, 6, 12), ("stream-K", "odd", 12001, 1, 16), ("reduced G", "odd", 801, 28, 1),
+    ("lanes, R = 0", "odd", 8193, 1, 3), ("lanes, R = 0", "odd", 4127, 84, 2),
+    ("lanes, R > 0", "odd", 12017, 12, 4), ("lanes, R > 0", "odd", 8191, 40, 7),
+    ("L = 1", "odd", 12015, 6, 12), ("L = 1", "odd", 12031, 20, 14),
+    ("stream-K", "odd", 12001, 1, 16), ("stream-K", "odd", 12017, 0, 17),
+    ("reduced G", "odd", 801, 28, 1), ("reduced G", "odd", 1041, 56, 2), ("reduced G", "odd", 783, 100, 1),
 ]
 
 
 def case_shape(case, G):
-    """(M, K, bk) of a case on G SMs: M = 128 T - short for the T nearest the preferred one whose schedule is the named branch"""
-    branch, kernel, K, short, T0 = case
-    bk = WBK if kernel == "ws" else BK
+    """(M, K) of a case on G SMs: M = 128 T - short for the T nearest the preferred one whose schedule is the named branch"""
+    branch, producer, K, short, T0 = case
     for T in sorted(range(1, 25), key=lambda t: (abs(t - T0), t)):
         M = BM * T - short
-        if M >= 1 and schedule_branch(M, K, bk, G)[0] == branch:
-            return M, K, bk
-    pytest.fail(f"no tile-row count puts K = {K} ({kernel}) in the branch '{branch}' on {G} SMs")
+        if M >= 1 and schedule_branch(M, K, G)[0] == branch:
+            return M, K
+    pytest.fail(f"no tile-row count puts K = {K} ({producer}) in the branch '{branch}' on {G} SMs")
 
 
 @pytest.mark.parametrize("case", CASES, ids=[f"{c[0]}-{c[1]}-K{c[2]}" for c in CASES])
-def test_condensation_meets_componentwise_bound(ctx, request, case):
+def test_condensation_meets_componentwise_bound(ctx, case):
     G = _G()
-    branch, kernel = case[0], case[1]
-    M, K, bk = case_shape(case, G)
-    assert schedule_branch(M, K, bk, G)[0] == branch
-    if kernel == "generic":
-        request.getfixturevalue("generic_kernel")
-    # odd K makes packed rows 8-byte aligned (k_syrk_diag<false>) unless there is a single row
-    assert (K % 2 == 1 and M > 1) == (kernel == "odd")
+    branch, producer = case[0], case[1]
+    M, K = case_shape(case, G)
+    assert schedule_branch(M, K, G)[0] == branch
+    # odd K makes packed rows 8-byte aligned (the 8-byte producer) unless there is a single row
+    assert (K % 2 == 1 and M > 1) == (producer == "odd")
     P = synth.make_qn_problem(K, M, 0, seed=M + K)
     k, T = _setup(ctx, P)
     k.condense()
     assert k.condense_mode_used() == 0
     Nref, B = _reference(P, k.DhInv(), k.Dd_inv())
     margin = _check_N(k.N(), Nref, B, K, G)
-    print(f"M={M} K={K} {kernel}: {branch} ({schedule_branch(M, K, bk, G)[1]} CTAs of {G} SMs), margin {margin:.3g}")
+    print(f"M={M} K={K} {producer}: {branch} ({schedule_branch(M, K, G)[1]} CTAs of {G} SMs), margin {margin:.3g}")
     k.close()
 
 
 def test_every_schedule_branch_is_reached():
-    """Every branch of build_schedule has a k_syrk_ws case on this device (restated arithmetic, not the kernels' results)."""
+    """Every branch of build_schedule has a case of each producer on this device, and the 8-byte producer's cases cover K mod 32 in
+    {1, 15, 17, 31} (restated arithmetic, not the kernels' results)."""
     G = _G()
-    ws = {c[0] for c in CASES if c[1] == "ws" and case_shape(c, G)}
-    assert ws == {"lanes, R = 0", "lanes, R > 0", "L = 1", "stream-K", "reduced G"}, (G, ws)
+    for producer in ("ws", "odd"):
+        reached = {c[0] for c in CASES if c[1] == producer and case_shape(c, G)}
+        assert reached == {"lanes, R = 0", "lanes, R > 0", "L = 1", "stream-K", "reduced G"}, (G, producer, reached)
+    assert {c[2] % WBK for c in CASES if c[1] == "odd"} == {1, 15, 17, 31}
 
 
 def _numpy_direction(P, DhInv, Dd_inv):
