@@ -67,6 +67,8 @@ __global__ void k_mds_ddinv(int mi, const double* __restrict__ dwd, const double
 //   (1,2),(1,3)            : 0 + Jcd[c-nxd][r]   /  0 + Jdd[c-nxd-neq][r]                                    :205-206
 //   (2,2),(2,3),(3,3)      : 0 + (-1)*sum_k Js[i,k]/Hxs[k]*Js[j,k]  (merge-join of two sorted sparse rows)    :239,268,276
 //                            then  - delta_cc  |  - Dd_inv - delta_cd  on the diagonal                         :245,289-290
+// The explicit 0 + is not a no-op: it turns -0.0 into +0.0, as the reference's `W += alpha*x` does. Without it a pair of sparse
+// rows that shares no column (acc = 0, -1 * acc = -0.0) and every -0.0 entry of Hd / Jcd / Jdd would keep the wrong sign bit.
 __global__ void __launch_bounds__(T)
 k_mds_build(int nxs, int nxd, int neq, int nineq, const double* __restrict__ Hd, const double* __restrict__ Jcd, const double* __restrict__ Jdd,
             const double* __restrict__ Dx, const double* __restrict__ dwx, const int* __restrict__ ptr, const int* __restrict__ col,
@@ -81,15 +83,15 @@ k_mds_build(int nxs, int nxd, int neq, int nineq, const double* __restrict__ Hd,
     double v;
     if(r < nxd) {
       if(c < nxd) {
-        v = Hd[(size_t)r * nxd + c];
+        v = __dadd_rn(0.0, Hd[(size_t)r * nxd + c]);
         if(r == c) {
           v = __dadd_rn(v, Dx[nxs + r]);
           v = __dadd_rn(v, dwx[nxs + r]);
         }
       } else if(c < nxd + neq) {
-        v = Jcd[(size_t)(c - nxd) * nxd + r];
+        v = __dadd_rn(0.0, Jcd[(size_t)(c - nxd) * nxd + r]);
       } else {
-        v = Jdd[(size_t)(c - nxd - neq) * nxd + r];
+        v = __dadd_rn(0.0, Jdd[(size_t)(c - nxd - neq) * nxd + r]);
       }
     } else {
       const int i = r - nxd, j = c - nxd;
@@ -104,7 +106,7 @@ k_mds_build(int nxs, int nxd, int neq, int nineq, const double* __restrict__ Hd,
         } else if(ci < cj) ki++;
         else kj++;
       }
-      v = __dmul_rn(-1.0, acc);
+      v = __dadd_rn(0.0, __dmul_rn(-1.0, acc));
       if(i == j) {
         if(i < neq) v = __dsub_rn(v, dcc[i]);
         else {
@@ -329,7 +331,7 @@ extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* 
 // Dense-Newton KKT classes (SURVEY 8 a16): hiopKKTLinSysDenseXYcYd / hiopKKTLinSysDenseXDYcYd
 // src/Optimization/hiopKKTLinSysDense.hpp:85-207, 249-370. Same addition order per entry as the reference's sequence of
 // addUpperTriangle / transAdd / addSubDiagonal calls -> bit-identical upper triangle; the lower triangle is zero like after
-// the reference's Msys.setToZero().
+// the reference's Msys.setToZero(). Copied entries of H, Jc and Jd start from 0 + like the reference's `+=` (-0.0 -> +0.0).
 // =====================================================================================================================
 namespace {
 
@@ -360,12 +362,12 @@ k_densekkt_build(int form, int nx, int neq, int nineq, const double* __restrict_
     if(j >= i) {
       if(i < nx) {
         if(j < nx) {
-          v = H[(size_t)i * nx + j];
+          v = __dadd_rn(0.0, H[(size_t)i * nx + j]);
           if(i == j) v = __dadd_rn(__dadd_rn(v, Dx[i]), dwx[i]);
         } else if(j >= yc0 && j < yd0) {
-          v = Jc[(size_t)(j - yc0) * nx + i];
+          v = __dadd_rn(0.0, Jc[(size_t)(j - yc0) * nx + i]);
         } else if(j >= yd0) {
-          v = Jd[(size_t)(j - yd0) * nx + i];
+          v = __dadd_rn(0.0, Jd[(size_t)(j - yd0) * nx + i]);
         }
       } else if(form == 0) {
         if(i == j) {

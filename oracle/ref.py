@@ -97,6 +97,23 @@ def _i(a):
     return a, a.ctypes.data_as(ip)
 
 
+def has_sp_times_vec() -> bool:
+    """ref_sp_times_vec is newer than the rest of the harness: an oracle/_ref built before it was added lacks it (make keeps a .so
+    that is newer than ref_harness.cpp)"""
+    return hasattr(lib(), "ref_sp_times_vec")
+
+
+def sp_times_vec(trans, m, n, iRow, jCol, vals, y, alpha, x):
+    """hiopMatrixSparseTriplet::timesVec (trans = 0) / transTimesVec (trans = 1) with beta = 1 on an m x n triplet matrix; returns y_out"""
+    f = lib().ref_sp_times_vec
+    f.argtypes = [ctypes.c_int] * 4 + [ip, ip, dp, ctypes.c_double, dp, ctypes.c_double, dp]
+    f.restype = None
+    (_, pi), (_, pj), (_, pv), (_, px) = _i(iRow), _i(jCol), _d(vals), _d(x)
+    y = np.array(y, dtype=np.float64)
+    f(trans, m, n, len(iRow), pi, pj, pv, 1.0, y.ctypes.data_as(dp), alpha, px)
+    return y
+
+
 # op codes of ref_vec_op (kept in sync with the enum in ref_harness.cpp)
 OPS = dict(axdzpy_w_pattern=1, axzpy=2, axdzpy=3, component_mult=4, component_div=5, component_div_w_sel=6,
            invert=7, select_pattern=8, add_constant=9, add_constant_w_sel=10, scale=11, axpy=12,

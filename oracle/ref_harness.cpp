@@ -767,5 +767,18 @@ void ref_sp_add_MDinvNtrans(int m1, int n, int nnz1, const int* iRow1, const int
   M1.addMDinvNtransToSymDeMatUTri(row_start, col_start, alpha, vd, M2, Wm);
   memcpy(W, Wm.local_data(), sizeof(double) * (size_t)Nw * Nw);
 }
+/// y = beta*y + alpha * M * x (trans = 0) or alpha * M^T * x (trans = 1), M m x n sparse triplet   :73-89, :110-126
+void ref_sp_times_vec(int trans, int m, int n, int nnz, const int* iRow, const int* jCol, const double* vals, double beta, double* y,
+                      double alpha, const double* x)
+{
+  hiopMatrixSparseTriplet M(m, n, nnz);
+  memcpy(M.i_row(), iRow, sizeof(int) * nnz); memcpy(M.j_col(), jCol, sizeof(int) * nnz); memcpy(M.M(), vals, sizeof(double) * nnz);
+  const int ny = trans ? n : m, nx = trans ? m : n;
+  hiopVectorPar vy(ny), vx(nx);
+  memcpy(vy.local_data(), y, sizeof(double) * ny); memcpy(vx.local_data(), x, sizeof(double) * nx);
+  if(trans) M.transTimesVec(beta, vy, alpha, vx);
+  else M.timesVec(beta, vy, alpha, vx);
+  memcpy(y, vy.local_data(), sizeof(double) * ny);
+}
 
 } // extern "C"

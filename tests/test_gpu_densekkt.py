@@ -39,7 +39,7 @@ def test_dense_kkt_against_reference_golden(ctx, form):
     it = {kk: g[kk] for kk in ("zl", "sxl", "zu", "sxu", "vl", "sdl", "vu", "sdu")}
     pat = {kk: g[kk] for kk in ("ixl", "ixu", "idl", "idu")}
     M, ret, ok, sol = _run(ctx, form, g["H"], g["Jc"], g["Jd"], it, pat, (g["dwx"], g["dwd"], g["dcc"], g["dcd"]), g[f"rhs{form}"])
-    np.testing.assert_array_equal(M, g[f"ref_M{form}"])
+    np.testing.assert_array_equal(M.view(np.uint64), g[f"ref_M{form}"].view(np.uint64))
     assert ret == int(g[f"ref_ret{form}"]) and ok
     assert np.abs(sol - g[f"ref_sol{form}"]).max() <= 1e-9 * np.abs(g[f"ref_sol{form}"]).max()
 
@@ -54,7 +54,7 @@ def test_dense_kkt_against_oracle(ctx, form, nx, neq, nineq, dw, dc):
     Mo, _, _ = ko.dense_build_kkt_matrix(form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas)
     rhs = np.random.default_rng(nx).standard_normal(Mo.shape[0])
     M, ret, ok, sol = _run(ctx, form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas, rhs)
-    np.testing.assert_array_equal(M, Mo)
+    np.testing.assert_array_equal(M.view(np.uint64), Mo.view(np.uint64))
     ret_o, f = ko.symdense_matrix_changed(Mo)
     assert ret == ret_o == neq + nineq and ok         # inertia the Newton driver requires (hiopAlgFilterIPM.cpp:2084-2096)
     K = np.triu(Mo) + np.triu(Mo, 1).T
@@ -84,3 +84,63 @@ def test_write_kkt_from_device(ctx, tmp_path):
     assert np.abs(back["M"] - np.triu(M)).max() <= 1e-19 + 1e-15 * np.abs(M).max()
     assert np.array_equal(back["pairs"][0][0], np.arange(k.N, dtype=np.float64))
     k.close()
+
+
+def _dominant_problem(nx, neq, nineq, seed, frac):
+    """H diagonally dominant (so any off-diagonal entry may be zeroed), about frac of H's off-diagonal pairs and of Jc, Jd set to -0.0"""
+    r = np.random.default_rng(seed)
+    p = synth.make_mds_problem(0, nx, neq, nineq, seed=seed, dwx=1e-4, dcc=1e-8)
+    H = 0.01 * r.standard_normal((nx, nx)) / np.sqrt(nx)
+    H = H + H.T + np.diag(r.uniform(1.0, 2.0, nx))
+    Z = np.triu(r.random((nx, nx)) < frac, 1)
+    H[Z | Z.T] = -0.0
+    Jc, Jd = p.Jcd.copy(), p.Jdd.copy()
+    Jc[r.random(Jc.shape) < frac] = -0.0
+    Jd[r.random(Jd.shape) < frac] = -0.0
+    it = dict(zl=p.zl, sxl=p.sxl, zu=p.zu, sxu=p.sxu, vl=p.vl, sdl=p.sdl, vu=p.vu, sdu=p.sdu)
+    pat = dict(ixl=p.ixl, ixu=p.ixu, idl=p.idl, idu=p.idu)
+    return H, Jc, Jd, it, pat, (p.delta_wx, p.delta_wd, p.delta_cc, p.delta_cd)
+
+
+@pytest.mark.parametrize("form", [0, 1])
+def test_dense_kkt_negative_zero_inputs(ctx, form):
+    """-0.0 in H, Jc and Jd: the reference's `+=` into a zeroed Msys stores +0.0, and so must the device"""
+    H, Jc, Jd, it, pat, deltas = _dominant_problem(80, 20, 25, 41, 0.2)
+    Mo, _, _ = ko.dense_build_kkt_matrix(form, H, Jc, Jd, it, pat, deltas)
+    rhs = np.random.default_rng(42).standard_normal(Mo.shape[0])
+    M, ret, ok, _ = _run(ctx, form, H, Jc, Jd, it, pat, deltas, rhs)
+    bad = np.nonzero(M.view(np.uint64) != Mo.view(np.uint64))
+    assert bad[0].size == 0, f"{bad[0].size} entries differ, first {[(i, j, M[i, j], Mo[i, j]) for i, j in zip(*bad)][:4]}"
+    assert np.signbit(Jc).any() and not np.signbit(Mo[Mo == 0.0]).any()
+    assert ret == 20 + 25 and ok
+
+
+def test_dense_kkt_cluster_bunch_kaufman_order(ctx):
+    """XDYcYd at N = 600 + 100 + 2 * 150 = 1000, past the cluster Bunch-Kaufman threshold: bit-identical assembly, the inertia, and the
+    solve within its backward error bound for the factor read back"""
+    from oracle import bounds
+    from test_gpu_symdense_paths import readback, factor_parts, theta
+    from hiop_b200.engine import KKTLinSysDense
+    H, Jc, Jd, it, pat, deltas = _dominant_problem(600, 100, 150, 43, 0.05)
+    Mo, _, _ = ko.dense_build_kkt_matrix(1, H, Jc, Jd, it, pat, deltas)
+    N = Mo.shape[0]
+    rhs = np.random.default_rng(44).standard_normal(N)
+    D = ctx.to_device
+    k = KKTLinSysDense(ctx, 600, 100, 150, "XDYcYd")
+    k.build_kkt_matrix(D(H), D(Jc), D(Jd), {kk: D(v) for kk, v in it.items()}, {kk: D(v) for kk, v in pat.items()}, [D(d) for d in deltas])
+    M = k.Msys()
+    np.testing.assert_array_equal(M.view(np.uint64), Mo.view(np.uint64))
+    assert k.factorize() == 100 + 150
+    rb = readback(k.linSys)
+    assert rb["plan"][0] == "BK_CLUSTER", rb["plan"]
+    x = D(rhs)
+    assert k.linSys.solve(x)
+    ctx.sync()
+    sol = x.cpu().numpy()
+    k.close()
+    L, d, dsub, perm = factor_parts(rb)
+    tn = lambda t: None if t is None else t.cpu().numpy()
+    A = np.triu(Mo) + np.triu(Mo, 1).T
+    ratio, omega = bounds.solve_backward_ratio(A[perm][:, perm], sol[perm], rhs[perm], tn(L), tn(d), tn(dsub), theta(L))
+    print(f"dense KKT N={N}: plan {rb['plan']}, solve margin {1 / max(ratio, 1e-300):.3g} (omega {omega:.2e})")
+    assert ratio <= 1.0

@@ -60,7 +60,7 @@ def test_mds_against_reference_golden(ctx):
     M, ret, ok, dx, dyc, dyd = _device_run(ctx, p, True)
     N = p.nxd + p.neq + p.nineq
     iu = np.triu_indices(N)
-    np.testing.assert_array_equal(M[iu], g["ref_M"][iu])       # assembly is bit-identical to the reference's methods
+    np.testing.assert_array_equal(M[iu].view(np.uint64), g["ref_M"][iu].view(np.uint64))  # assembly is bit-identical to the reference's methods
     assert ret == int(g["ref_ret"]) == p.neq + p.nineq and ok
     assert _full_residual(p, g["ref_Dx"], g["ref_Dd_inv"], dx, dyc, dyd) <= 1e-9
 
@@ -74,7 +74,7 @@ def test_mds_against_oracle(ctx, nxs, nxd, neq, nineq, safe):
     dxo, dyco, dydo = ko.mds_solve_compressed(p, f, Hxs, p.rx, p.ryc, p.ryd)
     M, ret, ok, dx, dyc, dyd = _device_run(ctx, p, safe)
     iu = np.triu_indices(nxd + neq + nineq)
-    np.testing.assert_array_equal(M[iu], Mo[iu])
+    np.testing.assert_array_equal(M[iu].view(np.uint64), Mo[iu].view(np.uint64))
     assert ret == reto == neq + nineq and ok
     for a, b in ((dx, dxo), (dyc, dyco), (dyd, dydo)):
         if b.size:

@@ -167,7 +167,21 @@ def test_dense_newton_kkt_matrix_matches_reference(form, nx, neq, nineq, dw, dc)
     deltas = (p.delta_wx, p.delta_wd, p.delta_cc, p.delta_cd)
     M_r = ref.densekkt_build(form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas)
     M, _, _ = ko.dense_build_kkt_matrix(form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas)
-    np.testing.assert_array_equal(M, M_r)          # same additions in the same order: bit-identical, lower triangle zero
+    np.testing.assert_array_equal(_u64(M), _u64(M_r))          # same additions in the same order: bit-identical, lower triangle zero
+
+
+@pytest.mark.parametrize("form", [0, 1])
+def test_dense_newton_kkt_matrix_negative_zeros_match_reference(form):
+    """-0.0 entries of H, Jc and Jd become +0.0 in the reference's Msys (`+=` into a zeroed matrix)"""
+    from oracle import mds_model as mm
+    p = mm.with_negative_zeros(synth.make_mds_problem(0, 25, 10, 4, seed=8, dwx=1e-4, dcc=1e-8), seed=9)
+    it = dict(zl=p.zl, sxl=p.sxl, zu=p.zu, sxu=p.sxu, vl=p.vl, sdl=p.sdl, vu=p.vu, sdu=p.sdu)
+    pat = dict(ixl=p.ixl, ixu=p.ixu, idl=p.idl, idu=p.idu)
+    deltas = (p.delta_wx, p.delta_wd, p.delta_cc, p.delta_cd)
+    M_r = ref.densekkt_build(form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas)
+    M, _, _ = ko.dense_build_kkt_matrix(form, p.Hd, p.Jcd, p.Jdd, it, pat, deltas)
+    np.testing.assert_array_equal(_u64(M), _u64(M_r))
+    assert np.signbit(p.Jcd).any() and not np.signbit(M_r[M_r == 0.0]).any()
 
 
 @pytest.mark.parametrize("n,m", [(800, 14), (300, 1), (500, 40)])
@@ -372,10 +386,13 @@ def test_mds_assembly_ops_match_reference():
     assert np.abs(Wo - Wr).max() <= 1e-13 * np.abs(Wr).max()
 
 
-def test_mds_build_kkt_matrix_matches_reference_methods():
-    """ko.mds_build_kkt_matrix against the reference's own matrix methods called in the order of
-    hiopKKTLinSysCompressedMDSXYcYd::build_kkt_matrix (src/Optimization/hiopKKTLinSysMDS.cpp:196-290)."""
-    p = synth.make_mds_problem(60, 25, 9, 14, dwx=1e-4, dcc=1e-6)
+def _u64(a):
+    return np.ascontiguousarray(a, dtype=np.float64).view(np.uint64)
+
+
+def _mds_build_with_reference_methods(p):
+    """(ko's M, the reference's W, Dx, Hxs, Dd_inv): W from the reference's own matrix methods called in the order of
+    hiopKKTLinSysCompressedMDSXYcYd::build_kkt_matrix (src/Optimization/hiopKKTLinSysMDS.cpp:196-290) on a zeroed matrix."""
     M, Dx, Hxs, Dd_inv = ko.mds_build_kkt_matrix(p)
     L, dp, ip = ref.lib(), ref.dp, ref.ip
     N = p.nxd + p.neq + p.nineq
@@ -406,7 +423,44 @@ def test_mds_build_kkt_matrix_matches_reference_methods():
     L.ref_sp_add_MDinvNtrans(p.neq, p.nxs, ic.size, pic, pjc, pvc, p.nineq, idd.size, pid, pjd, pvd, p.nxd, p.nxd + p.neq, -1.0, phx, N, wp)
     a, pa = D(Dd_inv); L.ref_mat_add_sub_diagonal(N, wp, p.nxd + p.neq, -1.0, p.nineq, pa)
     a, pa = D(p.delta_cd); L.ref_mat_add_sub_diagonal(N, wp, p.nxd + p.neq, -1.0, p.nineq, pa)
-    np.testing.assert_array_equal(M, W)
+    return M, W, Dx, Hxs, Dd_inv
+
+
+def test_mds_negative_zero_inputs_match_reference_methods():
+    """-0.0 in Hd, Jcd, Jdd and the sparse values, empty sparse rows and pairs of rows that share no column: the reference's `+=` into
+    a zeroed Msys stores +0.0 for all of them, and ko.mds_build_kkt_matrix must have the same bits."""
+    from oracle import mds_model as mm
+    p = mm.with_negative_zeros(synth.make_mds_problem(60, 25, 9, 14, dwx=1e-4, dcc=1e-6), seed=3)
+    r = np.random.default_rng(4)
+    cols = lambda i: [] if i % 3 == 0 else r.choice(60, 3, replace=False)
+    mm.with_pattern(p, [cols(i) for i in range(9)], [cols(i + 1) for i in range(14)], seed=5)
+    p.Jcs_vals[::4] = -0.0
+    M, W, *_ = _mds_build_with_reference_methods(p)
+    np.testing.assert_array_equal(_u64(M), _u64(W))
+    assert (W == 0.0).sum() > W.size // 2 and not np.signbit(W[W == 0.0]).any()
+
+
+def test_mds_sparse_mat_vecs_match_reference():
+    """ko.mds_pack / ko.mds_unpack's triplet loops against hiopMatrixSparseTriplet::timesVec / transTimesVec (beta = 1, alpha = -1)"""
+    if not ref.has_sp_times_vec():
+        pytest.skip("oracle/_ref was built before ref_sp_times_vec existed: rebuild it with `make -C oracle ref`")
+    n = 300
+    p = synth.make_mds_problem(n, 5, 20, 30, nnz_per_row=40, seed=6)
+    r = np.random.default_rng(7)
+    for iR, jC, v, m in ((p.iRow_c, p.jCol_c, p.Jcs_vals, 20), (p.iRow_d, p.jCol_d, p.Jds_vals, 30)):
+        for trans, ny, nx in ((0, m, n), (1, n, m)):
+            x, y = r.standard_normal(nx), r.standard_normal(ny)
+            y_r = ref.sp_times_vec(trans, m, n, iR, jC, v, y, -1.0, x)
+            y_m = (ko.sp_trans_times_vec if trans else ko.sp_times_vec)(iR, jC, v, y.copy(), -1.0, x)
+            np.testing.assert_array_equal(_u64(y_m), _u64(y_r))
+
+
+def test_mds_build_kkt_matrix_matches_reference_methods():
+    """ko.mds_build_kkt_matrix against the reference's own matrix methods called in the order of
+    hiopKKTLinSysCompressedMDSXYcYd::build_kkt_matrix (src/Optimization/hiopKKTLinSysMDS.cpp:196-290)."""
+    p = synth.make_mds_problem(60, 25, 9, 14, dwx=1e-4, dcc=1e-6)
+    M, W, Dx, Hxs, Dd_inv = _mds_build_with_reference_methods(p)
+    np.testing.assert_array_equal(_u64(M), _u64(W))
     # and the whole system is a valid KKT system: inertia (nxd, 0, neq+nineq) for the dense block
     ret_r, _, _, _ = ref.symdense_factor_solve(W)
     ret, f = ko.mds_factorize_with_curv_check(M, Hxs)
