@@ -125,6 +125,14 @@ def lib() -> ctypes.CDLL:
     f("hb_debug_diag128_profile", c_i, c_vp, c_i, P(c_ll))
     f("hb_debug_bk_profile", c_i, c_vp, c_i, P(c_ll))
     f("hb_debug_symdense_factor", c_i, c_vp, P(c_i), P(c_i), c_vp, c_vp, c_vp, c_vp)
+    f("hb_symdense_dist_create", c_i, c_vp, c_i, P(c_vp))
+    f("hb_symdense_dist_destroy", c_i, c_vp)
+    f("hb_symdense_dist_local", c_i, c_vp, P(c_vp), P(c_ll), P(c_i))
+    f("hb_symdense_dist_order", c_i, c_vp)
+    f("hb_symdense_dist_matrix_changed", c_i, c_vp, c_i)
+    f("hb_symdense_dist_inertia", c_i, c_vp, P(c_i), P(c_i), P(c_i))
+    f("hb_symdense_dist_solve", c_i, c_vp, c_dp, c_i)
+    f("hb_symdense_dist_profile", c_i, c_vp, c_i, P(ctypes.c_float))
     f("hb_microbench_peak", c_i, c_vp, c_i, P(c_d))
     # lowrank
     f("hb_lowrank_create", c_i, c_vp, c_ll, c_i, c_i, c_i, P(c_vp))
@@ -171,6 +179,8 @@ def lib() -> ctypes.CDLL:
     f("hb_mds_build_kkt_matrix", c_i, c_vp, *([c_dp] * 17))
     f("hb_mds_hxs_inertia", c_i, c_vp, P(c_i), P(c_i))
     f("hb_mds_solve_compressed", c_i, c_vp, c_vp, *([c_dp] * 6))
+    f("hb_mds_build_kkt_matrix_dist", c_i, c_vp, *([c_dp] * 16), c_vp)
+    f("hb_mds_solve_compressed_dist", c_i, c_vp, c_vp, *([c_dp] * 6))
     f("hb_iajaaa_write_matrix_host", c_i, ctypes.c_char_p, c_i, c_dp, c_i, c_i, c_i)
     f("hb_iajaaa_append_vector_host", c_i, ctypes.c_char_p, c_i, c_dp)
     f("hb_iajaaa_write_matrix", c_i, c_vp, ctypes.c_char_p, c_i, c_dp, c_i, c_i, c_i)

@@ -262,6 +262,7 @@ typedef int (*fn_get_uid)(ncclUniqueId_t*);
 typedef int (*fn_comm_init)(void**, int, ncclUniqueId_t, int);
 typedef int (*fn_comm_destroy)(void*);
 typedef int (*fn_allreduce)(const void*, void*, size_t, int, int, void*, cudaStream_t);
+typedef int (*fn_broadcast)(const void*, void*, size_t, int, int, void*, cudaStream_t);
 typedef const char* (*fn_errstr)(int);
 struct NcclApi
 {
@@ -270,6 +271,7 @@ struct NcclApi
   fn_comm_init comm_init = nullptr;
   fn_comm_destroy comm_destroy = nullptr;
   fn_allreduce allreduce = nullptr;
+  fn_broadcast broadcast = nullptr; // only the distributed dense factorization needs it (hb_symdense_dist.cu)
   fn_errstr errstr = nullptr;
   bool tried = false;
 } g_nccl;
@@ -291,6 +293,7 @@ int nccl_load()
   g_nccl.comm_init = (fn_comm_init)dlsym(h, "ncclCommInitRank");
   g_nccl.comm_destroy = (fn_comm_destroy)dlsym(h, "ncclCommDestroy");
   g_nccl.allreduce = (fn_allreduce)dlsym(h, "ncclAllReduce");
+  g_nccl.broadcast = (fn_broadcast)dlsym(h, "ncclBroadcast");
   g_nccl.errstr = (fn_errstr)dlsym(h, "ncclGetErrorString");
   if(!g_nccl.get_uid || !g_nccl.comm_init || !g_nccl.allreduce) return hb_fail(HB_ERR_COMM, "NCCL symbols missing%s", "");
   g_nccl.h = h;
@@ -350,5 +353,22 @@ int hb_allreduce_op(hb_ctx* c, double* buf, long long count, hb_op op)
   if(!c->nccl_comm) return hb_fail(HB_ERR_COMM, "communicator not initialised%s", "");
   int rc = g_nccl.allreduce(buf, buf, (size_t)count, 8, op, c->nccl_comm, c->stream);
   if(rc != 0) return hb_fail(HB_ERR_COMM, "ncclAllReduce failed: %s", g_nccl.errstr ? g_nccl.errstr(rc) : "?");
+  return HB_OK;
+}
+
+int hb_broadcast_ready(hb_ctx* c)
+{
+  if(c->nranks == 1) return HB_OK;
+  if(!c->nccl_comm) return hb_fail(HB_ERR_COMM, "communicator not initialised%s", "");
+  if(!g_nccl.broadcast) return hb_fail(HB_ERR_COMM, "the loaded NCCL library has no ncclBroadcast%s", "");
+  return HB_OK;
+}
+
+int hb_broadcast(hb_ctx* c, double* buf, long long count, int root, cudaStream_t st)
+{
+  if(c->nranks == 1 || count == 0) return HB_OK;
+  HB_CHECK(hb_broadcast_ready(c));
+  int rc = g_nccl.broadcast(buf, buf, (size_t)count, 8, root, c->nccl_comm, st); // in place; ncclFloat64 = 8
+  if(rc != 0) return hb_fail(HB_ERR_COMM, "ncclBroadcast failed: %s", g_nccl.errstr ? g_nccl.errstr(rc) : "?");
   return HB_OK;
 }

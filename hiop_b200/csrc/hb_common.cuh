@@ -204,6 +204,10 @@ enum hb_op { HB_SUM = 0, HB_MAX = 2, HB_MIN = 3 };
 
 // in-place all-reduce of `count` doubles over the context's ranks, on the context stream (nothing to do on one rank)
 int hb_allreduce_op(hb_ctx* c, double* buf, long long count, hb_op op);
+// in-place broadcast of `count` doubles from rank `root` over the context's ranks on stream st (nothing to do on one rank).
+// hb_broadcast_ready: HB_OK when it can run (one rank, or a communicator and an NCCL with ncclBroadcast), HB_ERR_COMM otherwise
+int hb_broadcast_ready(hb_ctx* c);
+int hb_broadcast(hb_ctx* c, double* buf, long long count, int root, cudaStream_t st);
 
 // Second stage of the per-CTA reductions: out[q] = ops[q] over partial[b * slots + q], b < nblocks, slots = ops.size() <= 8. Fixed
 // order: warp q owns slot q, lane l combines b = l, l + 32, ... in turn, then the warp combines its lanes with an xor tree.

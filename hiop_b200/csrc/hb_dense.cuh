@@ -118,6 +118,11 @@ int hb_big_init(hb_ctx* c, hb_big* b);
 int hb_big_reserve(hb_ctx* c, hb_big* b, int N, bool need_w);
 // pairs: factor the 128-column blocks in pairs (K = 256 trailing updates)
 int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ldl, bool pairs, int* info_dev);
+// the per-block pieces of hb_big_factor, for the distributed factorization (hb_symdense_dist.cu): one panel step (k_diag128 +
+// k_trsm_panel) and the K = 128 trailing update on a block-cyclic matrix
+int hb_big_panel(int N, double* A, long long lda, int k0, bool ldl, double* inv16, double* dinv, double* W, long long ldw, int* info_dev, cudaStream_t st);
+int hb_big_update_cyclic(int N, const double* P, long long ldp, const double* Q, long long ldq, int qsub, double* C, long long ldc, int nranks, int rank,
+                         int q0, int nq, cudaStream_t st);
 int hb_big_diag_profile(hb_ctx* c, hb_big* b, int N, double* A, long long lda, int k0, bool ldl, long long* prof_host8);
 int hb_big_trailing_from_state(hb_ctx* c, int N, double* A, long long lda, const double* W, long long ldw, const int* state_dev, int r0_min, cudaStream_t st);
 int hb_big_block_inverses(hb_ctx* c, hb_big* b, int N, const double* F, long long ldf, bool unit);

@@ -32,7 +32,9 @@ constexpr int TM = 128;  // tile rows (i)
 constexpr int PLD = TM + 4;
 constexpr int CLD = TM + 2;
 
-enum { EPI_SUB = 0, EPI_STORE = 1, EPI_STORE_LDL = 2 };
+// EPI_SUB_CYC: EPI_SUB on a block-cyclic C (the distributed factorization, hb_symdense_dist.cu): blockIdx.z picks the local block
+// q = cyc_q0 + z of global block k = q * cyc_p + cyc_r, whose 128 columns C + q * 128 * ldc holds; its tiles start at (k*128, k*128)
+enum { EPI_SUB = 0, EPI_STORE = 1, EPI_STORE_LDL = 2, EPI_SUB_CYC = 3 };
 
 struct GemmArgs
 {
@@ -50,6 +52,7 @@ struct GemmArgs
   long long ldw2;
   const double* dinv; // EPI_STORE_LDL: C = acc * dinv[j - j_base]
   const int* state;   // pivoted panels: k0 = state[0], kb = state[1] read on the device (Q = C + k0*ldc, origin k0 + kb)
+  int cyc_p, cyc_r, cyc_q0; // EPI_SUB_CYC
 };
 
 template <int TN>
@@ -80,10 +83,19 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
     i_base = j_base = jmin & ~1; // tile origins stay even (16-byte accesses); the column below the origin is masked out
     Q = g.C + (size_t)k0 * g.ldc;
   }
-  const int i0 = i_base + TM * blockIdx.x;
-  const int j0 = j_base + TN * (g.tj0 + blockIdx.y);
+  constexpr bool SUB = EPI == EPI_SUB || EPI == EPI_SUB_CYC;
+  double* C = g.C;
+  int i0 = i_base + TM * blockIdx.x;
+  int j0 = j_base + TN * (g.tj0 + blockIdx.y);
+  if(EPI == EPI_SUB_CYC) {
+    const int q = g.cyc_q0 + blockIdx.z, k0 = (q * g.cyc_p + g.cyc_r) * BB;
+    C = g.C + (ptrdiff_t)(q * BB - k0) * g.ldc;
+    i0 = k0 + TM * blockIdx.x;
+    j0 = k0 + TN * blockIdx.y;
+    jmin = k0;
+  }
   if(i0 >= g.i_end || j0 >= g.j_end) return;
-  if(EPI == EPI_SUB && i0 + TM - 1 < j0) return; // tile entirely above the diagonal
+  if(SUB && i0 + TM - 1 < j0) return; // tile entirely above the diagonal
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp & 3, wn = warp >> 2;
@@ -118,13 +130,13 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
 #pragma unroll
     for(int b = 0; b < NJ; b++) acc[a][b][0] = acc[a][b][1] = 0.0;
 
-  if(EPI == EPI_SUB) {
+  if(SUB) {
     // the read-modify-write epilogue stalled on HBM latency (24% of the stall samples): pull the C tile into L2 now, the reads then
     // overlap the MMA loop and the epilogue loads hit L2. One 128-byte line per request: TN columns x (TM*8/128) lines.
     for(int e = tid; e < TN * (TM * 8 / 128); e += 256) {
       const int jl = e / (TM * 8 / 128), seg = e % (TM * 8 / 128);
       const int gj = j0 + jl, gi = i0 + seg * 16;
-      if(gj < g.j_end && gi < g.i_end && gi + 15 >= gj) hb_prefetch_l2(&LC(g.C, g.ldc, gi, gj));
+      if(gj < g.j_end && gi < g.i_end && gi + 15 >= gj) hb_prefetch_l2(&LC(C, g.ldc, gi, gj));
     }
   }
 
@@ -172,7 +184,7 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
 #pragma unroll 1
   for(int b0 = 0; b0 < ITEMS; b0 += BATCH) {
     double2 cur[BATCH];
-    if(EPI == EPI_SUB) {
+    if(SUB) {
 #pragma unroll
       for(int s = 0; s < BATCH; s++) {
         const int e = tid + (b0 + s) * 256;
@@ -180,10 +192,10 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
         const int gi = i0 + il, gj = j0 + jl;
         cur[s] = make_double2(0.0, 0.0);
         if(gj < g.j_end && gj >= jmin && gi + 1 >= gj && gi < g.i_end) {
-          if(gi >= gj && gi + 1 < g.i_end) cur[s] = *reinterpret_cast<const double2*>(&LC(g.C, g.ldc, gi, gj));
+          if(gi >= gj && gi + 1 < g.i_end) cur[s] = *reinterpret_cast<const double2*>(&LC(C, g.ldc, gi, gj));
           else {
-            if(gi >= gj) cur[s].x = LC(g.C, g.ldc, gi, gj);
-            if(gi + 1 < g.i_end) cur[s].y = LC(g.C, g.ldc, gi + 1, gj);
+            if(gi >= gj) cur[s].x = LC(C, g.ldc, gi, gj);
+            if(gi + 1 < g.i_end) cur[s].y = LC(C, g.ldc, gi + 1, gj);
           }
         }
       }
@@ -195,12 +207,12 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
       const int gi = i0 + il, gj = j0 + jl;
       if(gj >= g.j_end || gj < jmin || gi >= g.i_end) continue;
       const double2 v = *reinterpret_cast<const double2*>(&sC[jl * CLD + il]);
-      if(EPI == EPI_SUB) {
+      if(SUB) {
         if(gi + 1 < gj) continue;
-        if(gi >= gj && gi + 1 < g.i_end) *reinterpret_cast<double2*>(&LC(g.C, g.ldc, gi, gj)) = make_double2(cur[s].x - v.x, cur[s].y - v.y);
+        if(gi >= gj && gi + 1 < g.i_end) *reinterpret_cast<double2*>(&LC(C, g.ldc, gi, gj)) = make_double2(cur[s].x - v.x, cur[s].y - v.y);
         else {
-          if(gi >= gj) LC(g.C, g.ldc, gi, gj) = cur[s].x - v.x;
-          if(gi + 1 < g.i_end) LC(g.C, g.ldc, gi + 1, gj) = cur[s].y - v.y;
+          if(gi >= gj) LC(C, g.ldc, gi, gj) = cur[s].x - v.x;
+          if(gi + 1 < g.i_end) LC(C, g.ldc, gi + 1, gj) = cur[s].y - v.y;
         }
       } else {
         const bool two = gi + 1 < g.i_end;
@@ -212,8 +224,8 @@ __global__ void __launch_bounds__(256, (TN == 64 ? 2 : 1)) k_gemm_pq(const GemmA
           const double r = g.dinv[c];
           o.x *= r; o.y *= r;
         }
-        if(two) *reinterpret_cast<double2*>(&LC(g.C, g.ldc, gi, gj)) = o;
-        else LC(g.C, g.ldc, gi, gj) = o.x;
+        if(two) *reinterpret_cast<double2*>(&LC(C, g.ldc, gi, gj)) = o;
+        else LC(C, g.ldc, gi, gj) = o.x;
       }
     }
   }
@@ -529,7 +541,7 @@ k_trsm_panel(double* __restrict__ A, long long lda, int N, int k0, const double*
   for(int e = tid; e < BB * XROWS / 2; e += 256) {
     const int c = e / (XROWS / 2), r = (e % (XROWS / 2)) * 2;
     const bool v = i0 + r < N;
-    hb_cp_async16(&S.X[c * XS + r], v ? &LC(A, lda, i0 + r, k0 + c) : A, v ? 16 : 0);
+    hb_cp_async16(&S.X[c * XS + r], v ? &LC(A, lda, i0 + r, k0 + c) : &LC(A, lda, k0, k0), v ? 16 : 0); // (a valid address either way)
   }
   for(int e = tid; e < 8 * 16 * 17; e += 256) S.Inv16[e] = inv16G[e];
   hb_cp_async_commit();
@@ -844,6 +856,7 @@ __global__ void k_scatter(int N, const int* __restrict__ perm, const double* __r
 int hb_big_init_attrs(hb_ctx* c)
 {
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<64, EPI_SUB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<64>::SMEM));
+  HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<64, EPI_SUB_CYC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<64>::SMEM));
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<128, EPI_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<128>::SMEM));
   HB_CUDA(cudaFuncSetAttribute(k_gemm_pq<128, EPI_STORE_LDL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GemmCfg<128>::SMEM));
   HB_CUDA(cudaFuncSetAttribute(k_diag128<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DiagSmem)));
@@ -912,17 +925,7 @@ int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ld
   const int nblk = (N + BB - 1) / BB;
   double* inv16 = b->dinv + BB;
   auto panel = [&](int blk, double* Wb) -> int { // diagonal block + panel solve of block blk on the panel stream
-    const int k0 = blk * BB, nb = N - k0 < BB ? N - k0 : BB, r0 = k0 + nb;
-    if(ldl) k_diag128<true><<<1, DTHREADS, sizeof(DiagSmem), sp>>>(A, lda, N, k0, inv16, b->dinv, info_dev, nullptr);
-    else k_diag128<false><<<1, DTHREADS, sizeof(DiagSmem), sp>>>(A, lda, N, k0, inv16, b->dinv, info_dev, nullptr);
-    HB_LAUNCHED();
-    if(r0 < N) { // nb == 128 here (only the last block can be partial)
-      const int ntile = (N - r0 + XROWS - 1) / XROWS;
-      if(ldl) k_trsm_panel<true><<<ntile, 256, sizeof(TrsmSmem), sp>>>(A, lda, N, k0, inv16, b->dinv, Wb, ldw);
-      else k_trsm_panel<false><<<ntile, 256, sizeof(TrsmSmem), sp>>>(A, lda, N, k0, inv16, b->dinv, nullptr, 0);
-      HB_LAUNCHED();
-    }
-    return HB_OK;
+    return hb_big_panel(N, A, lda, blk * BB, ldl, inv16, b->dinv, Wb, ldw, info_dev, sp);
   };
   auto update = [&](cudaStream_t st, const double* P, long long ldp, int kq0, int kb, int r0, int tj0, int ntj) -> int {
     // A(i,j) -= sum_p P[p][i] * L(j, kq0 + p) on the lower triangle from row/column r0 on, column tiles [tj0, tj0 + ntj) of 64
@@ -975,6 +978,45 @@ int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ld
   k_block_inverses<<<nblk, DTHREADS, sizeof(DiagSmem), su>>>(A, lda, N, ldl ? 1 : 0, b->InvAll);
   HB_LAUNCHED();
   b->inv_valid = true;
+  return HB_OK;
+}
+
+// One block step of the factorization on the caller's operands: k_diag128 on the diagonal block at (k0, k0), then k_trsm_panel on the
+// rows below it. LC(A, lda, i, j) must address element (i, j) for the columns of this block (global indices); nothing else of A is
+// touched. inv16: 8 * 16 * 17 doubles of scratch; dinv: receives 1/d of the block (LDL^T); W: LDL^T only, W[c * ldw + i] = the row i >= k0 + 128
+// of column c of W = L D (absolute i).
+int hb_big_panel(int N, double* A, long long lda, int k0, bool ldl, double* inv16, double* dinv, double* W, long long ldw, int* info_dev, cudaStream_t st)
+{
+  const int nb = N - k0 < BB ? N - k0 : BB, r0 = k0 + nb;
+  if(ldl) k_diag128<true><<<1, DTHREADS, sizeof(DiagSmem), st>>>(A, lda, N, k0, inv16, dinv, info_dev, nullptr);
+  else k_diag128<false><<<1, DTHREADS, sizeof(DiagSmem), st>>>(A, lda, N, k0, inv16, dinv, info_dev, nullptr);
+  HB_LAUNCHED();
+  if(r0 < N) { // nb == 128 here (only the last block can be partial)
+    const int ntile = (N - r0 + XROWS - 1) / XROWS;
+    if(ldl) k_trsm_panel<true><<<ntile, 256, sizeof(TrsmSmem), st>>>(A, lda, N, k0, inv16, dinv, W, ldw);
+    else k_trsm_panel<false><<<ntile, 256, sizeof(TrsmSmem), st>>>(A, lda, N, k0, inv16, dinv, nullptr, 0);
+    HB_LAUNCHED();
+  }
+  return HB_OK;
+}
+
+// The trailing update of hb_big_factor (K = 128, 128 x 64 tiles of the lower triangle) on a block-cyclic matrix: C holds the 128-column
+// blocks k = q * nranks + rank (local block q at C + q * 128 * ldc); the local blocks q0 .. q0 + nq - 1 receive
+// C(i, j) -= sum_p P[p * ldp + i] Q[p * ldq + j - qsub], i >= j. Every entry sees the same operands in the same order as in hb_big_factor.
+int hb_big_update_cyclic(int N, const double* P, long long ldp, const double* Q, long long ldq, int qsub, double* C, long long ldc, int nranks, int rank,
+                         int q0, int nq, cudaStream_t st)
+{
+  if(nq <= 0) return HB_OK;
+  GemmArgs g{};
+  g.P = P; g.ldp = ldp;
+  g.Q = Q; g.ldq = ldq; g.qsub = qsub;
+  g.kb = BB;
+  g.C = C; g.ldc = ldc;
+  g.i_end = N; g.j_end = N;
+  g.cyc_p = nranks; g.cyc_r = rank; g.cyc_q0 = q0;
+  const int nti = (N - (q0 * nranks + rank) * BB + TM - 1) / TM; // rows of the first (largest) block column
+  k_gemm_pq<64, EPI_SUB_CYC><<<dim3(nti, BB / 64, nq), 256, GemmCfg<64>::SMEM, st>>>(g);
+  HB_LAUNCHED();
   return HB_OK;
 }
 

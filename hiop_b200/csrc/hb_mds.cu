@@ -69,53 +69,77 @@ __global__ void k_mds_ddinv(int mi, const double* __restrict__ dwd, const double
 //                            then  - delta_cc  |  - Dd_inv - delta_cd  on the diagonal                         :245,289-290
 // The explicit 0 + is not a no-op: it turns -0.0 into +0.0, as the reference's `W += alpha*x` does. Without it a pair of sparse
 // rows that shares no column (acc = 0, -1 * acc = -0.0) and every -0.0 entry of Hd / Jcd / Jdd would keep the wrong sign bit.
-__global__ void __launch_bounds__(T)
-k_mds_build(int nxs, int nxd, int neq, int nineq, const double* __restrict__ Hd, const double* __restrict__ Jcd, const double* __restrict__ Jdd,
-            const double* __restrict__ Dx, const double* __restrict__ dwx, const int* __restrict__ ptr, const int* __restrict__ col,
-            const double* __restrict__ vals, const double* __restrict__ Hxs, const double* __restrict__ dcc, const double* __restrict__ Dd_inv,
-            const double* __restrict__ dcd, double* __restrict__ M)
+struct MdsBuildArgs
 {
-  const int N = nxd + neq + nineq;
+  int nxs, nxd, neq, nineq;
+  const double *Hd, *Jcd, *Jdd, *Dx, *dwx;
+  const int *ptr, *col;
+  const double *vals, *Hxs, *dcc, *Dd_inv, *dcd;
+};
+
+__device__ __forceinline__ double mds_entry(const MdsBuildArgs& a, int r, int c)
+{
+  const int nxd = a.nxd, neq = a.neq;
+  double v;
+  if(r < nxd) {
+    if(c < nxd) {
+      v = __dadd_rn(0.0, a.Hd[(size_t)r * nxd + c]);
+      if(r == c) {
+        v = __dadd_rn(v, a.Dx[a.nxs + r]);
+        v = __dadd_rn(v, a.dwx[a.nxs + r]);
+      }
+    } else if(c < nxd + neq) {
+      v = __dadd_rn(0.0, a.Jcd[(size_t)(c - nxd) * nxd + r]);
+    } else {
+      v = __dadd_rn(0.0, a.Jdd[(size_t)(c - nxd - neq) * nxd + r]);
+    }
+  } else {
+    const int i = r - nxd, j = c - nxd;
+    int ki = a.ptr[i], kj = a.ptr[j];
+    const int ei = a.ptr[i + 1], ej = a.ptr[j + 1];
+    double acc = 0.0;
+    while(ki < ei && kj < ej) {
+      const int ci = a.col[ki], cj = a.col[kj];
+      if(ci == cj) {
+        acc = __dadd_rn(acc, __dmul_rn(__ddiv_rn(a.vals[ki], a.Hxs[ci]), a.vals[kj]));
+        ki++; kj++;
+      } else if(ci < cj) ki++;
+      else kj++;
+    }
+    v = __dadd_rn(0.0, __dmul_rn(-1.0, acc));
+    if(i == j) {
+      if(i < neq) v = __dsub_rn(v, a.dcc[i]);
+      else {
+        v = __dsub_rn(v, a.Dd_inv[i - neq]);
+        v = __dsub_rn(v, a.dcd[i - neq]);
+      }
+    }
+  }
+  return v;
+}
+
+__global__ void __launch_bounds__(T) k_mds_build(const MdsBuildArgs a, double* __restrict__ M)
+{
+  const int N = a.nxd + a.neq + a.nineq;
   const long long total = (long long)N * N;
   for(long long e = (long long)blockIdx.x * T + threadIdx.x; e < total; e += (long long)gridDim.x * T) {
     const int r = (int)(e / N), c = (int)(e % N);
     if(c < r) continue;
-    double v;
-    if(r < nxd) {
-      if(c < nxd) {
-        v = __dadd_rn(0.0, Hd[(size_t)r * nxd + c]);
-        if(r == c) {
-          v = __dadd_rn(v, Dx[nxs + r]);
-          v = __dadd_rn(v, dwx[nxs + r]);
-        }
-      } else if(c < nxd + neq) {
-        v = __dadd_rn(0.0, Jcd[(size_t)(c - nxd) * nxd + r]);
-      } else {
-        v = __dadd_rn(0.0, Jdd[(size_t)(c - nxd - neq) * nxd + r]);
-      }
-    } else {
-      const int i = r - nxd, j = c - nxd;
-      int ki = ptr[i], kj = ptr[j];
-      const int ei = ptr[i + 1], ej = ptr[j + 1];
-      double acc = 0.0;
-      while(ki < ei && kj < ej) {
-        const int ci = col[ki], cj = col[kj];
-        if(ci == cj) {
-          acc = __dadd_rn(acc, __dmul_rn(__ddiv_rn(vals[ki], Hxs[ci]), vals[kj]));
-          ki++; kj++;
-        } else if(ci < cj) ki++;
-        else kj++;
-      }
-      v = __dadd_rn(0.0, __dmul_rn(-1.0, acc));
-      if(i == j) {
-        if(i < neq) v = __dsub_rn(v, dcc[i]);
-        else {
-          v = __dsub_rn(v, Dd_inv[i - neq]);
-          v = __dsub_rn(v, dcd[i - neq]);
-        }
-      }
-    }
-    M[(size_t)r * N + c] = v;
+    M[(size_t)r * N + c] = mds_entry(a, r, c);
+  }
+}
+
+// the same entries for the block rows one rank owns in hb_symdense_dist's block-cyclic layout: local row e holds global row
+// (e / 128 * P + rank) * 128 + e % 128, ld doubles per row
+__global__ void __launch_bounds__(T) k_mds_build_dist(const MdsBuildArgs a, int P, int rank, int nloc, double* __restrict__ M, long long ld)
+{
+  const int N = a.nxd + a.neq + a.nineq;
+  const long long total = (long long)nloc * 128 * N;
+  for(long long e = (long long)blockIdx.x * T + threadIdx.x; e < total; e += (long long)gridDim.x * T) {
+    const int lr = (int)(e / N), c = (int)(e % N);
+    const int r = (lr / 128 * P + rank) * 128 + lr % 128;
+    if(r >= N || c < r) continue;
+    M[(size_t)lr * ld + c] = mds_entry(a, r, c);
   }
 }
 
@@ -254,18 +278,17 @@ extern "C" int hb_mds_update(hb_mds* h, const double* zl, const double* sxl, con
   return HB_OK;
 }
 
-extern "C" int hb_mds_build_kkt_matrix(hb_mds* h, const double* Hd, const double* Hs_diag, const double* Jcd, const double* Jdd,
-                                       const double* Jcs_vals, const double* Jds_vals, const double* vl, const double* sdl, const double* vu,
-                                       const double* sdu, const double* idl, const double* idu, const double* delta_wx, const double* delta_wd,
-                                       const double* delta_cc, const double* delta_cd, double* Msys)
+namespace {
+// everything of build_kkt_matrix before the entries: the sparse values, Hxs (+ its Haynsworth counts), Dd_inv; the arguments of the entries
+int mds_prepare(hb_mds* h, const double* Hd, const double* Hs_diag, const double* Jcd, const double* Jdd, const double* Jcs_vals, const double* Jds_vals,
+                const double* vl, const double* sdl, const double* vu, const double* sdu, const double* idl, const double* idu, const double* delta_wx,
+                const double* delta_wd, const double* delta_cc, const double* delta_cd, MdsBuildArgs* args)
 {
-  HB_REQUIRE(h && Msys, "hb_mds_build_kkt_matrix: null argument");
   HB_REQUIRE(h->have_structure && h->have_update, "hb_mds_build_kkt_matrix: call hb_mds_set_sparsity and hb_mds_update first");
   HB_REQUIRE((h->nxd == 0 || Hd) && (h->nxs == 0 || Hs_diag) && (h->nxs + h->nxd == 0 || delta_wx), "hb_mds_build_kkt_matrix: null Hessian block");
   HB_REQUIRE(h->nineq == 0 || (vl && sdl && vu && sdu && idl && idu && delta_wd && delta_cd), "hb_mds_build_kkt_matrix: null d-side block");
   HB_REQUIRE(h->neq == 0 || delta_cc, "hb_mds_build_kkt_matrix: null delta_cc");
   hb_ctx* c = h->ctx;
-  const int N = h->nxd + h->neq + h->nineq;
   if(h->nnz_c) HB_CUDA(cudaMemcpyAsync(h->vals, Jcs_vals, sizeof(double) * h->nnz_c, cudaMemcpyDeviceToDevice, c->stream));
   if(h->nnz_d) HB_CUDA(cudaMemcpyAsync(h->vals + h->nnz_c, Jds_vals, sizeof(double) * h->nnz_d, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(int) * 2, c->stream));
@@ -277,9 +300,47 @@ extern "C" int hb_mds_build_kkt_matrix(hb_mds* h, const double* Hd, const double
     k_mds_ddinv<<<hb_grid(c, h->nineq, T), T, 0, c->stream>>>(h->nineq, delta_wd, vl, sdl, vu, sdu, idl, idu, h->Dd_inv);
     HB_LAUNCHED();
   }
+  *args = MdsBuildArgs{h->nxs, h->nxd, h->neq, h->nineq, Hd, Jcd, Jdd, h->Dx, delta_wx, h->csr_ptr, h->csr_col, h->vals, h->Hxs, delta_cc, h->Dd_inv,
+                       delta_cd};
+  return HB_OK;
+}
+} // namespace
+
+extern "C" int hb_mds_build_kkt_matrix(hb_mds* h, const double* Hd, const double* Hs_diag, const double* Jcd, const double* Jdd,
+                                       const double* Jcs_vals, const double* Jds_vals, const double* vl, const double* sdl, const double* vu,
+                                       const double* sdu, const double* idl, const double* idu, const double* delta_wx, const double* delta_wd,
+                                       const double* delta_cc, const double* delta_cd, double* Msys)
+{
+  HB_REQUIRE(h && Msys, "hb_mds_build_kkt_matrix: null argument");
+  MdsBuildArgs a;
+  HB_CHECK(mds_prepare(h, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd, &a));
+  hb_ctx* c = h->ctx;
+  const int N = h->nxd + h->neq + h->nineq;
   if(N > 0) {
-    k_mds_build<<<hb_grid(c, (long long)N * N, T), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, Hd, Jcd, Jdd, h->Dx, delta_wx, h->csr_ptr,
-                                                               h->csr_col, h->vals, h->Hxs, delta_cc, h->Dd_inv, delta_cd, Msys);
+    k_mds_build<<<hb_grid(c, (long long)N * N, T), T, 0, c->stream>>>(a, Msys);
+    HB_LAUNCHED();
+  }
+  h->built = true;
+  return HB_OK;
+}
+
+extern "C" int hb_mds_build_kkt_matrix_dist(hb_mds* h, const double* Hd, const double* Hs_diag, const double* Jcd, const double* Jdd,
+                                            const double* Jcs_vals, const double* Jds_vals, const double* vl, const double* sdl, const double* vu,
+                                            const double* sdu, const double* idl, const double* idu, const double* delta_wx, const double* delta_wd,
+                                            const double* delta_cc, const double* delta_cd, hb_symdense_dist* s)
+{
+  HB_REQUIRE(h && s, "hb_mds_build_kkt_matrix_dist: null argument");
+  const int N = h->nxd + h->neq + h->nineq;
+  double* M = nullptr;
+  long long ld = 0;
+  int nloc = 0;
+  HB_CHECK(hb_symdense_dist_local(s, &M, &ld, &nloc));
+  HB_REQUIRE(hb_symdense_dist_order(s) == N, "hb_mds_build_kkt_matrix_dist: the handle's order is not nxd + neq + nineq");
+  MdsBuildArgs a;
+  HB_CHECK(mds_prepare(h, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd, &a));
+  hb_ctx* c = h->ctx;
+  if(nloc > 0) {
+    k_mds_build_dist<<<hb_grid(c, (long long)nloc * 128 * N, T), T, 0, c->stream>>>(a, c->nranks, c->rank, nloc, M, ld);
     HB_LAUNCHED();
   }
   h->built = true;
@@ -301,10 +362,11 @@ extern "C" const double* hb_mds_Dx(hb_mds* h) { return h ? h->Dx.get() : nullptr
 extern "C" const double* hb_mds_Hxs(hb_mds* h) { return h ? h->Hxs.get() : nullptr; }
 extern "C" const double* hb_mds_Dd_inv(hb_mds* h) { return h ? h->Dd_inv.get() : nullptr; }
 
-extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc,
-                                       double* dyd)
+namespace {
+// solveCompressed around a dense solve of the packed rhs (in place, h->rhs): pack, solve, unpack
+template <typename Solve>
+int mds_solve(hb_mds* h, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc, double* dyd, Solve&& solve)
 {
-  HB_REQUIRE(h && s, "hb_mds_solve_compressed: null handle");
   HB_REQUIRE(h->built, "hb_mds_solve_compressed: build + factorize the KKT matrix first");
   hb_ctx* c = h->ctx;
   const int N = h->nxd + h->neq + h->nineq;
@@ -315,7 +377,7 @@ extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* 
   if(N) {
     k_mds_pack_rhs<<<hb_grid(c, N, T), T, 0, c->stream>>>(h->nxs, h->nxd, h->neq, h->nineq, rx, ryc, ryd, h->csr_ptr, h->csr_col, h->vals, h->rxs, h->rhs);
     HB_LAUNCHED();
-    const int rc = hb_symdense_solve(s, h->rhs, 1);
+    const int rc = solve(h->rhs.get());
     if(rc != 1) return rc < 0 ? rc : hb_fail(HB_ERR_NUMERIC, "hb_mds_solve_compressed: dense solve failed%s", "");
   }
   const int total = h->nxs + h->nxd + h->neq + h->nineq;
@@ -325,6 +387,22 @@ extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* 
     HB_LAUNCHED();
   }
   return HB_OK;
+}
+} // namespace
+
+extern "C" int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc,
+                                       double* dyd)
+{
+  HB_REQUIRE(h && s, "hb_mds_solve_compressed: null handle");
+  return mds_solve(h, rx, ryc, ryd, dx, dyc, dyd, [&](double* b) { return hb_symdense_solve(s, b, 1); });
+}
+
+extern "C" int hb_mds_solve_compressed_dist(hb_mds* h, hb_symdense_dist* s, const double* rx, const double* ryc, const double* ryd, double* dx,
+                                            double* dyc, double* dyd)
+{
+  HB_REQUIRE(h && s, "hb_mds_solve_compressed_dist: null handle");
+  HB_REQUIRE(hb_symdense_dist_order(s) == h->nxd + h->neq + h->nineq, "hb_mds_solve_compressed_dist: the handle's order is not nxd + neq + nineq");
+  return mds_solve(h, rx, ryc, ryd, dx, dyc, dyd, [&](double* b) { return hb_symdense_dist_solve(s, b, 1); });
 }
 
 // =====================================================================================================================

@@ -20,7 +20,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, sharding
 from ._lib import EngineError, check
 
 RES_NAMES = ["rx", "rd", "ryc", "ryd", "rxl", "rxu", "rdl", "rdu", "rszl", "rszu", "rsvl", "rsvu"]
@@ -214,6 +214,81 @@ class LinSolverSymDense:
         if rc < 0:
             check(rc, "hb_symdense_solve_host")
         return rc == 1
+
+
+class _DeviceArray:
+    """A borrowed device buffer of the library, seen by torch.as_tensor through the CUDA array interface (no copy)."""
+
+    def __init__(self, ptr: int, shape, owner):
+        self.__cuda_array_interface__ = dict(shape=tuple(shape), typestr="<f8", data=(ptr, False), version=3, strides=None)
+        self._owner = owner
+
+
+class LinSolverSymDenseDist:
+    """The dense symmetric solver with the matrix factored across the context's ranks (hb_symdense_dist): Cholesky or no-pivot LDL^T
+    on a 1-D block-cyclic layout of 128-row blocks (sharding.block_rows). Every call is collective over the ranks; with one rank (no
+    init_comm) it runs on one GPU. matrixChanged(mode) returns what LinSolverSymDense.matrixChanged does, the same on every rank;
+    solve(x) takes and returns x replicated on every rank."""
+
+    NOPIV, CHOLESKY = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY
+
+    def __init__(self, ctx: Context, n: int):
+        self.ctx, self.n = ctx, n
+        self.h = ctypes.c_void_p()
+        check(ctx.L.hb_symdense_dist_create(ctx.h, n, ctypes.byref(self.h)), "hb_symdense_dist_create")
+        ptr, ld, nb = ctypes.c_void_p(), ctypes.c_longlong(), ctypes.c_int()
+        check(ctx.L.hb_symdense_dist_local(self.h, ctypes.byref(ptr), ctypes.byref(ld), ctypes.byref(nb)), "hb_symdense_dist_local")
+        self.ld, self.n_blocks = ld.value, nb.value
+        self.rows = sharding.block_rows(n, int(ctx.L.hb_comm_size(ctx.h)), int(ctx.L.hb_comm_rank(ctx.h)))
+        assert len(self.rows) == self.n_blocks
+        self._local = torch.as_tensor(_DeviceArray(ptr.value or 0, (self.n_blocks * sharding.DIST_BLOCK, self.ld), self), device=ctx.device) \
+            if self.n_blocks else torch.empty((0, self.ld), dtype=torch.float64, device=ctx.device)
+
+    def close(self):
+        if self.h:
+            self._local = None
+            self.ctx.L.hb_symdense_dist_destroy(self.h)
+            self.h = None
+
+    def local(self) -> torch.Tensor:
+        """(n_blocks * 128) x ld view of this rank's block rows, stacked in the order of sharding.block_rows; columns >= n are padding"""
+        return self._local
+
+    def set_matrix(self, M: torch.Tensor):
+        """Copies this rank's block rows out of a full n x n device matrix (upper triangle read), on the engine stream."""
+        assert M.shape == (self.n, self.n)
+        self.ctx.stream.wait_stream(torch.cuda.current_stream(self.ctx.device))   # M may still be written on torch's stream
+        M.record_stream(self.ctx.stream)                                          # and must outlive the copies on the engine stream
+        with torch.cuda.stream(self.ctx.stream):
+            for q, (b, e) in enumerate(self.rows):
+                r = q * sharding.DIST_BLOCK
+                self._local[r:r + e - b, :self.n].copy_(M[b:e])
+
+    def matrixChanged(self, mode: int) -> int:
+        if mode not in (self.NOPIV, self.CHOLESKY):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
+            raise EngineError("LinSolverSymDenseDist: Bunch-Kaufman is not distributed (its pivot search needs every column); use LinSolverSymDense")
+        rc = self.ctx.L.hb_symdense_dist_matrix_changed(self.h, mode)
+        if rc < -1:
+            check(rc, "hb_symdense_dist_matrix_changed")
+        return rc
+
+    def inertia(self):
+        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        check(self.ctx.L.hb_symdense_dist_inertia(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "hb_symdense_dist_inertia")
+        return a.value, b.value, c.value
+
+    def solve(self, x: torch.Tensor) -> bool:
+        nrhs = x.numel() // max(self.n, 1) if self.n else 0
+        rc = self.ctx.L.hb_symdense_dist_solve(self.h, _ptr(x), nrhs)
+        if rc < 0:
+            check(rc, "hb_symdense_dist_solve")
+        return rc == 1
+
+    def profile(self, on: bool):
+        """arm (on=True) / read (on=False -> (panel chain, broadcast, trailing update) ms of the last factorization on this rank)"""
+        ms = (ctypes.c_float * 3)()
+        check(self.ctx.L.hb_symdense_dist_profile(self.h, int(on), ms), "hb_symdense_dist_profile")
+        return None if on else tuple(float(v) for v in ms)
 
 
 class KKTLinSysLowRank:
@@ -510,6 +585,21 @@ class KKTLinSysCompressedMDSXYcYd:
         if rc == -4:
             return False
         check(rc, "hb_mds_solve_compressed")
+        return True
+
+    def build_kkt_matrix_dist(self, dist: LinSolverSymDenseDist, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx,
+                              delta_wd, delta_cc, delta_cd):
+        """build_kkt_matrix into the block rows this rank owns in `dist` (order nxd + neq + nineq); the inputs are replicated"""
+        args = (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd)
+        self._keep["blk"] = args
+        check(self.ctx.L.hb_mds_build_kkt_matrix_dist(self.h, *[_ptr(t) for t in args], dist.h), "hb_mds_build_kkt_matrix_dist")
+
+    def solveCompressed_dist(self, dist: LinSolverSymDenseDist, rx, ryc, ryd, dx, dyc, dyd) -> bool:
+        """solveCompressed around dist (factored with dist.matrixChanged); the outputs are replicated on every rank"""
+        rc = self.ctx.L.hb_mds_solve_compressed_dist(self.h, dist.h, *[_ptr(t) for t in (rx, ryc, ryd, dx, dyc, dyd)])
+        if rc == -4:
+            return False
+        check(rc, "hb_mds_solve_compressed_dist")
         return True
 
     def Msys(self) -> np.ndarray:

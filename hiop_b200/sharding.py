@@ -1,8 +1,21 @@
-"""Column (n) partition of the quasi-Newton KKT path over ranks/GPUs -- the reference's MPI layout
+"""Layouts of the multi-rank paths.
+
+Column (n) partition of the quasi-Newton KKT path over ranks/GPUs -- the reference's MPI layout
 (src/Optimization/hiopHessianLowRank.hpp:88-89, col_part in src/LinAlg/hiopVectorPar.cpp:78-87): every n-vector and the
 columns of J, S_t, Y_t are split, every m- and l-sized object is replicated, and each reduction the reference does with
 MPI_Allreduce becomes one sum all-reduce (NCCL inside libhiopb200.so, see hb_comm_init)."""
 from __future__ import annotations
+
+
+# block size of the distributed dense factorization (hb_symdense_dist.cu; = hb_big_factor's)
+DIST_BLOCK = 128
+
+
+def block_rows(N: int, world: int, rank: int) -> list[tuple[int, int]]:
+    """[begin, end) of the global rows of each block row `rank` owns in the 1-D block-cyclic layout of hb_symdense_dist, in the order
+    they are stacked in its local storage: block row k (rows k*128 .. min(N, k*128+128)) belongs to rank k mod world."""
+    nblk = (N + DIST_BLOCK - 1) // DIST_BLOCK
+    return [(k * DIST_BLOCK, min(N, (k + 1) * DIST_BLOCK)) for k in range(rank, nblk, world)]
 
 
 def column_range(n: int, world: int, rank: int) -> tuple[int, int]:

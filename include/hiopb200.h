@@ -38,6 +38,7 @@ typedef struct hb_ctx hb_ctx;
 typedef struct hb_lowrank hb_lowrank;
 typedef struct hb_symdense hb_symdense;
 typedef struct hb_mds hb_mds;
+typedef struct hb_symdense_dist hb_symdense_dist;
 
 /* ------------------------------------------------------------------------------------------------------------
  * Context, memory, streams
@@ -197,6 +198,32 @@ int hb_debug_bk_profile(hb_ctx* ctx, int on, long long* prof_host8);
  * with the upper triangle valid as M (unpadded for odd N). ipiv_host: N pivots (LAPACK's convention), Bunch-Kaufman only.
  * perm_host / dsub_host: N entries each, cluster Bunch-Kaufman only. */
 int hb_debug_symdense_factor(hb_symdense* s, int* plan4, int* bk_widths, double* F_host, int* ipiv_host, int* perm_host, double* dsub_host);
+
+/* ---- the same system factored across the ranks of the context's communicator (hb_symdense_dist.cu) ----
+ * 1-D block-cyclic layout with block size 128: block row k (rows k*128 .. min(N, k*128+128)-1 of the N x N row-major matrix, full
+ * width) belongs to rank k mod P. Cholesky and no-pivot LDL^T only (Bunch-Kaufman's pivot search needs every column: use hb_symdense).
+ * Every call is collective: all ranks make the same calls in the same order. Without hb_comm_init, P = 1 and the handle works on one GPU.
+ * The factor is bit-identical to hb_symdense's look-ahead factorization with unpaired blocks (HB_DENSE_PAIR_MIN above N), for every P.
+ * create refuses on every rank (HB_ERR_INVALID) when the ranks pass different N, and with HB_ERR_COMM when P > 1 and NCCL has no
+ * ncclBroadcast or no communicator was initialised. */
+int hb_symdense_dist_create(hb_ctx* ctx, int N, hb_symdense_dist** out);
+int hb_symdense_dist_destroy(hb_symdense_dist* s);
+/* the rank's owned block rows, stacked in order (device, row-major, ld doubles per row): local block q is global block row
+ * k = q*P + rank. The caller fills their upper-triangle part (columns >= row) before each factorization, like hb_symdense_matrix.
+ * n_blocks may be 0 (N < 128*P). Every output pointer may be NULL. */
+int hb_symdense_dist_local(hb_symdense_dist* s, double** A_local, long long* ld, int* n_blocks);
+/* the order N of the handle (-1 for NULL) */
+int hb_symdense_dist_order(hb_symdense_dist* s);
+/* factorizes in place; the same return value on every rank, with the meaning of hb_symdense_matrix_changed (>= 0: number of negative
+ * eigenvalues, -1: null pivot or breakdown). HB_ERR_INVALID for HB_FACT_BUNCH_KAUFMAN (the handle stays usable). */
+int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode);
+int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_null, int* n_pos);
+/* x: N x nrhs (one rhs after the other, device), replicated on every rank in and out. 1 / 0 / HB_ERR_* like hb_symdense_solve. */
+int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs);
+/* diagnostics (tools/bench_dist_symdense.py): on != 0 times the phases of every following factorization with device events; on == 0
+ * stops and returns this rank's sums (ms) over the steps of the last one: panel chain (owner's k_diag128 + k_trsm_panel + packing),
+ * broadcast (including the wait for the owner), trailing update on the update stream. ms3 may be NULL. */
+int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3);
 
 /* ------------------------------------------------------------------------------------------------------------
  * hiopKKTLinSysLowRank + hiopHessianLowRank (B2; src/Optimization/hiopKKTLinSys.cpp:1031-1350,
@@ -387,7 +414,8 @@ int hb_lowrank_kkt_system_host(hb_lowrank* k, const double* Jc_host, const doubl
  * hiopKKTLinSysCompressedMDSXYcYd (src/Optimization/hiopKKTLinSysMDS.cpp:59-484): mixed dense-sparse Newton KKT.
  * x = (x_s, x_d) with nxs "sparse" and nxd "dense" variables; the Hessian is diag(H_s) (+) H_d, the Jacobians are
  * [J_s | J_d] with J_s sparse triplets (row-sorted) and J_d dense row-major. The condensed system has size
- * N = nxd + neq + nineq and is handed to an hb_symdense solver. Stays on one GPU.
+ * N = nxd + neq + nineq and is handed to an hb_symdense solver (one GPU) or to an hb_symdense_dist solver (the condensed matrix
+ * sharded over the ranks; the sparse block stays replicated).
  * ------------------------------------------------------------------------------------------------------------ */
 int hb_mds_create(hb_ctx* ctx, int nxs, int nxd, int neq, int nineq, hb_mds** out);
 int hb_mds_destroy(hb_mds* h);
@@ -413,6 +441,15 @@ int hb_mds_hxs_inertia(hb_mds* h, int* n_neg, int* n_zero);
 /* solveCompressed() (:307-403) around s (already factorized with hb_symdense_matrix_changed). rx has nxs+nxd entries. */
 int hb_mds_solve_compressed(hb_mds* h, hb_symdense* s, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc,
                             double* dyd);
+/* the same two steps on a distributed handle (hb_symdense_dist, order nxd + neq + nineq). The MDS inputs are replicated on every rank;
+ * build writes only the rank's owned block rows, each entry bit-identical to hb_mds_build_kkt_matrix's; the outputs of the solve are
+ * replicated. hb_mds_hxs_inertia is unchanged (the same on every rank). */
+int hb_mds_build_kkt_matrix_dist(hb_mds* h, const double* Hd, const double* Hs_diag, const double* Jcd, const double* Jdd,
+                                 const double* Jcs_vals, const double* Jds_vals, const double* vl, const double* sdl, const double* vu,
+                                 const double* sdu, const double* idl, const double* idu, const double* delta_wx, const double* delta_wd,
+                                 const double* delta_cc, const double* delta_cd, hb_symdense_dist* s);
+int hb_mds_solve_compressed_dist(hb_mds* h, hb_symdense_dist* s, const double* rx, const double* ryc, const double* ryd, double* dx, double* dyc,
+                                 double* dyd);
 /* ---- dense-Newton KKT classes hiopKKTLinSysDenseXYcYd (form 0) / hiopKKTLinSysDenseXDYcYd (form 1) ----
  * build_kkt_matrix (src/Optimization/hiopKKTLinSysDense.hpp:85-172, 249-330): fills Msys (N x N row-major, upper triangle;
  * N = nx+neq+nineq, resp. nx+2*nineq+neq) with [H+Dx+dwx, Jc^T, Jd^T; 0; -Dd^{-1}] resp. [H+Dx+dwx, 0, Jc^T, Jd^T; Dd+dwd, 0, -I;
