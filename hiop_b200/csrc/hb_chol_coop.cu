@@ -471,7 +471,7 @@ k_spd_solve_coop(const double* __restrict__ F, int ldf, int N, const double* __r
       acc = hb_warp_sum(acc);
       const double ri = rhs[i] - acc;
       if(lane == 0) r[i] = ri;
-      wmax = fmax(wmax, fabs(ri));
+      wmax = hb_nan_max(wmax, fabs(ri));
     }
     if(lane == 0) {
       const double m = wmax == wmax ? wmax : __longlong_as_double(0x7ff0000000000000LL); // NaN -> +inf so that it wins the max
@@ -479,7 +479,7 @@ k_spd_solve_coop(const double* __restrict__ F, int ldf, int N, const double* __r
     }
     grid.sync();
     nrm = __longlong_as_double((long long)*slot);
-    if(!(nrm >= tol) || nrm > 1.7e308 || nref >= max_refine) break;
+    if(isinf(nrm) || !(nrm >= tol) || nref >= max_refine) break; // a residual that is not finite stops the loop (reported as NaN)
     if(gtid == 0) nrm_bits[(nref + 1) & 1] = 0ull; // the other slot is idle until the next round's barrier
     for(int i = gtid; i < N; i += gthreads) v[i] = __ldcg(r + i) * s[i];
     grid.sync();
@@ -490,7 +490,7 @@ k_spd_solve_coop(const double* __restrict__ F, int ldf, int N, const double* __r
   }
   if(gtid == 0) {
     stats[0] = (double)nref;
-    stats[1] = nrm > 1.7e308 ? __longlong_as_double(0x7ff8000000000000LL) : nrm;
+    stats[1] = isinf(nrm) ? __longlong_as_double(0x7ff8000000000000LL) : nrm;
   }
 }
 

@@ -319,6 +319,11 @@ __device__ __forceinline__ double hb_warp_max(double v)
   for(int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// max(a, b) that keeps a NaN of either operand (fmax returns the other one); the same bits as fmax when neither is NaN
+__device__ __forceinline__ double hb_nan_max(double a, double b)
+{
+  return (a != a || b != b) ? a + b : fmax(a, b);
+}
 __device__ __forceinline__ double hb_warp_min(double v)
 {
 #pragma unroll

@@ -342,7 +342,8 @@ __device__ void dev_backward(const double* __restrict__ A, int lda, int N, doubl
 }
 
 // One-CTA SPD solve with equilibration scaling s and device-side refinement against the unscaled matrix Nref
-// (full symmetric storage, row-major, ld = ldn). stats: [0]=#refinements, [1]=last residual inf-norm, [2]=info.
+// (full symmetric storage, row-major, ld = ldn). stats: [0]=#refinements, [1]=last residual inf-norm (NaN when it is not finite:
+// the loop stops at the first such residual, a correction from it could only spread the NaN).
 __global__ void __launch_bounds__(SOLVE_THREADS)
 k_spd_solve_refine(const double* __restrict__ F, int ldf, int N, const double* __restrict__ s, const double* __restrict__ Nref, int ldn,
                    const double* __restrict__ rhs, double* __restrict__ x, double* __restrict__ work /* 2N */, double tol, int max_refine,
@@ -372,19 +373,23 @@ k_spd_solve_refine(const double* __restrict__ F, int ldf, int N, const double* _
       acc = hb_warp_sum(acc);
       const double ri = rhs[i] - acc;
       if(lane == 0) r[i] = ri;
-      wmax = fmax(wmax, fabs(ri));
+      wmax = hb_nan_max(wmax, fabs(ri));
     }
     __syncthreads();
     if(lane == 0) sm[warp] = wmax;
     __syncthreads();
     if(tid == 0) {
       double m = 0.0;
-      for(int w = 0; w < SOLVE_THREADS / 32; w++) m = fmax(m, sm[w]);
+      for(int w = 0; w < SOLVE_THREADS / 32; w++) m = hb_nan_max(m, sm[w]);
       s_nrm = m;
     }
     __syncthreads();
     nrm = s_nrm;
-    if(!(nrm >= tol) || nref >= max_refine) break; // also leaves on NaN
+    if(!isfinite(nrm)) {
+      nrm = __longlong_as_double(0x7ff8000000000000LL);
+      break;
+    }
+    if(!(nrm >= tol) || nref >= max_refine) break;
     for(int i = tid; i < N; i += SOLVE_THREADS) r[i] *= s[i];
     __syncthreads();
     dev_forward(F, ldf, N, r, false, sd);

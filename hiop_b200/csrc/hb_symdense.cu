@@ -38,7 +38,7 @@ constexpr int CONDENSED_BIG_MIN_N = 2049; // condensed N: the look-ahead Cholesk
 constexpr int SYTRS_CTA_MIN_N = 65, SYTRS_CTA_MAX_NRHS = 7;
 
 enum Factor { F_SYTF2, F_SYTRF_BLOCKED, F_BK_CLUSTER, F_PANEL_CHOL, F_PANEL_LDL, F_COOP_CHOL, F_BIG_CHOL, F_BIG_LDL };
-enum Solve { S_SYTRS, S_ONE_CTA, S_BIG };
+enum Solve { S_SYTRS, S_ONE_CTA, S_BIG, S_COOP_REFINE, S_ONE_CTA_REFINE };
 enum Inertia { I_IPIV, I_BLOCKDIAG, I_DIAG };
 struct Plan
 {
@@ -60,6 +60,25 @@ Plan symdense_plan(const hb_ctx* c, int mode, int N)
   if(N >= (ldl ? c->big_min_ldl : c->big_min_chol)) return {ldl ? F_BIG_LDL : F_BIG_CHOL, S_BIG, I_DIAG, N >= c->pair_min};
   const Factor f = ldl ? F_PANEL_LDL : coop_factor(c, N) ? F_COOP_CHOL : F_PANEL_CHOL;
   return {f, N >= BIG_SOLVE_MIN_N ? S_BIG : S_ONE_CTA, I_DIAG, false};
+}
+
+// The condensed N (second block of the table): the factor path, the solve with refinement, whether the 16 x 16 diagonal inverses of the
+// cooperative solve are formed after a factor that does not produce them itself, and the look-ahead pairing.
+struct CondensedPlan
+{
+  Factor f;
+  Solve s;
+  bool inverses;
+  bool pairs;
+};
+
+CondensedPlan condensed_plan(const hb_ctx* c, int N, int ldf, const double* F)
+{
+  const Solve s = c->coop_ctas > 0 && N >= COOP_MIN_N && N <= COOP_SOLVE_MAX_N ? S_COOP_REFINE : S_ONE_CTA_REFINE;
+  if(coop_factor(c, N)) return {F_COOP_CHOL, s, false, false};
+  const bool inv = N >= COOP_MIN_N && c->coop_ctas > 0;
+  if(N >= CONDENSED_BIG_MIN_N && (ldf & 1) == 0 && (reinterpret_cast<uintptr_t>(F) & 15u) == 0) return {F_BIG_CHOL, s, inv, N >= c->pair_min};
+  return {F_PANEL_CHOL, s, inv, false};
 }
 
 int bk_sytrs(hb_ctx* c, int N, const double* A, int lda, const int* ipiv_dev, double* B, int ldb, int nrhs)
@@ -103,12 +122,13 @@ int hb_dense_bk_small_solve(hb_ctx* c, int N, const double* A, int lda, const in
 
 int hb_dense_condensed_factor(hb_ctx* c, hb_big* big, int N, double* F, int ldf, double* invd, int* info_dev)
 {
-  if(coop_factor(c, N)) return hb_dense_chol_coop(c, N, F, ldf, info_dev, invd, nullptr);
-  if(N >= CONDENSED_BIG_MIN_N && (ldf & 1) == 0 && (reinterpret_cast<uintptr_t>(F) & 15u) == 0)
-    HB_CHECK(hb_big_factor(c, big, N, F, ldf, false, N >= c->pair_min, info_dev));
-  else
-    HB_CHECK(hb_dense_factor_panel(c, N, F, ldf, false, nullptr, info_dev));
-  if(N >= COOP_MIN_N && c->coop_ctas > 0) HB_CHECK(hb_dense_chol_diag_inverses(c, N, F, ldf, invd)); // for the cooperative solve
+  const CondensedPlan p = condensed_plan(c, N, ldf, F);
+  switch(p.f) {
+  case F_COOP_CHOL: HB_CHECK(hb_dense_chol_coop(c, N, F, ldf, info_dev, invd, nullptr)); break;
+  case F_BIG_CHOL: HB_CHECK(hb_big_factor(c, big, N, F, ldf, false, p.pairs, info_dev)); break;
+  default: HB_CHECK(hb_dense_factor_panel(c, N, F, ldf, false, nullptr, info_dev)); break;
+  }
+  if(p.inverses) HB_CHECK(hb_dense_chol_diag_inverses(c, N, F, ldf, invd));
   return HB_OK;
 }
 
@@ -116,7 +136,7 @@ int hb_dense_condensed_solve(hb_ctx* c, int N, const double* F, int ldf, const d
                              const double* rhs, double* x, double* work, double tol, int max_refine, double* stats_dev)
 {
   if(N == 0) return HB_OK;
-  if(c->coop_ctas > 0 && N >= COOP_MIN_N && N <= COOP_SOLVE_MAX_N)
+  if(condensed_plan(c, N, ldf, F).s == S_COOP_REFINE)
     return hb_dense_spd_solve_coop(c, N, F, ldf, invd, s, Nref, ldn, rhs, x, work, tol, max_refine, stats_dev);
   return hb_dense_spd_solve_refine(c, N, F, ldf, s, Nref, ldn, rhs, x, work, tol, max_refine, stats_dev);
 }
@@ -331,4 +351,37 @@ extern "C" int hb_debug_bk_profile(hb_ctx* c, int on, long long* prof_host8)
 {
   HB_REQUIRE(c, "null ctx");
   return hb_bkc_profile(c, on, prof_host8);
+}
+
+// diagnostics (tests): the condensed-N sequence of hb_lowrank (equilibrate, factor, solve with refinement) on caller matrices, with
+// scratch allocated like the handle's (ld N, one allocation per buffer).
+extern "C" int hb_debug_condensed_solve(hb_ctx* c, int N, const double* Nfact, const double* Nref, int ldn, const double* rhs, double* x,
+                                        double tol, int max_refine, int* plan4, double* s_host, double* Aeq_host, double* F_host,
+                                        double* stats_host, int* info_host)
+{
+  HB_REQUIRE(c && N > 0 && ldn >= N && Nfact && Nref && rhs && x && max_refine >= 0, "hb_debug_condensed_solve: bad arguments");
+  HB_CUDA(cudaSetDevice(c->device));
+  hb_big big;
+  hb_dev<double> F, s, invd, work, stats;
+  hb_dev<int> info;
+  HB_CHECK(F.reserve(c, (size_t)N * N, "the factor of N"));
+  HB_CHECK(s.reserve(c, N, "the scaling of N"));
+  HB_CHECK(work.reserve(c, 2 * (size_t)N + 2, "refinement scratch"));
+  HB_CHECK(invd.reserve(c, HB_CHOL_INV_DOUBLES(N), "diagonal-block inverses of N"));
+  HB_CHECK(stats.reserve(c, 4, "solve statistics"));
+  HB_CHECK(info.reserve(c, 1, "info word"));
+  const CondensedPlan p = condensed_plan(c, N, N, F);
+  if(plan4) { plan4[0] = p.f; plan4[1] = p.s; plan4[2] = p.inverses; plan4[3] = p.pairs; }
+  HB_CUDA(cudaMemsetAsync(info, 0, sizeof(int), c->stream));
+  HB_CHECK(hb_dense_equilibrate(c, N, Nfact, ldn, F, N, s));
+  if(Aeq_host) HB_CUDA(cudaMemcpyAsync(Aeq_host, F, sizeof(double) * (size_t)N * N, cudaMemcpyDeviceToHost, c->stream));
+  if(s_host) HB_CUDA(cudaMemcpyAsync(s_host, s, sizeof(double) * N, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  HB_CHECK(hb_dense_condensed_factor(c, &big, N, F, N, invd, info));
+  HB_CHECK(hb_dense_condensed_solve(c, N, F, N, invd, s, Nref, ldn, rhs, x, work, tol, max_refine, stats));
+  if(F_host) HB_CUDA(cudaMemcpyAsync(F_host, F, sizeof(double) * (size_t)N * N, cudaMemcpyDeviceToHost, c->stream));
+  if(stats_host) HB_CUDA(cudaMemcpyAsync(stats_host, stats, sizeof(double) * 2, cudaMemcpyDeviceToHost, c->stream));
+  if(info_host) HB_CUDA(cudaMemcpyAsync(info_host, info, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return HB_OK;
 }

@@ -198,6 +198,16 @@ int hb_debug_bk_profile(hb_ctx* ctx, int on, long long* prof_host8);
  * with the upper triangle valid as M (unpadded for odd N). ipiv_host: N pivots (LAPACK's convention), Bunch-Kaufman only.
  * perm_host / dsub_host: N entries each, cluster Bunch-Kaufman only. */
 int hb_debug_symdense_factor(hb_symdense* s, int* plan4, int* bk_widths, double* F_host, int* ipiv_host, int* perm_host, double* dsub_host);
+/* diagnostics (tests): the condensed-N solve of the quasi-Newton handle on caller matrices (N >= 1; device, row-major, ld ldn): equilibrate
+ * Nfact, Cholesky of the equilibrated matrix, then solve N x = rhs (device, N doubles each) refining with residuals rhs - Nref x until
+ * ||r||_inf < tol or max_refine corrections. The handle passes the same matrix as Nfact and Nref, with tol 1e-8 and max_refine 3.
+ * Synchronises the stream; every output may be NULL. plan4: factor and solve kernels of the condensed rows of the dispatch table in
+ * hb_symdense.cu (enum order there), 1 if the 16 x 16 diagonal inverses were formed after the factor, 1 if the look-ahead
+ * factorization took its blocks in pairs. s_host: the N scale factors. Aeq_host / F_host: the equilibrated matrix before the factor /
+ * the factor, N x N row-major with the upper triangle valid. stats_host: {corrections, last residual inf-norm (NaN if not finite)}.
+ * info_host: 0, or the order of the first leading minor that is not positive definite. */
+int hb_debug_condensed_solve(hb_ctx* ctx, int N, const double* Nfact, const double* Nref, int ldn, const double* rhs, double* x, double tol,
+                             int max_refine, int* plan4, double* s_host, double* Aeq_host, double* F_host, double* stats_host, int* info_host);
 
 /* ---- the same system factored across the ranks of the context's communicator (hb_symdense_dist.cu) ----
  * 1-D block-cyclic layout with block size 128: block row k (rows k*128 .. min(N, k*128+128)-1 of the N x N row-major matrix, full

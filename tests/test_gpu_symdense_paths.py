@@ -371,9 +371,10 @@ def test_condensed_solve_needs_no_refinement(make_ctx, m, coop):
     FP64, adding gamma(m+1)(|N||dy| + |rhs|)_i, and |rhs| <= |N||dy| + |r| moves |r| to the left: divide by 1 - gamma(m+1). The solve
     reports only ||r||_inf, so the check is ||r||_inf <= max_i bound_i (a norm comparison of the componentwise bound).
 
-    Which factorization runs is chosen by m inside the quasi-Newton handle (hb_dense_condensed_factor, dispatch table of hb_symdense.cu)
-    and is not read back here: m = 6144 is the paired look-ahead, 6145 (odd ld) the panels, 2049 / 2050 the panels / look-ahead, up to
-    2048 the cooperative kernels; without cooperative launches the panels and the one-CTA refinement solve."""
+    Which factorization runs is chosen by m inside the quasi-Newton handle (condensed_plan, dispatch table of hb_symdense.cu): m = 6144
+    is the paired look-ahead, 6145 (odd ld) the panels, 2049 / 2050 the panels / look-ahead, up to 2048 the cooperative kernels; without
+    cooperative launches the panels and the one-CTA refinement solve. test_gpu_condensed_refine.py asserts those rows through
+    hb_debug_condensed_solve, which runs the same plan."""
     ctx = make_ctx(**({} if coop else NOCOOP))
     P = synth.make_qn_problem(max(600, 3 * m), m, 4, seed=77 + m)
     p = _as_dict(P)
