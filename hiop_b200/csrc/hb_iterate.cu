@@ -241,23 +241,34 @@ extern "C" int hb_iterate_adjust_small_slacks(hb_lowrank* k, double* const* it, 
   const double small_val = eps * fmin(1.0, mu);
   const double scale_fact = pow(eps, 0.75);
   HB_CHECK(hb_ws_reserve(c, 64));
-  int* cnt = (int*)c->ws.get();
-  HB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(int), c->stream));
-  struct Blk { int s, z; const double* bound; const double* sel; long long len; };
-  const Blk blks[4] = {{SXL, ZL, xl, k->ixl, k->n}, {SXU, ZU, xu, k->ixu, k->n}, {SDL, VL, dl, k->idl, (long long)k->mineq},
-                       {SDU, VU, du, k->idu, (long long)k->mineq}};
+  int* cnt = (int*)c->ws.get(); // {x side, d side}
+  HB_CUDA(cudaMemsetAsync(cnt, 0, 2 * sizeof(int), c->stream));
+  struct Blk { int s, z; const double* bound; const double* sel; long long len; int side; };
+  const Blk blks[4] = {{SXL, ZL, xl, k->ixl, k->n, 0}, {SXU, ZU, xu, k->ixu, k->n, 0}, {SDL, VL, dl, k->idl, (long long)k->mineq, 1},
+                       {SDU, VU, du, k->idu, (long long)k->mineq, 1}};
   for(const Blk& b : blks) {
     if(b.len == 0) continue;
     double smin = 0.0;
     HB_CHECK(hb_vec_min_w_pattern(c, b.len, it[b.s], b.sel, &smin)); // slack.min_w_pattern(select) :432
     if(!(smin < small_val)) continue;
-    k_adjust_small_slack<<<hb_grid(c, b.len, ET), ET, 0, c->stream>>>(b.len, mu, small_val, scale_fact, b.bound, it_curr[b.z], b.sel, it[b.s], cnt);
+    k_adjust_small_slack<<<hb_grid(c, b.len, ET), ET, 0, c->stream>>>(b.len, mu, small_val, scale_fact, b.bound, it_curr[b.z], b.sel, it[b.s],
+                                                                      cnt + b.side);
     HB_LAUNCHED();
   }
-  int h = 0;
-  HB_CUDA(cudaMemcpyAsync(&h, cnt, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  int h[2] = {0, 0};
+  HB_CUDA(cudaMemcpyAsync(h, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if(num_adjusted) *num_adjusted = h;
+  double nx = h[0];
+  if(c->nranks > 1) { // the x-side slacks are sharded: numOfElemsLessThan sums their count over the ranks (hiopVectorPar.cpp:1222-1239), on
+                      // every rank, whether or not its blocks needed the kernel; the d side is replicated and counts once. The sum is exact.
+    c->red_host[0] = nx;
+    HB_CUDA(cudaMemcpyAsync(c->red_dev, c->red_host, sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    HB_CHECK(hb_allreduce_op(c, c->red_dev, 1, HB_SUM));
+    HB_CUDA(cudaMemcpyAsync(c->red_host, c->red_dev, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    HB_CUDA(cudaStreamSynchronize(c->stream));
+    nx = c->red_host[0];
+  }
+  if(num_adjusted) *num_adjusted = (int)nx + h[1];
   return HB_OK;
 }
 

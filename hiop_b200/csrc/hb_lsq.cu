@@ -65,12 +65,14 @@ extern "C" int hb_lowrank_lsq_duals(hb_lowrank* k, const double* grad_f, const d
   HB_CHECK(hb_dense_lsq_factor(c, m, M, m, k->info + 3));
   HB_CHECK(hb_dense_lsq_solve(c, m, M, m, rhs));
   HB_CUDA(cudaMemcpyAsync(k->info_host + 3, k->info + 3, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  if(me) HB_CUDA(cudaMemcpyAsync(yc, rhs, sizeof(double) * me, cudaMemcpyDeviceToDevice, c->stream));
-  if(mi) HB_CUDA(cudaMemcpyAsync(yd, rhs + me, sizeof(double) * mi, cudaMemcpyDeviceToDevice, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  if(k->info_host[3] != 0) { // "dpotrf (Chol fact) detected %d minor being indefinite" :722-725 -> the driver keeps the old duals
+  if(k->info_host[3] != 0) { // "dpotrf (Chol fact) detected %d minor being indefinite" :722-725 -> the driver keeps the old duals, so
+                             // yc and yd are left as the caller passed them (the reference returns before copyToStarting, :270-275, 318-320)
     snprintf(g_hb_err, sizeof(g_hb_err), "hb_lowrank_lsq_duals: J J^T + I is not SPD (leading minor %d)", k->info_host[3]);
     return HB_ERR_NUMERIC;
   }
+  if(me) HB_CUDA(cudaMemcpyAsync(yc, rhs, sizeof(double) * me, cudaMemcpyDeviceToDevice, c->stream));
+  if(mi) HB_CUDA(cudaMemcpyAsync(yd, rhs + me, sizeof(double) * mi, cudaMemcpyDeviceToDevice, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
   return HB_OK;
 }
