@@ -13,7 +13,7 @@ SO_PATH = os.environ.get("HIOPB200_SO") or os.path.join(_HERE, "libhiopb200.so")
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "hiopb200.h")
 
 HB_OK = 0
-HB_FACT_BUNCH_KAUFMAN, HB_FACT_NOPIV, HB_FACT_CHOLESKY = 0, 1, 2
+HB_FACT_BUNCH_KAUFMAN, HB_FACT_NOPIV, HB_FACT_CHOLESKY, HB_FACT_RBT_NOPIV = 0, 1, 2, 3
 HB_CONDENSE_AUTO, HB_CONDENSE_FP64_DMMA, HB_CONDENSE_INT8_CRT = -1, 0, 100
 
 c_dp = ctypes.c_void_p   # device or host pointer to doubles (passed as integer address)
@@ -134,6 +134,8 @@ def lib() -> ctypes.CDLL:
     f("hb_symdense_dist_inertia", c_i, c_vp, P(c_i), P(c_i), P(c_i))
     f("hb_symdense_dist_solve", c_i, c_vp, c_dp, c_i)
     f("hb_symdense_dist_profile", c_i, c_vp, c_i, P(ctypes.c_float))
+    f("hb_symdense_dist_rbt_stats", c_i, c_vp, P(c_i), P(ctypes.c_double), P(ctypes.c_float))
+    f("hb_debug_symdense_dist_rbt", c_i, c_vp, c_i)
     f("hb_microbench_peak", c_i, c_vp, c_i, P(c_d))
     # lowrank
     f("hb_lowrank_create", c_i, c_vp, c_ll, c_i, c_i, c_i, P(c_vp))

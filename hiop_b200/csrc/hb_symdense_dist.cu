@@ -19,6 +19,11 @@
 // Solves (x replicated on every rank): forward sweep, owner of block k: y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, z_k = y_k (/ d_k), then
 // the broadcast of rows k*128 .. N; backward sweep, owner of block k: x_k = L_kk^-T (z_k - L_>k,k^T x_>k), broadcast of its rows. Every
 // block is computed by its owner in the same order for every P, so the solution does not depend on P.
+//
+// Safe mode (HB_FACT_RBT_NOPIV): A' = U^T A U with a depth-2 random butterfly U = B2 B1 (rbt_transform: the mirror of the upper
+// triangle, then one pass per level, each output row formed from its row and its partner row), the no-pivot LDL^T above on A', and
+// solves refined against a kept copy of A' (rbt_solve). Every entry of A' is a fixed expression of oracle/rbt_model.py and the random
+// diagonals depend on N alone, so A', the factor and the solution do not depend on P either.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
 
@@ -156,6 +161,188 @@ __global__ void __launch_bounds__(DB * SOLVE_RHS) k_dist_bwd_diag(const double* 
   if(live) xw[(size_t)(k0 + i) * nrhs + c] = xs[cl * DB + i];
 }
 
+// ---- random butterfly transform (HB_FACT_RBT_NOPIV): A' = U^T A U, U = B2 B1 (oracle/rbt_model.py states every expression) ----------
+constexpr unsigned long long RBT_SEED = 0x5EED2011B7F10001ull, RBT_GOLDEN = 0x9E3779B97F4A7C15ull;
+constexpr double RBT_C = 0.7071067811865476; // the double nearest 1/sqrt(2)
+constexpr double RBT_EPS = 0x1p-52;          // refinement target of the backward error
+constexpr int RBT_MAX_CORR = 3;
+constexpr int RBT_COLS = 1024;               // columns per CTA of k_rbt_level (256 threads x 4)
+
+// r_t of butterfly `half` of `level`: 1 + (k - 2^19) / 2^23, k = the top 20 bits of splitmix64 of the counter (stream << 32 | t)
+__device__ __forceinline__ double rbt_diag(int level, int half, int t)
+{
+  unsigned long long z = RBT_SEED + RBT_GOLDEN * ((((unsigned long long)(2 * level + half)) << 32 | (unsigned)t) + 1ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  z ^= z >> 31;
+  return (double)((1LL << 23) + (long long)(z >> 44) - (1LL << 19)) / (double)(1 << 23);
+}
+
+// the entries of column i of a level's butterfly: rows lo and hi (lo = hi = i when unpaired), sign s of the hi side (+1 on the lo side)
+struct rbt_pos
+{
+  int lo, hi;
+  double s;
+  bool paired;
+};
+__device__ __forceinline__ rbt_pos rbt_at(int N, int level, int i)
+{
+  int o = 0, n = N;
+  if(level == 2) {
+    const int h = (N + 1) / 2;
+    if(i >= h) o = h, n = N - h;
+    else n = h;
+  }
+  const int hh = (n + 1) / 2, t = i - o;
+  if(t < n - hh) return {i, i + hh, 1.0, true};
+  if(t >= hh) return {i - hh, i, -1.0, true};
+  return {i, i, 1.0, false};
+}
+
+// f[(level - 1) * N + i]: the diagonal entry of column i at level 1 (B1) and 2 (B2); a function of N alone
+__global__ void k_rbt_table(int N, double* __restrict__ f)
+{
+  const int h = (N + 1) / 2;
+  for(int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
+    f[i] = rbt_diag(1, 0, i);
+    f[N + i] = i < h ? rbt_diag(2, 0, i) : rbt_diag(2, 1, i - h);
+  }
+}
+
+__device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / DB) * P + rank) * DB + y % DB; }
+
+// mirror: every owned row r gets dst(r, j) = src(j, r) for the columns q0 <= j < q0 + nq, j < r, where src holds the rows q0 .. of the
+// upper triangle (ld doubles each). 32 x 32 tiles through shared memory: rows y0 .. of the owned rows, starting at local row ybeg.
+__global__ void __launch_bounds__(256) k_rbt_mirror(int N, int P, int rank, int nrows, int ybeg, const double* __restrict__ src, long long ld, int q0,
+                                                    int nq, double* __restrict__ dst)
+{
+  __shared__ double tile[32][33];
+  const int y0 = ybeg + blockIdx.y * 32, j0 = q0 + blockIdx.x * 32, tx = threadIdx.x % 32, ty = threadIdx.x / 32;
+  for(int jj = ty; jj < 32; jj += 8) {
+    const int y = y0 + tx, j = j0 + jj;
+    const int r = rbt_global_row(y, P, rank);
+    tile[jj][tx] = (y < nrows && r < N && j < q0 + nq && j < r) ? src[(size_t)(j - q0) * ld + r] : 0.0;
+  }
+  __syncthreads();
+  for(int yy = ty; yy < 32; yy += 8) {
+    const int y = y0 + yy, j = j0 + tx;
+    const int r = rbt_global_row(y, P, rank);
+    if(y < nrows && r < N && j < q0 + nq && j < r) dst[(size_t)y * ld + j] = tile[tx][yy];
+  }
+}
+
+// one level B^T A B on full rows. CTA x = a source row q: local row x of `in` (src == nullptr: every partner is local) or row x of src
+// (global rows q0 .. q0 + nq, the owner's broadcast). Its partner r (q itself when unpaired), when this rank owns it, gets its whole
+// output row from rows r and q: out(r, j) = (f_r f_j) (t w) with t and w of oracle/rbt_model.py, in that operation order.
+__global__ void __launch_bounds__(256) k_rbt_level(int N, int level, const double* __restrict__ f, const double* __restrict__ in, long long ld, int P,
+                                                   int rank, const double* __restrict__ src, int q0, double* __restrict__ out)
+{
+  const int q = src ? q0 + blockIdx.x : rbt_global_row(blockIdx.x, P, rank);
+  if(q >= N) return;
+  const double* rowq = src ? src + (size_t)blockIdx.x * ld : in + (size_t)blockIdx.x * ld;
+  const rbt_pos pq = rbt_at(N, level, q);
+  const int r = pq.lo == q ? pq.hi : pq.lo;
+  if((r / DB) % P != rank) return;
+  const size_t lr = (size_t)(r / DB / P) * DB + r % DB;
+  const double* rowr = in + lr * ld;
+  const rbt_pos pr = rbt_at(N, level, r);
+  const double* RL = pr.lo == r ? rowr : rowq;
+  const double* RH = pr.hi == r ? rowr : rowq;
+  const double* fl = f + (size_t)(level - 1) * N;
+  const double fi = fl[r];
+  double* o = out + lr * ld;
+  const int jend = min(N, (int)(blockIdx.y + 1) * RBT_COLS);
+  for(int j = blockIdx.y * RBT_COLS + threadIdx.x; j < jend; j += 256) {
+    const rbt_pos pj = rbt_at(N, level, j);
+    const double all = RL[pj.lo], ahh = RH[pj.hi], ss = pr.s * pj.s;
+    double t, w;
+    if(pr.paired && pj.paired) {
+      t = __dadd_rn(__dadd_rn(all, __dmul_rn(ss, ahh)), __dadd_rn(__dmul_rn(pj.s, RL[pj.hi]), __dmul_rn(pr.s, RH[pj.lo])));
+      w = 0.5;
+    } else if(pr.paired || pj.paired) {
+      t = __dadd_rn(all, __dmul_rn(ss, ahh));
+      w = RBT_C;
+    } else {
+      t = all;
+      w = 1.0;
+    }
+    o[j] = __dmul_rn(__dmul_rn(fi, fl[j]), __dmul_rn(t, w));
+  }
+}
+
+// one level on the replicated row-major vectors (N x nrhs): B^T v (trans) or B v
+__global__ void k_rbt_vec(int N, int nrhs, int level, const double* __restrict__ f, const double* __restrict__ in, double* __restrict__ out, int trans)
+{
+  const double* fl = f + (size_t)(level - 1) * N;
+  const long long total = (long long)N * nrhs;
+  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int i = (int)(e / nrhs), c = (int)(e % nrhs);
+    const rbt_pos p = rbt_at(N, level, i);
+    const double vl = in[(size_t)p.lo * nrhs + c], vh = in[(size_t)p.hi * nrhs + c];
+    double v;
+    if(!p.paired) v = __dmul_rn(fl[i], vl);
+    else if(trans) v = __dmul_rn(fl[i], __dmul_rn(__dadd_rn(vl, __dmul_rn(p.s, vh)), RBT_C));
+    else v = __dmul_rn(__dadd_rn(__dmul_rn(fl[p.lo], vl), __dmul_rn(p.s, __dmul_rn(fl[p.hi], vh))), RBT_C);
+    out[e] = v;
+  }
+}
+
+// CTA per owned row r of A' (full rows): out_r = sum_j |A'(r, j)| (norm) or r_r = b'_r - sum_j A'(r, j) x'_j per rhs, in a fixed order
+__global__ void __launch_bounds__(256) k_rbt_rows(int N, int P, int rank, const double* __restrict__ A, long long ld, int nrhs, const double* __restrict__ x,
+                                                  const double* __restrict__ b, double* __restrict__ out)
+{
+  __shared__ double red[8];
+  const int r = rbt_global_row(blockIdx.x, P, rank);
+  if(r >= N) {
+    if(!x && threadIdx.x == 0) out[blockIdx.x] = 0.0;
+    return;
+  }
+  const double* row = A + (size_t)blockIdx.x * ld;
+  if(!x) {
+    double acc = 0.0;
+    for(int j = threadIdx.x; j < N; j += 256) acc += fabs(row[j]);
+    acc = hb_block_sum<256>(acc, red);
+    if(threadIdx.x == 0) out[blockIdx.x] = acc;
+    return;
+  }
+  for(int c = 0; c < nrhs; c++) {
+    double acc = 0.0;
+    for(int j = threadIdx.x; j < N; j += 256) acc += row[j] * x[(size_t)j * nrhs + c];
+    acc = hb_block_sum<256>(acc, red);
+    if(threadIdx.x == 0) out[(size_t)r * nrhs + c] = b[(size_t)r * nrhs + c] - acc;
+    __syncthreads();
+  }
+}
+
+__device__ __forceinline__ double rbt_nanmax(double m, double v) { return (v > m || v != v) ? v : m; }
+
+// one CTA per column c: out[c * 3 + k] = max_i |v_k(i, c)| over the N rows of the row-major N x ncols arrays v_0, v_1, v_2 (0 for an
+// absent one), NaN kept, in a fixed order
+__global__ void __launch_bounds__(256) k_rbt_max(int N, int ncols, const double* __restrict__ v0, const double* __restrict__ v1, const double* __restrict__ v2,
+                                                 double* __restrict__ out)
+{
+  __shared__ double sm[3][256];
+  const double* v[3] = {v0, v1, v2};
+  const int c = blockIdx.x;
+  for(int k = 0; k < 3; k++) {
+    double m = 0.0;
+    if(v[k])
+      for(int i = threadIdx.x; i < N; i += 256) m = rbt_nanmax(m, fabs(v[k][(size_t)i * ncols + c]));
+    sm[k][threadIdx.x] = m;
+  }
+  __syncthreads();
+  if(threadIdx.x < 3) {
+    double m = 0.0;
+    for(int t = 0; t < 256; t++) m = rbt_nanmax(m, sm[threadIdx.x][t]);
+    out[(size_t)c * 3 + threadIdx.x] = m;
+  }
+}
+
+__global__ void k_rbt_axpy(long long n, const double* __restrict__ d, double* __restrict__ x)
+{
+  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) x[e] += d[e];
+}
+
 enum { PH_PANEL = 0, PH_BCAST, PH_UPDATE, PH_COUNT };
 
 // Every rank's local result rc (HB_OK or an HB_ERR_* code) made common before the next collective, so that a rank whose allocation
@@ -199,6 +386,15 @@ struct hb_symdense_dist
   int mode = -1;
   bool factored = false;
   int n_neg = 0, n_null = 0, n_pos = 0;
+  // HB_FACT_RBT_NOPIV, allocated by the first RBT factorization: A' (full rows, owned like A), the butterfly diagonals (2 N), the row
+  // sums of |A'| and norm scratch; the solve adds b', the residual and the per-rhs norms
+  bool rbt_ready = false;
+  hb_dev<double> Ak, rbt_f, rbt_rows, rbt_nrm, rbt_b, rbt_r;
+  hb_pinned<double> rbt_nrm_host;
+  hb_event ev_rbt[2];
+  double rbt_anorm = 0.0, rbt_berr = 0.0;
+  int rbt_corr = 0;
+  float rbt_ms = 0.f;
   ~hb_symdense_dist()
   {
     if(sp) cudaStreamSynchronize(sp);
@@ -301,19 +497,137 @@ extern "C" int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3)
   return HB_OK;
 }
 
+// the RBT buffers, on the first RBT factorization of the handle (every rank calls it, then agree())
+static int rbt_reserve(hb_symdense_dist* s)
+{
+  if(s->rbt_ready) return HB_OK;
+  hb_ctx* c = s->ctx;
+  HB_CHECK(s->Ak.reserve(c, (size_t)s->nloc * DB * s->ld, "the transformed matrix A'"));
+  HB_CHECK(s->rbt_f.reserve(c, (size_t)2 * s->N, "butterfly diagonals"));
+  HB_CHECK(s->rbt_rows.reserve(c, (size_t)s->nloc * DB, "row sums of |A'|"));
+  HB_CHECK(s->rbt_nrm.reserve(c, 4, "norm of A'"));
+  for(int e = 0; e < 2; e++) HB_CHECK(s->ev_rbt[e].create(cudaEventDefault));
+  k_rbt_table<<<hb_grid(c, s->N), 256, 0, c->stream>>>(s->N, s->rbt_f);
+  HB_LAUNCHED();
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  s->rbt_ready = true;
+  return HB_OK;
+}
+
+// true when every row's partner at `level` is owned by the rank that owns the row, decided from N and P alone (every rank agrees): all
+// pairing distances are multiples of 128 P
+static bool rbt_level_local(int N, int P, int level)
+{
+  if(P == 1) return true;
+  auto ok = [&](int n) { const int hh = (n + 1) / 2; return n - hh == 0 || hh % (DB * P) == 0; };
+  if(level == 1) return ok(N);
+  const int h = (N + 1) / 2;
+  return ok(h) && ok(N - h);
+}
+
+// the first `stages` steps of A' = U^T A U on the owned rows: the mirror of the upper triangle into the lower part of every row, then
+// B2^T A B2 (stage 1) and B1^T (.) B1 (stage 2). The result is left in A; after stage 2 it is also kept in Ak, with ||A'||_inf in
+// rbt_anorm. Every rank issues the same broadcasts: the owner of block k sends its rows from its own buffer, the others receive them in
+// the first panel broadcast buffer.
+static int rbt_transform(hb_symdense_dist* s, int stages)
+{
+  hb_ctx* c = s->ctx;
+  const int N = s->N, P = s->P, rank = s->rank, nrows = s->nloc * DB;
+  const long long ld = s->ld;
+  cudaStream_t st = c->stream;
+  double* recv = s->bbuf[0];
+  if(s->profile) HB_CUDA(cudaEventRecord(s->ev_rbt[0], st));
+  // mirror
+  for(int k = 0; k < s->nblk; k++) {
+    const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
+    double* src = P == 1 ? s->A.get() : (owner == rank ? s->A.get() + (size_t)(k / P) * DB * ld : recv);
+    if(P > 1) HB_CHECK(hb_broadcast(c, src, (long long)nb * ld, owner, st));
+    const int q0 = P == 1 ? 0 : k0, nq = P == 1 ? N : nb;
+    const int qa = k <= rank ? 0 : (k - rank + P - 1) / P; // first owned block at or after k
+    if(nrows > qa * DB) {
+      k_rbt_mirror<<<dim3((nq + 31) / 32, (nrows - qa * DB + 31) / 32), 256, 0, st>>>(N, P, rank, nrows, qa * DB, src, ld, q0, nq, s->A);
+      HB_LAUNCHED();
+    }
+    if(P == 1) break;
+  }
+  // the two levels: A -> Ak (B2), Ak -> A (B1)
+  const int chunks = (N + RBT_COLS - 1) / RBT_COLS;
+  for(int st_i = 0; st_i < stages; st_i++) {
+    const int level = st_i == 0 ? 2 : 1;
+    const double* in = st_i == 0 ? s->A.get() : s->Ak.get();
+    double* out = st_i == 0 ? s->Ak.get() : s->A.get();
+    if(rbt_level_local(N, P, level)) {
+      if(nrows > 0) {
+        k_rbt_level<<<dim3(nrows, chunks), 256, 0, st>>>(N, level, s->rbt_f, in, ld, P, rank, nullptr, 0, out);
+        HB_LAUNCHED();
+      }
+      continue;
+    }
+    for(int k = 0; k < s->nblk; k++) {
+      const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
+      double* src = owner == rank ? const_cast<double*>(in) + (size_t)(k / P) * DB * ld : recv;
+      HB_CHECK(hb_broadcast(c, src, (long long)nb * ld, owner, st));
+      k_rbt_level<<<dim3(nb, chunks), 256, 0, st>>>(N, level, s->rbt_f, in, ld, P, rank, src, k0, out);
+      HB_LAUNCHED();
+    }
+  }
+  if(stages == 1) HB_CUDA(cudaMemcpyAsync(s->A, s->Ak, sizeof(double) * nrows * ld, cudaMemcpyDeviceToDevice, st));
+  if(s->profile) HB_CUDA(cudaEventRecord(s->ev_rbt[1], st));
+  if(stages == 2) {
+    HB_CUDA(cudaMemcpyAsync(s->Ak, s->A, sizeof(double) * nrows * ld, cudaMemcpyDeviceToDevice, st));
+    if(nrows > 0) {
+      k_rbt_rows<<<nrows, 256, 0, st>>>(N, P, rank, s->Ak, ld, 0, nullptr, nullptr, s->rbt_rows);
+      HB_LAUNCHED();
+    }
+    k_rbt_max<<<1, 256, 0, st>>>(nrows, 1, s->rbt_rows, nullptr, nullptr, s->rbt_nrm);
+    HB_LAUNCHED();
+    HB_CHECK(hb_allreduce_op(c, s->rbt_nrm, 1, HB_MAX));
+    HB_CUDA(cudaMemcpyAsync(s->red_host, s->rbt_nrm, sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
+  HB_CUDA(cudaStreamSynchronize(st));
+  if(stages == 2) s->rbt_anorm = s->red_host[0];
+  s->rbt_ms = 0.f;
+  if(s->profile) HB_CUDA(cudaEventElapsedTime(&s->rbt_ms, s->ev_rbt[0], s->ev_rbt[1]));
+  return HB_OK;
+}
+
+extern "C" int hb_debug_symdense_dist_rbt(hb_symdense_dist* s, int stages)
+{
+  HB_REQUIRE(s && stages >= 0 && stages <= 2, "hb_debug_symdense_dist_rbt: bad arguments");
+  if(s->N == 0) return HB_OK;
+  HB_CUDA(cudaSetDevice(s->ctx->device));
+  HB_CHECK(agree(s->ctx, rbt_reserve(s)));
+  s->factored = false;
+  return rbt_transform(s, stages);
+}
+
+extern "C" int hb_symdense_dist_rbt_stats(hb_symdense_dist* s, int* corrections, double* backward_error, float* transform_ms)
+{
+  HB_REQUIRE(s, "null handle");
+  if(corrections) *corrections = s->rbt_corr;
+  if(backward_error) *backward_error = s->rbt_berr;
+  if(transform_ms) *transform_ms = s->rbt_ms;
+  return HB_OK;
+}
+
 extern "C" int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode)
 {
   HB_REQUIRE(s, "null handle");
   if(mode == HB_FACT_BUNCH_KAUFMAN)
-    return hb_fail(HB_ERR_INVALID, "hb_symdense_dist_matrix_changed: Bunch-Kaufman is not distributed (its pivot search needs every column); use hb_symdense%s", "");
-  HB_REQUIRE(mode == HB_FACT_NOPIV || mode == HB_FACT_CHOLESKY, "hb_symdense_dist_matrix_changed: bad mode");
+    return hb_fail(HB_ERR_INVALID, "hb_symdense_dist_matrix_changed: Bunch-Kaufman is not distributed (its pivot search needs every column); use hb_symdense "
+                                   "or HB_FACT_RBT_NOPIV%s", "");
+  HB_REQUIRE(mode == HB_FACT_NOPIV || mode == HB_FACT_CHOLESKY || mode == HB_FACT_RBT_NOPIV, "hb_symdense_dist_matrix_changed: bad mode");
   hb_ctx* c = s->ctx;
   const int N = s->N, P = s->P, rank = s->rank;
-  const bool ldl = mode == HB_FACT_NOPIV;
+  const bool ldl = mode != HB_FACT_CHOLESKY;
   s->mode = mode;
   s->factored = false;
   if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
   HB_CUDA(cudaSetDevice(c->device));
+  if(mode == HB_FACT_RBT_NOPIV) {
+    HB_CHECK(agree(c, rbt_reserve(s)));
+    HB_CHECK(rbt_transform(s, 2));
+  }
   cudaStream_t su = c->stream, sp = s->sp;
   const long long ld = s->ld;
   double* A = s->A;
@@ -397,29 +711,14 @@ extern "C" int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_
   return HB_OK;
 }
 
-extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
+// the forward and backward sweeps of the factor on the replicated row-major N x nrhs vectors xw, in place
+static int dist_sweeps(hb_symdense_dist* s, double* xw, int nrhs)
 {
-  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_dist_solve: bad arguments");
-  if(s->N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_dist_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_dist_solve: no valid factorization (call hb_symdense_dist_matrix_changed)%s", "");
   hb_ctx* c = s->ctx;
   const int N = s->N, P = s->P, rank = s->rank;
-  const bool ldl = s->mode == HB_FACT_NOPIV;
+  const bool ldl = s->mode != HB_FACT_CHOLESKY;
   const long long ld = s->ld;
   cudaStream_t st = c->stream;
-  HB_CUDA(cudaSetDevice(c->device));
-  auto reserve = [&]() -> int {
-    HB_CHECK(s->xw.reserve(c, (size_t)N * nrhs, "solve rows"));
-    HB_CHECK(s->ybuf.reserve(c, (size_t)DB * nrhs, "solve block"));
-    HB_CHECK(s->tdot.reserve(c, (size_t)DB * nrhs, "solve block products"));
-    return HB_OK;
-  };
-  HB_CHECK(agree(c, reserve()));
-  double* xw = s->xw;
-  const int tg = hb_grid(c, (long long)N * nrhs);
-  k_dist_to_rows<<<tg, 256, 0, st>>>(N, nrhs, x, xw, 0);
-  HB_LAUNCHED();
   const int ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
   for(int k = 0; k < s->nblk; k++) {
     const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb;
@@ -447,7 +746,97 @@ extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
     }
     HB_CHECK(hb_broadcast(c, xw + (size_t)k0 * nrhs, (long long)nb * nrhs, owner, st));
   }
+  return HB_OK;
+}
+
+// RBT solve on the row-major xw (b in, x out): b' = U^T b, the sweeps, refinement against A', x = U x'. The stopping rule reads only
+// replicated values (the residual is formed by the owner of each block row and broadcast), so every rank makes the same decisions.
+static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs)
+{
+  hb_ctx* c = s->ctx;
+  const int N = s->N, P = s->P, rank = s->rank, nrows = s->nloc * DB;
+  cudaStream_t st = c->stream;
+  const int tg = hb_grid(c, (long long)N * nrhs);
+  double *bp = s->rbt_b, *rw = s->rbt_r, *nrm = rw + (size_t)N * nrhs; // per rhs: max |r|, max |x'|, max |b'|
+  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, s->rbt_f, xw, rw, 1);
+  HB_LAUNCHED();
+  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 1, s->rbt_f, rw, bp, 1);
+  HB_LAUNCHED();
+  HB_CUDA(cudaMemcpyAsync(xw, bp, sizeof(double) * N * nrhs, cudaMemcpyDeviceToDevice, st));
+  HB_CHECK(dist_sweeps(s, xw, nrhs));
+  double om = 0.0, prev = INFINITY;
+  int corr = 0;
+  for(;;) {
+    if(nrows > 0) {
+      k_rbt_rows<<<nrows, 256, 0, st>>>(N, P, rank, s->Ak, s->ld, nrhs, xw, bp, rw);
+      HB_LAUNCHED();
+    }
+    for(int k = 0; k < s->nblk; k++) {
+      const int k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
+      HB_CHECK(hb_broadcast(c, rw + (size_t)k0 * nrhs, (long long)nb * nrhs, k % P, st));
+    }
+    k_rbt_max<<<nrhs, 256, 0, st>>>(N, nrhs, rw, xw, bp, nrm);
+    HB_LAUNCHED();
+    HB_CUDA(cudaMemcpyAsync(s->rbt_nrm_host, nrm, sizeof(double) * 3 * nrhs, cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaStreamSynchronize(st));
+    om = 0.0;
+    for(int q = 0; q < nrhs; q++) {
+      const double* m3 = s->rbt_nrm_host.get() + 3 * q;
+      const double den = s->rbt_anorm * m3[1] + m3[2];
+      const double w = den > 0.0 ? m3[0] / den : (m3[0] == 0.0 ? 0.0 : INFINITY);
+      om = (w > om || w != w) ? w : om;
+    }
+    if(!(corr < RBT_MAX_CORR && om > RBT_EPS && om <= 0.5 * prev)) break;
+    HB_CHECK(dist_sweeps(s, rw, nrhs));
+    k_rbt_axpy<<<tg, 256, 0, st>>>((long long)N * nrhs, rw, xw);
+    HB_LAUNCHED();
+    corr++;
+    prev = om;
+  }
+  s->rbt_corr = corr;
+  s->rbt_berr = om;
+  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 1, s->rbt_f, xw, rw, 0);
+  HB_LAUNCHED();
+  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, s->rbt_f, rw, xw, 0);
+  HB_LAUNCHED();
+  return std::isfinite(om) ? 1 : 0;
+}
+
+extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
+{
+  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_dist_solve: bad arguments");
+  if(s->N == 0 || nrhs == 0) return 1;
+  HB_REQUIRE(x, "hb_symdense_dist_solve: null rhs");
+  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_dist_solve: no valid factorization (call hb_symdense_dist_matrix_changed)%s", "");
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  const bool rbt = s->mode == HB_FACT_RBT_NOPIV;
+  cudaStream_t st = c->stream;
+  HB_CUDA(cudaSetDevice(c->device));
+  auto reserve = [&]() -> int {
+    HB_CHECK(s->xw.reserve(c, (size_t)N * nrhs, "solve rows"));
+    HB_CHECK(s->ybuf.reserve(c, (size_t)DB * nrhs, "solve block"));
+    HB_CHECK(s->tdot.reserve(c, (size_t)DB * nrhs, "solve block products"));
+    if(rbt) {
+      HB_CHECK(s->rbt_b.reserve(c, (size_t)N * nrhs, "transformed rhs"));
+      HB_CHECK(s->rbt_r.reserve(c, (size_t)N * nrhs + 3 * nrhs, "residual and norms"));
+      HB_CHECK(s->rbt_nrm_host.reserve(c, 3 * (size_t)nrhs, "norms"));
+    }
+    return HB_OK;
+  };
+  HB_CHECK(agree(c, reserve()));
+  double* xw = s->xw;
+  const int tg = hb_grid(c, (long long)N * nrhs);
+  k_dist_to_rows<<<tg, 256, 0, st>>>(N, nrhs, x, xw, 0);
+  HB_LAUNCHED();
+  int ok = 1;
+  if(rbt) {
+    ok = rbt_solve(s, xw, nrhs);
+    if(ok < 0) return ok;
+  } else {
+    HB_CHECK(dist_sweeps(s, xw, nrhs));
+  }
   k_dist_to_rows<<<tg, 256, 0, st>>>(N, nrhs, x, xw, 1);
   HB_LAUNCHED();
-  return 1;
+  return ok;
 }

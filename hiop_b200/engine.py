@@ -225,12 +225,13 @@ class _DeviceArray:
 
 
 class LinSolverSymDenseDist:
-    """The dense symmetric solver with the matrix factored across the context's ranks (hb_symdense_dist): Cholesky or no-pivot LDL^T
-    on a 1-D block-cyclic layout of 128-row blocks (sharding.block_rows). Every call is collective over the ranks; with one rank (no
+    """The dense symmetric solver with the matrix factored across the context's ranks (hb_symdense_dist): Cholesky, no-pivot LDL^T, or
+    (RBT_NOPIV, the safe mode) no-pivot LDL^T of a random butterfly transform U^T A U with refined solves, on a 1-D block-cyclic layout
+    of 128-row blocks (sharding.block_rows). Every call is collective over the ranks; with one rank (no
     init_comm) it runs on one GPU. matrixChanged(mode) returns what LinSolverSymDense.matrixChanged does, the same on every rank;
     solve(x) takes and returns x replicated on every rank."""
 
-    NOPIV, CHOLESKY = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY
+    NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
 
     def __init__(self, ctx: Context, n: int):
         self.ctx, self.n = ctx, n
@@ -265,8 +266,9 @@ class LinSolverSymDenseDist:
                 self._local[r:r + e - b, :self.n].copy_(M[b:e])
 
     def matrixChanged(self, mode: int) -> int:
-        if mode not in (self.NOPIV, self.CHOLESKY):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
-            raise EngineError("LinSolverSymDenseDist: Bunch-Kaufman is not distributed (its pivot search needs every column); use LinSolverSymDense")
+        if mode not in (self.NOPIV, self.CHOLESKY, self.RBT_NOPIV):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
+            raise EngineError("LinSolverSymDenseDist: Bunch-Kaufman is not distributed (its pivot search needs every column); use RBT_NOPIV "
+                              "for the safe mode, or LinSolverSymDense")
         rc = self.ctx.L.hb_symdense_dist_matrix_changed(self.h, mode)
         if rc < -1:
             check(rc, "hb_symdense_dist_matrix_changed")
@@ -289,6 +291,12 @@ class LinSolverSymDenseDist:
         ms = (ctypes.c_float * 3)()
         check(self.ctx.L.hb_symdense_dist_profile(self.h, int(on), ms), "hb_symdense_dist_profile")
         return None if on else tuple(float(v) for v in ms)
+
+    def rbt_stats(self):
+        """(corrections, backward error) of the last RBT solve and the transform time (ms; 0 unless profiling) of the last RBT factorization"""
+        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
+        check(self.ctx.L.hb_symdense_dist_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_dist_rbt_stats")
+        return n.value, be.value, float(ms.value)
 
 
 class KKTLinSysLowRank:
@@ -593,6 +601,18 @@ class KKTLinSysCompressedMDSXYcYd:
         args = (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd)
         self._keep["blk"] = args
         check(self.ctx.L.hb_mds_build_kkt_matrix_dist(self.h, *[_ptr(t) for t in args], dist.h), "hb_mds_build_kkt_matrix_dist")
+
+    def factorizeWithCurvCheck_dist(self, dist: LinSolverSymDenseDist, safe_mode: bool) -> int:
+        """factorizeWithCurvCheck on dist (filled by build_kkt_matrix_dist): the random-butterfly LDL^T in safe mode (HiOp's stable
+        linsol_mode), the no-pivot LDL^T otherwise, plus the inertia of the sparse block (Haynsworth); the same value on every rank"""
+        n_neg = dist.matrixChanged(dist.RBT_NOPIV if safe_mode else dist.NOPIV)
+        if n_neg < 0:
+            return -1
+        a, b = ctypes.c_int(), ctypes.c_int()
+        check(self.ctx.L.hb_mds_hxs_inertia(self.h, ctypes.byref(a), ctypes.byref(b)), "hb_mds_hxs_inertia")
+        if b.value > 0:
+            return -1
+        return n_neg + a.value
 
     def solveCompressed_dist(self, dist: LinSolverSymDenseDist, rx, ryc, ryd, dx, dyc, dyd) -> bool:
         """solveCompressed around dist (factored with dist.matrixChanged); the outputs are replicated on every rank"""

@@ -169,6 +169,7 @@ int hb_mat_add_upper_to_sym_upper(hb_ctx*, int n, const double* A, long long lda
 #define HB_FACT_BUNCH_KAUFMAN 0 /* pivoted LDL^T (DSYTRF / magma_dsytrf_gpu semantics), inertia from 1x1/2x2 pivots */
 #define HB_FACT_NOPIV 1         /* LDL^T without pivoting (magma_dsytrf_nopiv_gpu, linsol_mode=speculative) */
 #define HB_FACT_CHOLESKY 2      /* LL^T for SPD systems (DPOTRF; duals LSQ + condensed QN system) */
+#define HB_FACT_RBT_NOPIV 3     /* random butterfly transform, LDL^T without pivoting, refinement (hb_symdense_dist only; linsol_mode=stable) */
 
 int hb_symdense_create(hb_ctx* ctx, int N, hb_symdense** out);
 int hb_symdense_destroy(hb_symdense* s);
@@ -211,7 +212,8 @@ int hb_debug_condensed_solve(hb_ctx* ctx, int N, const double* Nfact, const doub
 
 /* ---- the same system factored across the ranks of the context's communicator (hb_symdense_dist.cu) ----
  * 1-D block-cyclic layout with block size 128: block row k (rows k*128 .. min(N, k*128+128)-1 of the N x N row-major matrix, full
- * width) belongs to rank k mod P. Cholesky and no-pivot LDL^T only (Bunch-Kaufman's pivot search needs every column: use hb_symdense).
+ * width) belongs to rank k mod P. Cholesky, no-pivot LDL^T and its random-butterfly safe mode (Bunch-Kaufman's pivot search needs every
+ * column: use hb_symdense, or HB_FACT_RBT_NOPIV).
  * Every call is collective: all ranks make the same calls in the same order. Without hb_comm_init, P = 1 and the handle works on one GPU.
  * The factor is bit-identical to hb_symdense's look-ahead factorization with unpaired blocks (HB_DENSE_PAIR_MIN above N), for every P.
  * create refuses on every rank (HB_ERR_INVALID) when the ranks pass different N, and with HB_ERR_COMM when P > 1 and NCCL has no
@@ -225,11 +227,30 @@ int hb_symdense_dist_local(hb_symdense_dist* s, double** A_local, long long* ld,
 /* the order N of the handle (-1 for NULL) */
 int hb_symdense_dist_order(hb_symdense_dist* s);
 /* factorizes in place; the same return value on every rank, with the meaning of hb_symdense_matrix_changed (>= 0: number of negative
- * eigenvalues, -1: null pivot or breakdown). HB_ERR_INVALID for HB_FACT_BUNCH_KAUFMAN (the handle stays usable). */
+ * eigenvalues, -1: null pivot or breakdown). HB_ERR_INVALID for HB_FACT_BUNCH_KAUFMAN (the handle stays usable).
+ * HB_FACT_RBT_NOPIV (the safe mode): A' = U^T A U with U = B2 B1 a depth-2 random butterfly (B1 of order N, B2 = diag of two of orders
+ * ceil(N/2) and floor(N/2); random diagonals in [15/16, 17/16) drawn from N and a fixed seed only, never from P), then the no-pivot LDL^T
+ * of A'. U is nonsingular, so the inertia of A' (the return value, hb_symdense_dist_inertia) is that of A; mixing every row with its
+ * butterfly partners lets the no-pivot factorization take KKT matrices with zero or indefinite diagonal entries. A' and the factor are
+ * the same bits for every P (oracle/rbt_model.py restates every entry). The transform needs both triangles of every row and rows of other
+ * ranks: the upper triangle is mirrored into the lower part through one broadcast of every block row, and each butterfly level
+ * broadcasts every block row again unless all partners are local (P = 1, or the pairing distances are multiples of 128 P). A' is kept
+ * for the refinement: the first RBT factorization allocates a second copy of the owned block rows (the handle's device memory doubles),
+ * 2 N butterfly diagonals and N / P row sums; a handle that never sees this mode allocates none of it. */
 int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode);
 int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_null, int* n_pos);
-/* x: N x nrhs (one rhs after the other, device), replicated on every rank in and out. 1 / 0 / HB_ERR_* like hb_symdense_solve. */
+/* x: N x nrhs (one rhs after the other, device), replicated on every rank in and out. 1 / 0 / HB_ERR_* like hb_symdense_solve.
+ * After HB_FACT_RBT_NOPIV: b' = U^T b, the two sweeps of the factor, then refinement against the kept A' (the owner of each block row
+ * forms its rows of b' - A' x' in a fixed order and broadcasts them), x = U x'. Stopping rule, on values every rank holds alike:
+ * omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf); correct while omega > 2^-52, fewer than 3
+ * corrections were made and omega is at most half its value before the last correction. Returns 0 when omega is not finite. */
 int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs);
+/* the last RBT solve's corrections and omega (above), and the last RBT factorization's mirror + butterfly time (ms, device events, only
+ * while hb_symdense_dist_profile is on; 0 otherwise). Every output may be NULL. */
+int hb_symdense_dist_rbt_stats(hb_symdense_dist* s, int* corrections, double* backward_error, float* transform_ms);
+/* diagnostics (tests): the first `stages` steps of the RBT transform on the owned block rows, in place and without factoring (collective;
+ * 0: the mirrored full rows, 1: B2^T A B2, 2: A'); the handle then holds no factorization. */
+int hb_debug_symdense_dist_rbt(hb_symdense_dist* s, int stages);
 /* diagnostics (tools/bench_dist_symdense.py): on != 0 times the phases of every following factorization with device events; on == 0
  * stops and returns this rank's sums (ms) over the steps of the last one: panel chain (owner's k_diag128 + k_trsm_panel + packing),
  * broadcast (including the wait for the owner), trailing update on the update stream. ms3 may be NULL. */

@@ -6,9 +6,11 @@
 Prints one JSON line per (N, mode, P) from rank 0: factor and solve ms (device events, maximum over ranks, after warm-up), N^3/3 over
 the factor time, the bytes one factorization broadcasts (from the shapes), the per-phase sums of one profiled factorization (maximum
 over ranks: panel chain, broadcast including the wait for the owner, trailing update), hb_symdense's time on the same matrix on rank 0
-with its default dispatch and with its blocks never paired (K = 128 updates), max |x_dist - x_single| / |x|, and the card's name and power limit. Then one line for a mixed dense-sparse
-step in speculative mode (no-pivot LDL^T: update + build + factor + solve) at bench.py's MDS size, distributed against the replicated
-single-GPU step, with the residual of the uncondensed system (must be <= 1e-8)."""
+with its default dispatch and with its blocks never paired (K = 128 updates), max |x_dist - x_single| / |x|, and the card's name and power limit.
+Mode rbt (the safe mode, HB_FACT_RBT_NOPIV) adds the transform time of one profiled factorization, the corrections and backward error of
+the refined solve, and whether its inertia equals hb_symdense's Bunch-Kaufman on rank 0 on the same matrix. Then one line each for a mixed
+dense-sparse step in speculative mode (no-pivot LDL^T) and in stable mode (RBT; update + build + factor + solve) at bench.py's MDS size,
+distributed against the replicated single-GPU step, with the residual of the uncondensed system (must be <= 1e-8)."""
 import argparse
 import json
 import os
@@ -21,7 +23,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CHOL, NOPIV = 2, 1
+CHOL, NOPIV, RBT, BK = 2, 1, 3, 0
 BLOCK, HDR = 128, 136   # hb_symdense_dist.cu: block size, broadcast header (doubles)
 
 
@@ -173,8 +175,11 @@ def main():
                                   "phase_ms_max_over_ranks": {"panel_chain": phases[0], "broadcast": phases[1], "trailing_update": phases[2]},
                                   "single_gpu_hb_symdense_rank0": single, **info}), flush=True)
 
+        run_rbt(N, ctx, world, rank, rmax, timed, info)
+
     if not args.no_mds:
         run_mds(args, ctx, world, rank, rmax, timed, info)
+        run_mds(args, ctx, world, rank, rmax, timed, info, stable=True)
     if ctx_k128:
         ctx_k128.close()
     ctx.close()
@@ -182,7 +187,54 @@ def main():
         dist.destroy_process_group()
 
 
-def run_mds(args, ctx, world, rank, rmax, timed, info):
+def run_rbt(N, ctx, world, rank, rmax, timed, info):
+    """the safe mode on the no-pivot matrix of make_matrix: factor and solve ms, transform ms, corrections, backward error, inertia check"""
+    from hiop_b200.engine import LinSolverSymDense, LinSolverSymDenseDist
+    dev = ctx.device
+    M = make_matrix(NOPIV, N, dev, seed=N + RBT)
+    b = torch.randn(N, generator=torch.Generator(device=dev).manual_seed(7), dtype=torch.float64, device=dev)
+    torch.cuda.synchronize()
+    s = LinSolverSymDenseDist(ctx, N)
+    x = torch.empty_like(b)
+
+    def factor():
+        s.set_matrix(M)
+        rc = s.matrixChanged(RBT)
+        assert rc == N // 3, rc
+    copy_ms = timed(lambda: s.set_matrix(M), 1)
+    factor()
+    f_ms = timed(factor, 3) - copy_ms
+    s.profile(True)
+    factor()
+    s.profile(False)
+    transform_ms = s.rbt_stats()[2]
+    inertia = s.inertia()
+
+    def solve():
+        with torch.cuda.stream(ctx.stream):
+            x.copy_(b)
+        assert s.solve(x)
+    solve()
+    s_ms = timed(solve, 3)
+    corr, berr, _ = s.rbt_stats()
+    s.close()
+    f_ms, s_ms, transform_ms = rmax(f_ms), rmax(s_ms), rmax(transform_ms)
+    same = None
+    if rank == 0:
+        ss = LinSolverSymDense(ctx, N, BK)
+        ss.set_matrix(M)
+        rc_bk = ss.matrixChanged()
+        same = rc_bk == N // 3 and ss.inertia() == inertia
+        ss.close()
+    del M
+    torch.cuda.empty_cache()
+    if rank == 0:
+        print(json.dumps({"N": N, "mode": "rbt", "P": world, "factor_ms": f_ms, "solve_ms": s_ms, "transform_ms": transform_ms,
+                          "corrections": corr, "backward_error": berr, "inertia": list(inertia), "inertia_equals_bunch_kaufman_rank0": same,
+                          **info}), flush=True)
+
+
+def run_mds(args, ctx, world, rank, rmax, timed, info, stable=False):
     import bench
     from hiop_b200.engine import KKTLinSysCompressedMDSXYcYd, LinSolverSymDenseDist
     nxs, nxd, m = args.mds_ns, args.mds_nd, args.mds_m
@@ -202,7 +254,10 @@ def run_mds(args, ctx, world, rank, rmax, timed, info):
         def step_dist():
             k.update(T["zl"], T["sxl"], T["zu"], T["sxu"], T["ixl"], T["ixu"])
             k.build_kkt_matrix_dist(s, *blocks)
-            assert s.matrixChanged(NOPIV) == neq + nineq
+            if stable:
+                assert k.factorizeWithCurvCheck_dist(s, safe_mode=True) == neq + nineq
+            else:
+                assert s.matrixChanged(NOPIV) == neq + nineq
             assert k.solveCompressed_dist(s, T["rx"], T["ryc"], T["ryd"], dx, dyc, dyd)
         for _ in range(max(args.warmup, 1)):
             step_dist()
@@ -212,6 +267,11 @@ def run_mds(args, ctx, world, rank, rmax, timed, info):
         s.close()
         single = None
         if rank == 0:
+            if stable:       # the single-GPU stable step: Bunch-Kaufman
+                k.close()
+                k = KKTLinSysCompressedMDSXYcYd(ctx, nxs, nxd, neq, nineq, safe_mode=True)
+                k.set_sparsity(T["iRc"], T["jCc"], T["iRd"], T["jCd"])
+
             def step_single():
                 k.update(T["zl"], T["sxl"], T["zu"], T["sxu"], T["ixl"], T["ixu"])
                 k.build_kkt_matrix(*blocks)
@@ -224,7 +284,7 @@ def run_mds(args, ctx, world, rank, rmax, timed, info):
         k.close()
     assert resid <= 1e-8, resid
     if rank == 0:
-        print(json.dumps({"workload": f"mds speculative step n_s={nxs} n_d={nxd} m={m} (N={N})", "P": world, "ms_per_step": ms,
+        print(json.dumps({"workload": f"mds {'stable' if stable else 'speculative'} step n_s={nxs} n_d={nxd} m={m} (N={N})", "P": world, "ms_per_step": ms,
                           "kkt_residual_rel_independent_operators": resid, "single_gpu_replicated_step_rank0": single, **info}), flush=True)
 
 
