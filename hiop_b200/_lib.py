@@ -63,6 +63,7 @@ def lib() -> ctypes.CDLL:
     f("hb_ctx_device", c_i, c_vp)
     f("hb_ctx_enable_timing", c_i, c_vp, c_i)
     f("hb_ctx_last_syrk_ms", c_i, c_vp, P(ctypes.c_float))
+    f("hb_syrk_schedule_view", c_i, c_i, c_ll, c_i, c_i, P(c_i), c_vp, c_vp)
     f("hb_malloc", c_i, c_vp, ctypes.c_size_t, P(c_vp))
     f("hb_free", c_i, c_vp, c_vp)
     f("hb_malloc_host", c_i, c_vp, ctypes.c_size_t, P(c_vp))

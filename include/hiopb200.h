@@ -71,6 +71,13 @@ int hb_ctx_enable_timing(hb_ctx* ctx, int on);
 int hb_ctx_phase_timeline(hb_ctx* ctx, int on, float* ms_host10);
 int hb_ctx_last_syrk_ms(hb_ctx* ctx, float* ms_host);
 
+/* The work schedule of the FP64 DMMA SYRK (k_syrk_ws) for M rows (the fused rhs row included), K columns and G SMs, built on the host
+ * (no device needed). *nslots receives the number of workspace slots; the first min(cap, *nslots) slots s are described by
+ * slots_host[5s .. 5s+4] = {CTA, tile row, tile column, first K chunk, K chunk count} (chunks of 32 columns, tiles of 128 rows) and by
+ * frags_host[128s .. 128s+127]: how many times the CTA computes each m16n8 fragment (16-row block r, 8-column block c at 16r + c) of
+ * the tile per 16 columns of K. k_syrk_fixup sums the slots of a tile in increasing s. */
+int hb_syrk_schedule_view(int M, long long K, int G, int cap, int* nslots, long long* slots_host, unsigned char* frags_host);
+
 /* Measured roofline denominators of this device (a few milliseconds each, CUDA events on the context stream):
  * which = 0: FP64 tensor pipe, mma.sync.m8n8k4.f64 issued back to back from registers (TFLOP/s; SASS DMMA.8x8x4, half the rate of 2);
  * which = 1: wgmma.mma_async m64n256k32 s8 issued back to back by two warpgroups per SM on resident operands (TOP/s, 2 ops per MAC);
