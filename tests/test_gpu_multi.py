@@ -5,19 +5,27 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 from hiop_b200 import sharding, synth
 from oracle import kkt_oracle as ko
+from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu
 
 
-def _worker(rank, world, uid, n, m, l, out):
-    from hiop_b200.engine import Context, KKTLinSysLowRank
+def _worker(rank, world, uid, out, n, m, l):
+    from hiop_b200.engine import Context
     torch.cuda.set_device(rank)
     ctx = Context(rank)
-    ctx.init_comm(world, rank, uid)
+    try:
+        ctx.init_comm(world, rank, uid)
+        _run(ctx, rank, world, n, m, l, out)
+    finally:
+        ctx.close()
+
+
+def _run(ctx, rank, world, n, m, l, out):
+    from hiop_b200.engine import KKTLinSysLowRank
     P = synth.make_qn_problem(n, m, l, seed=77)
     b, e = sharding.column_range(n, world, rank)
     sl = slice(b, e)
@@ -64,20 +72,11 @@ def _worker(rank, world, uid, n, m, l, out):
     ctx.sync()
     out[f"lsq{rank}"] = np.concatenate([yc.cpu().numpy(), yd.cpu().numpy()])
     k.close()
-    ctx.close()
 
 
 @pytest.mark.parametrize("n,m,l", [(40001, 70, 6), (9000, 140, 0)])
 def test_two_gpu_sharded_matches_oracle(n, m, l):
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs")
-    from hiop_b200 import _lib
-    import ctypes
-    buf = ctypes.create_string_buffer(128)
-    _lib.check(_lib.lib().hb_comm_unique_id(buf), "hb_comm_unique_id")
-    mgr = mp.Manager()
-    out = mgr.dict()
-    mp.spawn(_worker, args=(2, buf.raw, n, m, l, out), nprocs=2, join=True)
+    out = run_ranks(_worker, 2, (n, m, l), comm="nccl")
     P = synth.make_qn_problem(n, m, l, seed=77)
     Dx, DhInv, Dd, Dd_inv = ko.kkt_update(P.zl, P.sxl, P.zu, P.sxu, P.ixl, P.ixu, P.vl, P.sdl, P.vu, P.sdu, P.idl, P.idu, P.sigma)
     st = ko.QnState(P.Jc, P.Jd, DhInv, Dd_inv, P.St, P.Yt, P.L, P.D, P.sigma)

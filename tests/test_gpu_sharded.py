@@ -9,8 +9,8 @@ Every output of a sharded run falls in one of three kinds, each checked without 
 End-to-end results are also held to the oracle. Two defects are pinned here: the adjusted-slack count must be the global one on every
 rank, and a failed LSQ factorization must leave the caller's multipliers untouched (on one GPU too).
 
-One spawn per world size runs every case; each rank writes arrays back through a manager, and a hung collective fails the test after
-a timeout with every rank terminated. Skipped when fewer than P GPUs are present."""
+One multirank.run_ranks call per world size runs every case; each rank writes arrays back through a manager, and a hung collective
+fails the test after a timeout with every rank terminated. Skipped when fewer than P GPUs are present."""
 import ctypes
 import functools
 import time
@@ -18,11 +18,11 @@ import time
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 from hiop_b200 import sharding, synth
 from oracle import bounds
 from oracle import kkt_oracle as ko
+from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -33,7 +33,6 @@ REPLICATED = ("N", "Z", "V", "p2l", "dy", "ir_info", "ir_m", "norms", "ftb", "fl
 COLUMN_LOCAL = ("gx", "step_n", "plh", "mtv_T", "kfull_elem")
 SUMMED = ("Caug", "SSt", "vec_dot", "vec_one", "vec_logbar", "mv")
 EXTREMAL = {"vec_inf": np.max, "vec_min": np.min, "vec_ftb": np.min}
-TIMEOUT = 900.0
 
 
 def _kkt_cases(world, num_sms):
@@ -255,7 +254,7 @@ def _run_case(ctx, case, world, rank, single):
     return (_run_kkt if case[0] == "kkt" else _run_secant)(ctx, case, world, rank, single)
 
 
-def _worker(rank, world, uid, cases, out):
+def _worker(rank, world, uid, out, cases):
     from hiop_b200.engine import Context
     torch.cuda.set_device(rank)
     ctx = Context(rank)
@@ -265,31 +264,6 @@ def _worker(rank, world, uid, cases, out):
             out[f"{name}/{rank}"] = _run_case(ctx, case, world, rank, single=False)
     finally:
         ctx.close()
-
-
-def _spawn(world, cases):
-    """{name: [rank 0's outputs, ...]} of one sharded run of every case; every rank is terminated on a failure or after TIMEOUT"""
-    uid = None
-    if world > 1:
-        from hiop_b200 import _lib
-        buf = ctypes.create_string_buffer(128)
-        _lib.check(_lib.lib().hb_comm_unique_id(buf), "hb_comm_unique_id")
-        uid = buf.raw
-    with mp.Manager() as mgr:
-        out = mgr.dict()
-        pc = mp.start_processes(_worker, args=(world, uid, cases, out), nprocs=world, join=False, start_method="spawn")
-        deadline = time.monotonic() + TIMEOUT
-        try:
-            while not pc.join(timeout=max(1.0, deadline - time.monotonic())):
-                if time.monotonic() >= deadline:
-                    raise TimeoutError(f"the {world} ranks did not finish within {TIMEOUT:.0f} s (a collective that never completed?)")
-        finally:
-            for p in pc.processes:
-                if p.is_alive():
-                    p.terminate()
-            for p in pc.processes:
-                p.join(30)
-        return {name: [out[f"{name}/{r}"] for r in range(world)] for name, _ in cases}
 
 
 def _singles(cases, world):
@@ -320,7 +294,8 @@ def _results(world):
         cases = _kkt_cases(world, torch.cuda.get_device_properties(0).multi_processor_count) + SECANT_CASES
         try:
             t0 = time.monotonic()
-            S = _spawn(world, cases)
+            out = run_ranks(_worker, world, (cases,), comm="nccl")
+            S = {name: [out[f"{name}/{r}"] for r in range(world)] for name, _ in cases}
             t1 = time.monotonic()
             G = _singles(cases, world)
             print(f"\nP = {world}: sharded run {t1 - t0:.1f} s, one-GPU shard runs {time.monotonic() - t1:.1f} s")

@@ -2,17 +2,17 @@
 bit for bit against hb_symdense's look-ahead path at K = 128 and across P, the backward-error bounds and inertia of
 test_gpu_symdense_paths.py, failure and misuse, and the mixed dense-sparse path on top of it.
 
-Single-rank cases run on one GPU. Multi-rank cases spawn one process per GPU (torch.multiprocessing, like test_gpu_multi.py) and skip
-when fewer GPUs are present."""
+Single-rank cases run on one GPU. Multi-rank cases spawn one process per GPU (multirank.run_ranks) and skip when fewer GPUs are
+present."""
 import ctypes
 
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 from hiop_b200 import sharding, synth
 from oracle import bounds
+from multirank import run_ranks
 
 CHOL, NOPIV, BK = 2, 1, 0
 ERR_INVALID, ERR_STATE = -1, -5                              # HB_ERR_* of include/hiopb200.h
@@ -324,57 +324,47 @@ def test_mds_dist_build_bit_identical_at_the_bench_sparse_shape(make_ctx):
 
 
 # ---- several ranks -------------------------------------------------------------------------------------------------------------------------
-def _rank_worker(rank, world, uid, cases, out):
+def _rank_worker(rank, world, uid, out, cases):
     from hiop_b200.engine import Context
     torch.cuda.set_device(rank)
     import os
     os.environ["HB_DENSE_PAIR_MIN"] = str(1 << 30)
     ctx = Context(rank)
-    ctx.init_comm(world, rank, uid)
-    for mode, N in cases:
-        M, _ = matrix(mode, N, seed=N + mode, device=ctx.device)
-        rc, inr, rows, sols = factor_dist(ctx, mode, M, [rhs(N, N, 1), rhs(N, N + 1, 3)])
-        out[(rank, mode, N)] = (rc, inr, rows, sols)
-    # failure on a block owned by rank 1: the same value on every rank, then an SPD matrix factors
-    from hiop_b200.engine import LinSolverSymDenseDist
-    N = 700
-    s = LinSolverSymDenseDist(ctx, N)
-    M, _ = matrix(CHOL, N, 3, ctx.device)
-    Mb = M.clone()
-    Mb[128 + 7, 128 + 7] = -1.0
-    s.set_matrix(Mb)
-    r1 = s.matrixChanged(CHOL)
-    s.set_matrix(M)
-    r2 = s.matrixChanged(CHOL)
-    s.close()
-    out[(rank, "fail")] = (r1, r2)
-    # the mixed dense-sparse path: this rank's rows of the distributed build, and the replicated solution
-    for name in MDS_SHAPES:
-        p = mds_problem(name)
-        dist = LinSolverSymDenseDist(ctx, p.nxd + p.neq + p.nineq)
-        _, rows, ret, ok, dx, dyc, dyd = mds_run(ctx, p, dist)
-        dist.close()
-        out[(rank, "mds", name)] = (rows, ret, ok, dx, dyc, dyd)
-    ctx.close()
-
-
-def _spawn(world, cases):
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    from hiop_b200 import _lib
-    buf = ctypes.create_string_buffer(128)
-    _lib.check(_lib.lib().hb_comm_unique_id(buf), "hb_comm_unique_id")
-    mgr = mp.Manager()
-    out = mgr.dict()
-    mp.spawn(_rank_worker, args=(world, buf.raw, cases, out), nprocs=world, join=True)
-    return dict(out)
+    try:
+        ctx.init_comm(world, rank, uid)
+        for mode, N in cases:
+            M, _ = matrix(mode, N, seed=N + mode, device=ctx.device)
+            rc, inr, rows, sols = factor_dist(ctx, mode, M, [rhs(N, N, 1), rhs(N, N + 1, 3)])
+            out[(rank, mode, N)] = (rc, inr, rows, sols)
+        # failure on a block owned by rank 1: the same value on every rank, then an SPD matrix factors
+        from hiop_b200.engine import LinSolverSymDenseDist
+        N = 700
+        s = LinSolverSymDenseDist(ctx, N)
+        M, _ = matrix(CHOL, N, 3, ctx.device)
+        Mb = M.clone()
+        Mb[128 + 7, 128 + 7] = -1.0
+        s.set_matrix(Mb)
+        r1 = s.matrixChanged(CHOL)
+        s.set_matrix(M)
+        r2 = s.matrixChanged(CHOL)
+        s.close()
+        out[(rank, "fail")] = (r1, r2)
+        # the mixed dense-sparse path: this rank's rows of the distributed build, and the replicated solution
+        for name in MDS_SHAPES:
+            p = mds_problem(name)
+            dist = LinSolverSymDenseDist(ctx, p.nxd + p.neq + p.nineq)
+            _, rows, ret, ok, dx, dyc, dyd = mds_run(ctx, p, dist)
+            dist.close()
+            out[(rank, "mds", name)] = (rows, ret, ok, dx, dyc, dyd)
+    finally:
+        ctx.close()
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("world,cases", [(2, [(CHOL, 4099), (NOPIV, 4099)]), (4, [(CHOL, 1000), (NOPIV, 1000), (CHOL, 300), (NOPIV, 300)])],
                          ids=["p2", "p4"])
 def test_ranks_match_one_rank_bit_for_bit(make_ctx, world, cases):
-    out = _spawn(world, cases)
+    out = run_ranks(_rank_worker, world, (cases,), comm="nccl")
     ctx = make_ctx(HB_DENSE_PAIR_MIN=1 << 30)
     for mode, N in cases:
         M, _ = matrix(mode, N, seed=N + mode, device=ctx.device)

@@ -3,20 +3,19 @@ oracle/rbt_model.py, its factor bit for bit against hb_symdense's no-pivot facto
 Bunch-Kaufman, the refined solve, failure and resources, the mixed dense-sparse step in stable mode, and P = 2, 4 against P = 1.
 
 Single-rank cases run on one GPU. Multi-rank cases spawn one process per GPU and skip when fewer GPUs are present."""
-import ctypes
 from types import SimpleNamespace
 import pathlib
 
 import numpy as np
 import pytest
 import torch
-import torch.multiprocessing as mp
 
 from hiop_b200 import sharding, synth
 from oracle import bounds
 from oracle import rbt_model as rbt
 from test_cpu_rbt_model import FAMILIES
 from test_gpu_symdense_dist import K128, local_rows, upper_nan, factor_single, same_rows, factor_parts_from_rows
+from multirank import run_ranks
 
 RBT, NOPIV, CHOL, BK = 3, 1, 2, 0
 GOLDEN = pathlib.Path(__file__).parent / "golden"
@@ -274,30 +273,20 @@ def _case(N):
     return A, np.random.default_rng(N).standard_normal((N, 2))
 
 
-def _rank_worker(rank, world, uid, sizes, out):
+def _rank_worker(rank, world, uid, out, sizes):
     import os
     from hiop_b200.engine import Context
     torch.cuda.set_device(rank)
     os.environ["HB_DENSE_PAIR_MIN"] = str(1 << 30)
     ctx = Context(rank)
-    ctx.init_comm(world, rank, uid)
-    for N in sizes:
-        A, b = _case(N)
-        rc, inr, rows, x, stats = rbt_dist(ctx, A, b)
-        out[(rank, N)] = (rc, inr, rows, x, stats[0])
-    ctx.close()
-
-
-def _spawn(world, sizes):
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    from hiop_b200 import _lib
-    buf = ctypes.create_string_buffer(128)
-    _lib.check(_lib.lib().hb_comm_unique_id(buf), "hb_comm_unique_id")
-    mgr = mp.Manager()
-    out = mgr.dict()
-    mp.spawn(_rank_worker, args=(world, buf.raw, sizes, out), nprocs=world, join=True)
-    return dict(out)
+    try:
+        ctx.init_comm(world, rank, uid)
+        for N in sizes:
+            A, b = _case(N)
+            rc, inr, rows, x, stats = rbt_dist(ctx, A, b)
+            out[(rank, N)] = (rc, inr, rows, x, stats[0])
+    finally:
+        ctx.close()
 
 
 @pytest.mark.gpu
@@ -305,7 +294,7 @@ def _spawn(world, sizes):
 def test_ranks_match_one_rank_bit_for_bit(make_ctx, world, sizes):
     """every owned row of the factor, the inertia, the solution and the number of corrections are those of P = 1; at N = 300 and P = 4
     rank 3 owns no block and still takes part in every collective"""
-    out = _spawn(world, sizes)
+    out = run_ranks(_rank_worker, world, (sizes,), comm="nccl")
     ctx = make_ctx(HB_DENSE_PAIR_MIN=1 << 30)
     for N in sizes:
         A, b = _case(N)
