@@ -118,27 +118,17 @@ __device__ __forceinline__ double mds_entry(const MdsBuildArgs& a, int r, int c)
   return v;
 }
 
-__global__ void __launch_bounds__(T) k_mds_build(const MdsBuildArgs a, double* __restrict__ M)
+// The upper-triangle entries of the first `rows` rows one rank owns in hb_symdense_dist's block-cyclic layout: local row lr holds
+// global row (lr / 128 * P + rank) * 128 + lr % 128, ld doubles per row. P = 1, rank = 0, ld = rows = N is the N x N matrix.
+// `rows` must not reach past global row N - 1.
+__global__ void __launch_bounds__(T) k_mds_build(const MdsBuildArgs a, int P, int rank, int rows, double* __restrict__ M, long long ld)
 {
   const int N = a.nxd + a.neq + a.nineq;
-  const long long total = (long long)N * N;
-  for(long long e = (long long)blockIdx.x * T + threadIdx.x; e < total; e += (long long)gridDim.x * T) {
-    const int r = (int)(e / N), c = (int)(e % N);
-    if(c < r) continue;
-    M[(size_t)r * N + c] = mds_entry(a, r, c);
-  }
-}
-
-// the same entries for the block rows one rank owns in hb_symdense_dist's block-cyclic layout: local row e holds global row
-// (e / 128 * P + rank) * 128 + e % 128, ld doubles per row
-__global__ void __launch_bounds__(T) k_mds_build_dist(const MdsBuildArgs a, int P, int rank, int nloc, double* __restrict__ M, long long ld)
-{
-  const int N = a.nxd + a.neq + a.nineq;
-  const long long total = (long long)nloc * 128 * N;
+  const long long total = (long long)rows * N;
   for(long long e = (long long)blockIdx.x * T + threadIdx.x; e < total; e += (long long)gridDim.x * T) {
     const int lr = (int)(e / N), c = (int)(e % N);
     const int r = (lr / 128 * P + rank) * 128 + lr % 128;
-    if(r >= N || c < r) continue;
+    if(c < r) continue;
     M[(size_t)lr * ld + c] = mds_entry(a, r, c);
   }
 }
@@ -317,7 +307,7 @@ extern "C" int hb_mds_build_kkt_matrix(hb_mds* h, const double* Hd, const double
   hb_ctx* c = h->ctx;
   const int N = h->nxd + h->neq + h->nineq;
   if(N > 0) {
-    k_mds_build<<<hb_grid(c, (long long)N * N, T), T, 0, c->stream>>>(a, Msys);
+    k_mds_build<<<hb_grid(c, (long long)N * N, T), T, 0, c->stream>>>(a, 1, 0, N, Msys, N);
     HB_LAUNCHED();
   }
   h->built = true;
@@ -340,7 +330,9 @@ extern "C" int hb_mds_build_kkt_matrix_dist(hb_mds* h, const double* Hd, const d
   HB_CHECK(mds_prepare(h, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd, &a));
   hb_ctx* c = h->ctx;
   if(nloc > 0) {
-    k_mds_build_dist<<<hb_grid(c, (long long)nloc * 128 * N, T), T, 0, c->stream>>>(a, c->nranks, c->rank, nloc, M, ld);
+    // every owned block has 128 rows but the matrix's last one
+    const int last = ((nloc - 1) * c->nranks + c->rank) * 128, rows = (nloc - 1) * 128 + std::min(128, N - last);
+    k_mds_build<<<hb_grid(c, (long long)rows * N, T), T, 0, c->stream>>>(a, c->nranks, c->rank, rows, M, ld);
     HB_LAUNCHED();
   }
   h->built = true;

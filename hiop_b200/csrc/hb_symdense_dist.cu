@@ -314,8 +314,6 @@ __global__ void __launch_bounds__(256) k_rbt_rows(int N, int P, int rank, const 
   }
 }
 
-__device__ __forceinline__ double rbt_nanmax(double m, double v) { return (v > m || v != v) ? v : m; }
-
 // one CTA per column c: out[c * 3 + k] = max_i |v_k(i, c)| over the N rows of the row-major N x ncols arrays v_0, v_1, v_2 (0 for an
 // absent one), NaN kept, in a fixed order
 __global__ void __launch_bounds__(256) k_rbt_max(int N, int ncols, const double* __restrict__ v0, const double* __restrict__ v1, const double* __restrict__ v2,
@@ -327,20 +325,15 @@ __global__ void __launch_bounds__(256) k_rbt_max(int N, int ncols, const double*
   for(int k = 0; k < 3; k++) {
     double m = 0.0;
     if(v[k])
-      for(int i = threadIdx.x; i < N; i += 256) m = rbt_nanmax(m, fabs(v[k][(size_t)i * ncols + c]));
+      for(int i = threadIdx.x; i < N; i += 256) m = hb_nan_max(m, fabs(v[k][(size_t)i * ncols + c]));
     sm[k][threadIdx.x] = m;
   }
   __syncthreads();
   if(threadIdx.x < 3) {
     double m = 0.0;
-    for(int t = 0; t < 256; t++) m = rbt_nanmax(m, sm[threadIdx.x][t]);
+    for(int t = 0; t < 256; t++) m = hb_nan_max(m, sm[threadIdx.x][t]);
     out[(size_t)c * 3 + threadIdx.x] = m;
   }
-}
-
-__global__ void k_rbt_axpy(long long n, const double* __restrict__ d, double* __restrict__ x)
-{
-  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) x[e] += d[e];
 }
 
 enum { PH_PANEL = 0, PH_BCAST, PH_UPDATE, PH_COUNT };
@@ -788,8 +781,7 @@ static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs)
     }
     if(!(corr < RBT_MAX_CORR && om > RBT_EPS && om <= 0.5 * prev)) break;
     HB_CHECK(dist_sweeps(s, rw, nrhs));
-    k_rbt_axpy<<<tg, 256, 0, st>>>((long long)N * nrhs, rw, xw);
-    HB_LAUNCHED();
+    HB_CHECK(hb_vec_axpy(c, (long long)N * nrhs, xw, 1.0, rw));
     corr++;
     prev = om;
   }

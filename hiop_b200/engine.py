@@ -572,14 +572,12 @@ class KKTLinSysCompressedMDSXYcYd:
         self._keep["it"] = (zl, sxl, zu, sxu, ixl, ixu)
         check(self.ctx.L.hb_mds_update(self.h, *[_ptr(t) for t in (zl, sxl, zu, sxu, ixl, ixu)]), "hb_mds_update")
 
-    def build_kkt_matrix(self, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd):
-        args = (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd)
-        self._keep["blk"] = args
-        check(self.ctx.L.hb_mds_build_kkt_matrix(self.h, *[_ptr(t) for t in args], ctypes.c_void_p(self.linSys._mptr)), "hb_mds_build_kkt_matrix")
+    def _build(self, name, blocks, target):
+        self._keep["blk"] = blocks
+        check(getattr(self.ctx.L, name)(self.h, *[_ptr(t) for t in blocks], target), name)
 
-    def factorizeWithCurvCheck(self) -> int:
-        """Number of negative eigenvalues of the whole XYcYd system via Haynsworth additivity, or -1 (:78-110)."""
-        n_neg = self.linSys.matrixChanged()
+    def _with_hxs_inertia(self, n_neg: int) -> int:
+        """n_neg of the dense factor plus the negative count of the eliminated sparse block (Haynsworth additivity), or -1"""
         if n_neg < 0:
             return -1
         a, b = ctypes.c_int(), ctypes.c_int()
@@ -588,39 +586,38 @@ class KKTLinSysCompressedMDSXYcYd:
             return -1
         return n_neg + a.value
 
-    def solveCompressed(self, rx, ryc, ryd, dx, dyc, dyd) -> bool:
-        rc = self.ctx.L.hb_mds_solve_compressed(self.h, self.linSys.h, *[_ptr(t) for t in (rx, ryc, ryd, dx, dyc, dyd)])
+    def _solve(self, name, solver, vecs) -> bool:
+        rc = getattr(self.ctx.L, name)(self.h, solver, *[_ptr(t) for t in vecs])
         if rc == -4:
             return False
-        check(rc, "hb_mds_solve_compressed")
+        check(rc, name)
         return True
+
+    def build_kkt_matrix(self, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd):
+        self._build("hb_mds_build_kkt_matrix", (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc,
+                                                delta_cd), ctypes.c_void_p(self.linSys._mptr))
+
+    def factorizeWithCurvCheck(self) -> int:
+        """Number of negative eigenvalues of the whole XYcYd system via Haynsworth additivity, or -1 (:78-110)."""
+        return self._with_hxs_inertia(self.linSys.matrixChanged())
+
+    def solveCompressed(self, rx, ryc, ryd, dx, dyc, dyd) -> bool:
+        return self._solve("hb_mds_solve_compressed", self.linSys.h, (rx, ryc, ryd, dx, dyc, dyd))
 
     def build_kkt_matrix_dist(self, dist: LinSolverSymDenseDist, Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx,
                               delta_wd, delta_cc, delta_cd):
         """build_kkt_matrix into the block rows this rank owns in `dist` (order nxd + neq + nineq); the inputs are replicated"""
-        args = (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd, delta_cc, delta_cd)
-        self._keep["blk"] = args
-        check(self.ctx.L.hb_mds_build_kkt_matrix_dist(self.h, *[_ptr(t) for t in args], dist.h), "hb_mds_build_kkt_matrix_dist")
+        self._build("hb_mds_build_kkt_matrix_dist", (Hd, Hs_diag, Jcd, Jdd, Jcs_vals, Jds_vals, vl, sdl, vu, sdu, idl, idu, delta_wx, delta_wd,
+                                                     delta_cc, delta_cd), dist.h)
 
     def factorizeWithCurvCheck_dist(self, dist: LinSolverSymDenseDist, safe_mode: bool) -> int:
         """factorizeWithCurvCheck on dist (filled by build_kkt_matrix_dist): the random-butterfly LDL^T in safe mode (HiOp's stable
         linsol_mode), the no-pivot LDL^T otherwise, plus the inertia of the sparse block (Haynsworth); the same value on every rank"""
-        n_neg = dist.matrixChanged(dist.RBT_NOPIV if safe_mode else dist.NOPIV)
-        if n_neg < 0:
-            return -1
-        a, b = ctypes.c_int(), ctypes.c_int()
-        check(self.ctx.L.hb_mds_hxs_inertia(self.h, ctypes.byref(a), ctypes.byref(b)), "hb_mds_hxs_inertia")
-        if b.value > 0:
-            return -1
-        return n_neg + a.value
+        return self._with_hxs_inertia(dist.matrixChanged(dist.RBT_NOPIV if safe_mode else dist.NOPIV))
 
     def solveCompressed_dist(self, dist: LinSolverSymDenseDist, rx, ryc, ryd, dx, dyc, dyd) -> bool:
         """solveCompressed around dist (factored with dist.matrixChanged); the outputs are replicated on every rank"""
-        rc = self.ctx.L.hb_mds_solve_compressed_dist(self.h, dist.h, *[_ptr(t) for t in (rx, ryc, ryd, dx, dyc, dyd)])
-        if rc == -4:
-            return False
-        check(rc, "hb_mds_solve_compressed_dist")
-        return True
+        return self._solve("hb_mds_solve_compressed_dist", dist.h, (rx, ryc, ryd, dx, dyc, dyd))
 
     def Msys(self) -> np.ndarray:
         N = self.nxd + self.neq + self.nineq
