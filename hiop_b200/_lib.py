@@ -126,6 +126,9 @@ def lib() -> ctypes.CDLL:
     f("hb_debug_diag128_profile", c_i, c_vp, c_i, P(c_ll))
     f("hb_debug_bk_profile", c_i, c_vp, c_i, P(c_ll))
     f("hb_debug_symdense_factor", c_i, c_vp, P(c_i), P(c_i), c_vp, c_vp, c_vp, c_vp)
+    f("hb_symdense_rbt_stats", c_i, c_vp, P(c_i), P(ctypes.c_double), P(ctypes.c_float))
+    f("hb_debug_symdense_rbt", c_i, c_vp, c_vp, c_vp)
+    f("hb_rbt_schedule_view", c_i, c_i, c_i, P(c_i), c_vp, c_vp, c_vp)
     f("hb_debug_condensed_solve", c_i, c_vp, c_i, c_vp, c_vp, c_i, c_vp, c_vp, c_d, c_i, *([c_vp] * 6))
     f("hb_symdense_dist_create", c_i, c_vp, c_i, P(c_vp))
     f("hb_symdense_dist_destroy", c_i, c_vp)

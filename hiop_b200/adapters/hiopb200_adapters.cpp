@@ -136,9 +136,11 @@ int hiopLinSolverSymDenseB200::matrixChanged()
   // never re-creates linSys_ when safe_mode flips (hiopKKTLinSysMDS.cpp:405-430 does so only under HIOP_USE_MAGMA), so a mode
   // frozen at construction would lose the reference's stability fallback.
   int mode = (safe_mode_ == nullptr || *safe_mode_) ? HB_FACT_BUNCH_KAUFMAN : HB_FACT_NOPIV;
-  const char* force = getenv("HIOP_B200_LINSOL"); // "bk" | "nopiv": overrides the safe_mode choice
+  // "bk" | "nopiv": overrides the safe_mode choice; "rbt": the random-butterfly safe mode wherever Bunch-Kaufman would run
+  const char* force = getenv("HIOP_B200_LINSOL");
   if(force && !strcmp(force, "bk")) mode = HB_FACT_BUNCH_KAUFMAN;
   if(force && !strcmp(force, "nopiv")) mode = HB_FACT_NOPIV;
+  if(force && !strcmp(force, "rbt") && mode == HB_FACT_BUNCH_KAUFMAN) mode = HB_FACT_RBT_NOPIV;
   nlp_->runStats.linsolv.tmFactTime.start();
   // M_ lives in host memory (mem_space=default): upload + factorize (the MAGMA twin does the same H2D per factorization,
   // hiopLinSolverSymDenseMagma.cpp:139-146)

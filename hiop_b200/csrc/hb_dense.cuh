@@ -1,6 +1,7 @@
 // Internal API of the dense symmetric factorizations / solves on device: the device helpers their kernel files share, the entry points
 // of each kernel file (each runs one path, no fall-back), and the per-caller dispatch of hb_symdense.cu that chooses between them.
 #pragma once
+#include <functional>
 #include "hb_common.cuh"
 
 // ---- device helpers ----
@@ -142,3 +143,77 @@ int hb_bkc_profile(hb_ctx* c, int on, long long* prof_host8);
 // (1x1 / 2x2 blocks marked by ipiv, off-diagonal in dsub), or of a Cholesky / no-pivot LDL^T factor (signs of the diagonal)
 int hb_dense_inertia_blockdiag(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, int* out3_dev);
 int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev);
+
+// ---- random butterfly transform (HB_FACT_RBT_NOPIV, hb_rbt.cu): A' = U^T A U, U = B2 B1, shared by hb_symdense and hb_symdense_dist ----
+// oracle/rbt_model.py states every expression; both handles produce the same bits of A', b' and x for a given N.
+constexpr double HB_RBT_C = 0.7071067811865476; // the double nearest 1/sqrt(2)
+constexpr double HB_RBT_EPS = 0x1p-52;          // refinement target of the backward error
+constexpr int HB_RBT_MAX_CORR = 3;
+constexpr int HB_DIST_DB = 128;                 // block size of the block-cyclic layout of hb_symdense_dist (rows of one block)
+
+// the entries of column i of a level's butterfly: rows lo and hi (lo = hi = i when unpaired), sign s of the hi side (+1 on the lo side)
+struct rbt_pos
+{
+  int lo, hi;
+  double s;
+  bool paired;
+};
+__host__ __device__ __forceinline__ rbt_pos rbt_at(int N, int level, int i)
+{
+  int o = 0, n = N;
+  if(level == 2) {
+    const int h = (N + 1) / 2;
+    if(i >= h) o = h, n = N - h;
+    else n = h;
+  }
+  const int hh = (n + 1) / 2, t = i - o;
+  if(t < n - hh) return {i, i + hh, 1.0, true};
+  if(t >= hh) return {i - hh, i, -1.0, true};
+  return {i, i, 1.0, false};
+}
+
+// out(i, j) of one level, B^T a B, from a(lo_i, lo_j), a(hi_i, hi_j), a(lo_i, hi_j), a(hi_i, lo_j): (f_i f_j) (t w) in the model's order
+__device__ __forceinline__ double rbt_entry(double all, double ahh, double alh, double ahl, const rbt_pos& pi, const rbt_pos& pj, double fi, double fj)
+{
+  const double ss = pi.s * pj.s;
+  double t, w;
+  if(pi.paired && pj.paired) {
+    t = __dadd_rn(__dadd_rn(all, __dmul_rn(ss, ahh)), __dadd_rn(__dmul_rn(pj.s, alh), __dmul_rn(pi.s, ahl)));
+    w = 0.5;
+  } else if(pi.paired || pj.paired) {
+    t = __dadd_rn(all, __dmul_rn(ss, ahh));
+    w = HB_RBT_C;
+  } else {
+    t = all;
+    w = 1.0;
+  }
+  return __dmul_rn(__dmul_rn(fi, fj), __dmul_rn(t, w));
+}
+
+// global row of local row y of rank `rank` in the block-cyclic layout (P = 1: y)
+__host__ __device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / HB_DIST_DB) * P + rank) * HB_DIST_DB + y % HB_DIST_DB; }
+
+// f[(level - 1) * N + i]: the diagonal entry of column i at level 1 (B1) and 2 (B2), a function of N alone (2 N doubles)
+int hb_rbt_table(hb_ctx* c, int N, double* f);
+// x (N x nrhs, one rhs after the other) -> xw (row-major N x nrhs), or back
+int hb_rbt_to_rows(hb_ctx* c, int N, int nrhs, double* x, double* xw, bool back);
+// rows of a row-major A' (full rows, ld; the nrows local rows of rank `rank` of P in the block-cyclic layout): x == NULL: out[y] =
+// sum_j |A'(y, j)| per local row y; else out[r * nrhs + q] = b'(r, q) - sum_j A'(r, j) x'(j, q) per global row r (x, b row-major)
+int hb_rbt_rows(hb_ctx* c, int N, int P, int rank, int nrows, const double* A, long long ld, int nrhs, const double* x, const double* b, double* out);
+// out[0] = max_i |v(i)| over n entries (NaN kept): ||A'||_inf from the row sums
+int hb_rbt_max1(hb_ctx* c, int n, const double* v, double* out);
+// The refined RBT solve on the row-major N x nrhs xw (b in, x out): b' = U^T b (kept in bp), sweeps(xw), then while the stopping rule
+// allows: residual(x', b', r) forms r = b' - A' x' in rw, sweeps(rw), x' += r; finally x = U x'. omega = max over the rhs of
+// ||r||_inf / (anorm ||x'||_inf + ||b'||_inf); correct while omega > HB_RBT_EPS, fewer than HB_RBT_MAX_CORR corrections were made and omega
+// is at most half its value before the last correction. rw: N nrhs + 3 nrhs doubles, nrm_host: 3 nrhs pinned doubles. Returns 1, 0 when
+// omega is not finite, or an HB_ERR_* code; *corr and *berr receive the corrections and the last omega.
+int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, double* xw, double* bp, double* rw, double* nrm_host,
+                 const std::function<int(double*)>& sweeps, const std::function<int(const double*, const double*, double*)>& residual, int* corr,
+                 double* berr);
+// One GPU: A' from the upper triangle of A (ld lda; the other triangle is not read) in one pass (k_rbt_fused): the upper triangle of A'
+// into F (ldf; may be A itself when hb_rbt_in_place(N), NULL for none), the full A' into Ak (ldk), ||A'||_inf into nrm_dev[0].
+// part: hb_rbt_part_doubles(N) doubles of row-sum scratch.
+bool hb_rbt_in_place(int N);
+size_t hb_rbt_part_doubles(int N);
+int hb_rbt_fused(hb_ctx* c, int N, const double* f, const double* A, long long lda, double* F, long long ldf, double* Ak, long long ldk, double* part,
+                 double* nrm_dev);

@@ -14,6 +14,7 @@
 //                 BK     < 96                              DSYTF2, one CTA                        DSYTRS                         serial, LAPACK ipiv
 //                 NOPIV  >= big_min_ldl (257)              look-ahead LDL^T (odd N: padded copy)  blocked                        parallel, diagonal
 //                 NOPIV  < big_min_ldl                     panels                                 blocked from 257, else one CTA parallel, diagonal
+//                 RBT    any                               k_rbt_fused (hb_rbt.cu), then NOPIV's   U^T, NOPIV's, refinement, U    NOPIV's
 //                 CHOL   >= big_min_chol (1025)            look-ahead (odd N: padded copy)        blocked                        parallel, diagonal
 //                 CHOL   65 .. 2048 and < big_min_chol     coop                                   blocked from 257, else one CTA parallel, diagonal
 //                 CHOL   other                             panels                                 blocked from 257, else one CTA parallel, diagonal
@@ -24,6 +25,8 @@
 //                 CHOL   other                             panels                                 one CTA
 //   V, Mdir       BK     any                               DSYTF2                                 DSYTRS
 //
+// RBT (safe mode) is NOPIV's plan on A' = U^T A U: the fused transform reads the upper triangle of M once and writes A' into the factor
+// buffer (M in place for N != 1 mod 4, the padded copy for odd N on the look-ahead path) and into a kept full copy for the refinement.
 // DSYTRS sweeps each rhs with one CTA when nrhs < 8 and N > 64, else one thread per rhs. The look-ahead factorizations take their
 // 128-column blocks in pairs from pair_min on. Without cooperative launches (unsupported, or HB_CHOL_COOP=0) no "coop" path runs: the
 // factor takes the panels and the condensed solve the one-CTA refinement (and no 16 x 16 inverses are formed).
@@ -173,6 +176,14 @@ struct hb_symdense
   int bk_widths = 0;        // cluster Bunch-Kaufman: OR of the panel widths (8 / 16 / 32 / 64) the last factorization launched (no order)
   bool factored = false;
   int n_neg = 0, n_null = 0, n_pos = 0;
+  // HB_FACT_RBT_NOPIV, allocated by the first RBT factorization: A' (N x N, full), the butterfly diagonals (2 N), row-sum scratch and
+  // ||A'||_inf; the solve adds the rows of x and b', the residual and per-rhs norms
+  hb_dev<double> Ak, rbt_f, rbt_part, rbt_nrm, rbt_xw, rbt_b, rbt_r, rbt_col;
+  hb_pinned<double> rbt_nrm_host;
+  hb_event ev_rbt[2];
+  double rbt_anorm = 0.0, rbt_berr = 0.0;
+  int rbt_corr = 0;
+  float rbt_ms = 0.f;
 };
 
 extern "C" int hb_symdense_create(hb_ctx* c, int N, hb_symdense** out)
@@ -202,29 +213,80 @@ extern "C" int hb_symdense_destroy(hb_symdense* s)
 
 extern "C" double* hb_symdense_matrix(hb_symdense* s) { return s ? s->M.get() : nullptr; }
 
-extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
+// the RBT buffers, on the first RBT factorization of the handle
+static int rbt_reserve(hb_symdense* s)
 {
-  HB_REQUIRE(s, "null handle");
-  HB_REQUIRE(mode == HB_FACT_BUNCH_KAUFMAN || mode == HB_FACT_NOPIV || mode == HB_FACT_CHOLESKY, "hb_symdense_matrix_changed: bad mode");
+  if(s->Ak) return HB_OK;
   hb_ctx* c = s->ctx;
   const int N = s->N;
-  s->mode = mode;
-  s->factored = false;
-  if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
-  HB_CUDA(cudaMemsetAsync(s->info, 0, sizeof(int) * 4, c->stream));
-  s->F = s->M; s->ldf = N; s->big.inv_valid = false;
-  const Plan p = symdense_plan(c, mode, N);
-  s->plan = p;
-  s->bk_widths = 0;
+  HB_CHECK(s->rbt_f.reserve(c, (size_t)2 * N, "butterfly diagonals"));
+  HB_CHECK(s->rbt_part.reserve(c, hb_rbt_part_doubles(N), "row sums of |A'|"));
+  HB_CHECK(s->rbt_nrm.reserve(c, 1, "norm of A'"));
+  HB_CHECK(s->rbt_nrm_host.reserve(c, 3, "norms"));
+  for(int e = 0; e < 2; e++) HB_CHECK(s->ev_rbt[e].create(cudaEventDefault));
+  HB_CHECK(hb_rbt_table(c, N, s->rbt_f));
+  return s->Ak.reserve(c, (size_t)N * N, "the transformed matrix A'"); // last: its presence marks the set complete
+}
+
+// A' = U^T A U from the upper triangle of M into the factor buffer s->F (upper triangle) and s->Ak (full), ||A'||_inf into rbt_anorm
+static int rbt_transform(hb_symdense* s)
+{
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  const bool direct = s->F != s->M.get() || hb_rbt_in_place(N);
+  HB_CUDA(cudaEventRecord(s->ev_rbt[0], c->stream));
+  HB_CHECK(hb_rbt_fused(c, N, s->rbt_f, s->M, N, direct ? s->F : nullptr, s->ldf, s->Ak, N, s->rbt_part, s->rbt_nrm));
+  HB_CUDA(cudaEventRecord(s->ev_rbt[1], c->stream));
+  if(!direct) HB_CUDA(cudaMemcpyAsync(s->M, s->Ak, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, c->stream)); // small N only
+  HB_CUDA(cudaMemcpyAsync(s->rbt_nrm_host, s->rbt_nrm, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  s->rbt_anorm = s->rbt_nrm_host[0];
+  HB_CUDA(cudaEventElapsedTime(&s->rbt_ms, s->ev_rbt[0], s->ev_rbt[1]));
+  return HB_OK;
+}
+
+// where the factor of a plan lives: M, or for odd N on the look-ahead and cluster paths a copy with an even leading dimension (the
+// 16-byte operand copies)
+static int factor_buffer(hb_symdense* s, const Plan& p, bool copy)
+{
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  s->F = s->M; s->ldf = N;
   const bool big = p.f == F_BIG_CHOL || p.f == F_BIG_LDL;
-  if((big || p.f == F_BK_CLUSTER) && (N & 1)) { // even leading dimension for the 16-byte operand copies
+  if((big || p.f == F_BK_CLUSTER) && (N & 1)) {
     const long long ld = (N + 7) & ~7LL;
     if(!s->Fpad) {
       HB_CHECK(s->Fpad.reserve(c, (size_t)ld * N, "the padded factor"));
       HB_CUDA(cudaMemsetAsync(s->Fpad, 0, sizeof(double) * (size_t)ld * N, c->stream));
     }
-    HB_CUDA(cudaMemcpy2DAsync(s->Fpad, sizeof(double) * ld, s->M, sizeof(double) * N, sizeof(double) * N, N, cudaMemcpyDeviceToDevice, c->stream));
+    if(copy)
+      HB_CUDA(cudaMemcpy2DAsync(s->Fpad, sizeof(double) * ld, s->M, sizeof(double) * N, sizeof(double) * N, N, cudaMemcpyDeviceToDevice, c->stream));
     s->F = s->Fpad; s->ldf = ld;
+  }
+  return HB_OK;
+}
+
+extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
+{
+  HB_REQUIRE(s, "null handle");
+  HB_REQUIRE(mode == HB_FACT_BUNCH_KAUFMAN || mode == HB_FACT_NOPIV || mode == HB_FACT_CHOLESKY || mode == HB_FACT_RBT_NOPIV,
+             "hb_symdense_matrix_changed: bad mode");
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  const bool rbt = mode == HB_FACT_RBT_NOPIV;
+  s->mode = mode;
+  s->factored = false;
+  if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
+  HB_CUDA(cudaMemsetAsync(s->info, 0, sizeof(int) * 4, c->stream));
+  s->big.inv_valid = false;
+  const Plan p = symdense_plan(c, rbt ? HB_FACT_NOPIV : mode, N);
+  s->plan = p;
+  s->bk_widths = 0;
+  const bool big = p.f == F_BIG_CHOL || p.f == F_BIG_LDL;
+  HB_CHECK(factor_buffer(s, p, !rbt));
+  if(rbt) {
+    HB_CHECK(rbt_reserve(s));
+    HB_CHECK(rbt_transform(s));
   }
   const long long ldw = (N + 7) & ~7LL;
   if(p.f == F_BK_CLUSTER) {
@@ -273,12 +335,9 @@ extern "C" int hb_symdense_inertia(hb_symdense* s, int* n_neg, int* n_null, int*
   return HB_OK;
 }
 
-extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
+// the sweeps of the current factor on nrhs right-hand sides stored one after the other, in place
+static int plan_sweeps(hb_symdense* s, double* x, int nrhs)
 {
-  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_solve: bad arguments");
-  if(s->N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_solve: no valid factorization (call hb_symdense_matrix_changed)%s", "");
   hb_ctx* c = s->ctx;
   switch(s->plan.s) {
   case S_BIG: {
@@ -290,10 +349,76 @@ extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
   }
   case S_SYTRS: HB_CHECK(bk_sytrs(c, s->N, s->M, s->N, s->ipiv, x, s->N, nrhs)); break;
   case S_ONE_CTA:
-    for(int r = 0; r < nrhs; r++) HB_CHECK(hb_dense_tri_solve(c, s->N, s->M, s->N, s->mode == HB_FACT_NOPIV, x + (size_t)r * s->N));
+    for(int r = 0; r < nrhs; r++) HB_CHECK(hb_dense_tri_solve(c, s->N, s->M, s->N, s->mode != HB_FACT_CHOLESKY, x + (size_t)r * s->N));
     break;
   }
+  return HB_OK;
+}
+
+// RBT: hb_rbt_solve on the rows of x (row-major N x nrhs), the sweeps of the NOPIV plan on columns, the residual against the kept A'
+static int rbt_solve(hb_symdense* s, double* x, int nrhs)
+{
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  const size_t n = (size_t)N * nrhs;
+  HB_CHECK(s->rbt_xw.reserve(c, n, "solve rows"));
+  HB_CHECK(s->rbt_b.reserve(c, n, "transformed rhs"));
+  HB_CHECK(s->rbt_r.reserve(c, n + 3 * (size_t)nrhs, "residual and norms"));
+  HB_CHECK(s->rbt_nrm_host.reserve(c, 3 * (size_t)nrhs, "norms"));
+  if(nrhs > 1) HB_CHECK(s->rbt_col.reserve(c, n, "solve columns"));
+  auto sweeps = [&](double* v) -> int {
+    if(nrhs == 1) return plan_sweeps(s, v, 1); // one rhs: rows and columns are the same array
+    HB_CHECK(hb_rbt_to_rows(c, N, nrhs, s->rbt_col, v, true));
+    HB_CHECK(plan_sweeps(s, s->rbt_col, nrhs));
+    return hb_rbt_to_rows(c, N, nrhs, s->rbt_col, v, false);
+  };
+  auto residual = [&](const double* xr, const double* b, double* r) { return hb_rbt_rows(c, N, 1, 0, N, s->Ak, N, nrhs, xr, b, r); };
+  HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, s->rbt_xw, false));
+  const int ok = hb_rbt_solve(c, N, nrhs, s->rbt_f, s->rbt_anorm, s->rbt_xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual, &s->rbt_corr,
+                              &s->rbt_berr);
+  if(ok < 0) return ok;
+  HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, s->rbt_xw, true));
+  return ok;
+}
+
+extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
+{
+  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_solve: bad arguments");
+  if(s->N == 0 || nrhs == 0) return 1;
+  HB_REQUIRE(x, "hb_symdense_solve: null rhs");
+  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_solve: no valid factorization (call hb_symdense_matrix_changed)%s", "");
+  if(s->mode == HB_FACT_RBT_NOPIV) return rbt_solve(s, x, nrhs);
+  HB_CHECK(plan_sweeps(s, x, nrhs));
   return 1;
+}
+
+extern "C" int hb_symdense_rbt_stats(hb_symdense* s, int* corrections, double* backward_error, float* transform_ms)
+{
+  HB_REQUIRE(s, "null handle");
+  if(corrections) *corrections = s->rbt_corr;
+  if(backward_error) *backward_error = s->rbt_berr;
+  if(transform_ms) *transform_ms = s->rbt_ms;
+  return HB_OK;
+}
+
+// diagnostics (tests): the RBT transform of the upper triangle of M without factoring; A' (full) and the factor buffer's upper triangle
+extern "C" int hb_debug_symdense_rbt(hb_symdense* s, double* Ak_host, double* F_host)
+{
+  HB_REQUIRE(s, "null handle");
+  if(s->N == 0) return HB_OK;
+  hb_ctx* c = s->ctx;
+  const int N = s->N;
+  HB_CUDA(cudaSetDevice(c->device));
+  s->factored = false;
+  s->plan = symdense_plan(c, HB_FACT_NOPIV, N);
+  HB_CHECK(factor_buffer(s, s->plan, false));
+  HB_CHECK(rbt_reserve(s));
+  HB_CHECK(rbt_transform(s));
+  if(Ak_host) HB_CUDA(cudaMemcpyAsync(Ak_host, s->Ak, sizeof(double) * N * N, cudaMemcpyDeviceToHost, c->stream));
+  if(F_host)
+    HB_CUDA(cudaMemcpy2DAsync(F_host, sizeof(double) * N, s->F, sizeof(double) * s->ldf, sizeof(double) * N, N, cudaMemcpyDeviceToHost, c->stream));
+  HB_CUDA(cudaStreamSynchronize(c->stream));
+  return HB_OK;
 }
 
 extern "C" int hb_symdense_matrix_changed_host(hb_symdense* s, const double* M_host, int mode)

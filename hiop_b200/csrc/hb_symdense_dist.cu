@@ -22,14 +22,14 @@
 //
 // Safe mode (HB_FACT_RBT_NOPIV): A' = U^T A U with a depth-2 random butterfly U = B2 B1 (rbt_transform: the mirror of the upper
 // triangle, then one pass per level, each output row formed from its row and its partner row), the no-pivot LDL^T above on A', and
-// solves refined against a kept copy of A' (rbt_solve). Every entry of A' is a fixed expression of oracle/rbt_model.py and the random
+// solves refined against a kept copy of A' (rbt_solve, the refinement loop of hb_rbt.cu). Every entry of A' is a fixed expression of oracle/rbt_model.py and the random
 // diagonals depend on N alone, so A', the factor and the solution do not depend on P either.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
 
 namespace {
 
-constexpr int DB = 128;          // block size = hb_big_factor's
+constexpr int DB = HB_DIST_DB;   // block size = hb_big_factor's
 constexpr int HDR = 136;         // broadcast header: 1/d (128 doubles), info word (as the first int of slot 128), pad to 16 bytes
 constexpr int SOLVE_RHS = 4;     // right-hand sides per CTA of the diagonal-block solves
 constexpr int DLD = DB + 1;      // shared-memory stride of the diagonal block
@@ -68,17 +68,6 @@ __global__ void __launch_bounds__(1024) k_dist_inertia(const double* __restrict_
   atomicAdd(&cnt[0], neg); atomicAdd(&cnt[1], nul); atomicAdd(&cnt[2], pos);
   __syncthreads();
   if(threadIdx.x < 3) out3[threadIdx.x] = (double)cnt[threadIdx.x];
-}
-
-// x (N x nrhs, one rhs after the other) <-> xw (row-major N x nrhs: the rows of a block are contiguous for the broadcasts)
-__global__ void k_dist_to_rows(int N, int nrhs, double* __restrict__ x, double* __restrict__ xw, int back)
-{
-  const long long total = (long long)N * nrhs;
-  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const long long i = e / nrhs, c = e % nrhs;
-    if(back) x[c * N + i] = xw[e];
-    else xw[e] = x[c * N + i];
-  }
 }
 
 // the nb x nb diagonal block of block column k0 into shared memory: S[j * DLD + i] = L(k0 + i, k0 + j), i >= j
@@ -161,55 +150,9 @@ __global__ void __launch_bounds__(DB * SOLVE_RHS) k_dist_bwd_diag(const double* 
   if(live) xw[(size_t)(k0 + i) * nrhs + c] = xs[cl * DB + i];
 }
 
-// ---- random butterfly transform (HB_FACT_RBT_NOPIV): A' = U^T A U, U = B2 B1 (oracle/rbt_model.py states every expression) ----------
-constexpr unsigned long long RBT_SEED = 0x5EED2011B7F10001ull, RBT_GOLDEN = 0x9E3779B97F4A7C15ull;
-constexpr double RBT_C = 0.7071067811865476; // the double nearest 1/sqrt(2)
-constexpr double RBT_EPS = 0x1p-52;          // refinement target of the backward error
-constexpr int RBT_MAX_CORR = 3;
+// ---- random butterfly transform (HB_FACT_RBT_NOPIV): A' = U^T A U, U = B2 B1 (oracle/rbt_model.py states every expression; the
+// diagonals, the vector and row kernels and the refined solve are shared with hb_symdense in hb_rbt.cu) ------------------------------
 constexpr int RBT_COLS = 1024;               // columns per CTA of k_rbt_level (256 threads x 4)
-
-// r_t of butterfly `half` of `level`: 1 + (k - 2^19) / 2^23, k = the top 20 bits of splitmix64 of the counter (stream << 32 | t)
-__device__ __forceinline__ double rbt_diag(int level, int half, int t)
-{
-  unsigned long long z = RBT_SEED + RBT_GOLDEN * ((((unsigned long long)(2 * level + half)) << 32 | (unsigned)t) + 1ull);
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  z ^= z >> 31;
-  return (double)((1LL << 23) + (long long)(z >> 44) - (1LL << 19)) / (double)(1 << 23);
-}
-
-// the entries of column i of a level's butterfly: rows lo and hi (lo = hi = i when unpaired), sign s of the hi side (+1 on the lo side)
-struct rbt_pos
-{
-  int lo, hi;
-  double s;
-  bool paired;
-};
-__device__ __forceinline__ rbt_pos rbt_at(int N, int level, int i)
-{
-  int o = 0, n = N;
-  if(level == 2) {
-    const int h = (N + 1) / 2;
-    if(i >= h) o = h, n = N - h;
-    else n = h;
-  }
-  const int hh = (n + 1) / 2, t = i - o;
-  if(t < n - hh) return {i, i + hh, 1.0, true};
-  if(t >= hh) return {i - hh, i, -1.0, true};
-  return {i, i, 1.0, false};
-}
-
-// f[(level - 1) * N + i]: the diagonal entry of column i at level 1 (B1) and 2 (B2); a function of N alone
-__global__ void k_rbt_table(int N, double* __restrict__ f)
-{
-  const int h = (N + 1) / 2;
-  for(int i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
-    f[i] = rbt_diag(1, 0, i);
-    f[N + i] = i < h ? rbt_diag(2, 0, i) : rbt_diag(2, 1, i - h);
-  }
-}
-
-__device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / DB) * P + rank) * DB + y % DB; }
 
 // mirror: every owned row r gets dst(r, j) = src(j, r) for the columns q0 <= j < q0 + nq, j < r, where src holds the rows q0 .. of the
 // upper triangle (ld doubles each). 32 x 32 tiles through shared memory: rows y0 .. of the owned rows, starting at local row ybeg.
@@ -254,85 +197,7 @@ __global__ void __launch_bounds__(256) k_rbt_level(int N, int level, const doubl
   const int jend = min(N, (int)(blockIdx.y + 1) * RBT_COLS);
   for(int j = blockIdx.y * RBT_COLS + threadIdx.x; j < jend; j += 256) {
     const rbt_pos pj = rbt_at(N, level, j);
-    const double all = RL[pj.lo], ahh = RH[pj.hi], ss = pr.s * pj.s;
-    double t, w;
-    if(pr.paired && pj.paired) {
-      t = __dadd_rn(__dadd_rn(all, __dmul_rn(ss, ahh)), __dadd_rn(__dmul_rn(pj.s, RL[pj.hi]), __dmul_rn(pr.s, RH[pj.lo])));
-      w = 0.5;
-    } else if(pr.paired || pj.paired) {
-      t = __dadd_rn(all, __dmul_rn(ss, ahh));
-      w = RBT_C;
-    } else {
-      t = all;
-      w = 1.0;
-    }
-    o[j] = __dmul_rn(__dmul_rn(fi, fl[j]), __dmul_rn(t, w));
-  }
-}
-
-// one level on the replicated row-major vectors (N x nrhs): B^T v (trans) or B v
-__global__ void k_rbt_vec(int N, int nrhs, int level, const double* __restrict__ f, const double* __restrict__ in, double* __restrict__ out, int trans)
-{
-  const double* fl = f + (size_t)(level - 1) * N;
-  const long long total = (long long)N * nrhs;
-  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const int i = (int)(e / nrhs), c = (int)(e % nrhs);
-    const rbt_pos p = rbt_at(N, level, i);
-    const double vl = in[(size_t)p.lo * nrhs + c], vh = in[(size_t)p.hi * nrhs + c];
-    double v;
-    if(!p.paired) v = __dmul_rn(fl[i], vl);
-    else if(trans) v = __dmul_rn(fl[i], __dmul_rn(__dadd_rn(vl, __dmul_rn(p.s, vh)), RBT_C));
-    else v = __dmul_rn(__dadd_rn(__dmul_rn(fl[p.lo], vl), __dmul_rn(p.s, __dmul_rn(fl[p.hi], vh))), RBT_C);
-    out[e] = v;
-  }
-}
-
-// CTA per owned row r of A' (full rows): out_r = sum_j |A'(r, j)| (norm) or r_r = b'_r - sum_j A'(r, j) x'_j per rhs, in a fixed order
-__global__ void __launch_bounds__(256) k_rbt_rows(int N, int P, int rank, const double* __restrict__ A, long long ld, int nrhs, const double* __restrict__ x,
-                                                  const double* __restrict__ b, double* __restrict__ out)
-{
-  __shared__ double red[8];
-  const int r = rbt_global_row(blockIdx.x, P, rank);
-  if(r >= N) {
-    if(!x && threadIdx.x == 0) out[blockIdx.x] = 0.0;
-    return;
-  }
-  const double* row = A + (size_t)blockIdx.x * ld;
-  if(!x) {
-    double acc = 0.0;
-    for(int j = threadIdx.x; j < N; j += 256) acc += fabs(row[j]);
-    acc = hb_block_sum<256>(acc, red);
-    if(threadIdx.x == 0) out[blockIdx.x] = acc;
-    return;
-  }
-  for(int c = 0; c < nrhs; c++) {
-    double acc = 0.0;
-    for(int j = threadIdx.x; j < N; j += 256) acc += row[j] * x[(size_t)j * nrhs + c];
-    acc = hb_block_sum<256>(acc, red);
-    if(threadIdx.x == 0) out[(size_t)r * nrhs + c] = b[(size_t)r * nrhs + c] - acc;
-    __syncthreads();
-  }
-}
-
-// one CTA per column c: out[c * 3 + k] = max_i |v_k(i, c)| over the N rows of the row-major N x ncols arrays v_0, v_1, v_2 (0 for an
-// absent one), NaN kept, in a fixed order
-__global__ void __launch_bounds__(256) k_rbt_max(int N, int ncols, const double* __restrict__ v0, const double* __restrict__ v1, const double* __restrict__ v2,
-                                                 double* __restrict__ out)
-{
-  __shared__ double sm[3][256];
-  const double* v[3] = {v0, v1, v2};
-  const int c = blockIdx.x;
-  for(int k = 0; k < 3; k++) {
-    double m = 0.0;
-    if(v[k])
-      for(int i = threadIdx.x; i < N; i += 256) m = hb_nan_max(m, fabs(v[k][(size_t)i * ncols + c]));
-    sm[k][threadIdx.x] = m;
-  }
-  __syncthreads();
-  if(threadIdx.x < 3) {
-    double m = 0.0;
-    for(int t = 0; t < 256; t++) m = hb_nan_max(m, sm[threadIdx.x][t]);
-    out[(size_t)c * 3 + threadIdx.x] = m;
+    o[j] = rbt_entry(RL[pj.lo], RH[pj.hi], RL[pj.hi], RH[pj.lo], pr, pj, fi, fl[j]);
   }
 }
 
@@ -500,8 +365,7 @@ static int rbt_reserve(hb_symdense_dist* s)
   HB_CHECK(s->rbt_rows.reserve(c, (size_t)s->nloc * DB, "row sums of |A'|"));
   HB_CHECK(s->rbt_nrm.reserve(c, 4, "norm of A'"));
   for(int e = 0; e < 2; e++) HB_CHECK(s->ev_rbt[e].create(cudaEventDefault));
-  k_rbt_table<<<hb_grid(c, s->N), 256, 0, c->stream>>>(s->N, s->rbt_f);
-  HB_LAUNCHED();
+  HB_CHECK(hb_rbt_table(c, s->N, s->rbt_f));
   HB_CUDA(cudaStreamSynchronize(c->stream));
   s->rbt_ready = true;
   return HB_OK;
@@ -568,12 +432,8 @@ static int rbt_transform(hb_symdense_dist* s, int stages)
   if(s->profile) HB_CUDA(cudaEventRecord(s->ev_rbt[1], st));
   if(stages == 2) {
     HB_CUDA(cudaMemcpyAsync(s->Ak, s->A, sizeof(double) * nrows * ld, cudaMemcpyDeviceToDevice, st));
-    if(nrows > 0) {
-      k_rbt_rows<<<nrows, 256, 0, st>>>(N, P, rank, s->Ak, ld, 0, nullptr, nullptr, s->rbt_rows);
-      HB_LAUNCHED();
-    }
-    k_rbt_max<<<1, 256, 0, st>>>(nrows, 1, s->rbt_rows, nullptr, nullptr, s->rbt_nrm);
-    HB_LAUNCHED();
+    HB_CHECK(hb_rbt_rows(c, N, P, rank, nrows, s->Ak, ld, 0, nullptr, nullptr, s->rbt_rows));
+    HB_CHECK(hb_rbt_max1(c, nrows, s->rbt_rows, s->rbt_nrm));
     HB_CHECK(hb_allreduce_op(c, s->rbt_nrm, 1, HB_MAX));
     HB_CUDA(cudaMemcpyAsync(s->red_host, s->rbt_nrm, sizeof(double), cudaMemcpyDeviceToHost, st));
   }
@@ -742,56 +602,22 @@ static int dist_sweeps(hb_symdense_dist* s, double* xw, int nrhs)
   return HB_OK;
 }
 
-// RBT solve on the row-major xw (b in, x out): b' = U^T b, the sweeps, refinement against A', x = U x'. The stopping rule reads only
-// replicated values (the residual is formed by the owner of each block row and broadcast), so every rank makes the same decisions.
+// RBT solve on the row-major xw (b in, x out): hb_rbt_solve with the sweeps above, and residual rows formed by the owner of each block
+// row and broadcast, so that the stopping rule reads only replicated values and every rank makes the same decisions.
 static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs)
 {
   hb_ctx* c = s->ctx;
   const int N = s->N, P = s->P, rank = s->rank, nrows = s->nloc * DB;
-  cudaStream_t st = c->stream;
-  const int tg = hb_grid(c, (long long)N * nrhs);
-  double *bp = s->rbt_b, *rw = s->rbt_r, *nrm = rw + (size_t)N * nrhs; // per rhs: max |r|, max |x'|, max |b'|
-  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, s->rbt_f, xw, rw, 1);
-  HB_LAUNCHED();
-  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 1, s->rbt_f, rw, bp, 1);
-  HB_LAUNCHED();
-  HB_CUDA(cudaMemcpyAsync(xw, bp, sizeof(double) * N * nrhs, cudaMemcpyDeviceToDevice, st));
-  HB_CHECK(dist_sweeps(s, xw, nrhs));
-  double om = 0.0, prev = INFINITY;
-  int corr = 0;
-  for(;;) {
-    if(nrows > 0) {
-      k_rbt_rows<<<nrows, 256, 0, st>>>(N, P, rank, s->Ak, s->ld, nrhs, xw, bp, rw);
-      HB_LAUNCHED();
-    }
+  auto sweeps = [&](double* v) { return dist_sweeps(s, v, nrhs); };
+  auto residual = [&](const double* x, const double* b, double* r) -> int {
+    HB_CHECK(hb_rbt_rows(c, N, P, rank, nrows, s->Ak, s->ld, nrhs, x, b, r));
     for(int k = 0; k < s->nblk; k++) {
       const int k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
-      HB_CHECK(hb_broadcast(c, rw + (size_t)k0 * nrhs, (long long)nb * nrhs, k % P, st));
+      HB_CHECK(hb_broadcast(c, r + (size_t)k0 * nrhs, (long long)nb * nrhs, k % P, c->stream));
     }
-    k_rbt_max<<<nrhs, 256, 0, st>>>(N, nrhs, rw, xw, bp, nrm);
-    HB_LAUNCHED();
-    HB_CUDA(cudaMemcpyAsync(s->rbt_nrm_host, nrm, sizeof(double) * 3 * nrhs, cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaStreamSynchronize(st));
-    om = 0.0;
-    for(int q = 0; q < nrhs; q++) {
-      const double* m3 = s->rbt_nrm_host.get() + 3 * q;
-      const double den = s->rbt_anorm * m3[1] + m3[2];
-      const double w = den > 0.0 ? m3[0] / den : (m3[0] == 0.0 ? 0.0 : INFINITY);
-      om = (w > om || w != w) ? w : om;
-    }
-    if(!(corr < RBT_MAX_CORR && om > RBT_EPS && om <= 0.5 * prev)) break;
-    HB_CHECK(dist_sweeps(s, rw, nrhs));
-    HB_CHECK(hb_vec_axpy(c, (long long)N * nrhs, xw, 1.0, rw));
-    corr++;
-    prev = om;
-  }
-  s->rbt_corr = corr;
-  s->rbt_berr = om;
-  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 1, s->rbt_f, xw, rw, 0);
-  HB_LAUNCHED();
-  k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, s->rbt_f, rw, xw, 0);
-  HB_LAUNCHED();
-  return std::isfinite(om) ? 1 : 0;
+    return HB_OK;
+  };
+  return hb_rbt_solve(c, N, nrhs, s->rbt_f, s->rbt_anorm, xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual, &s->rbt_corr, &s->rbt_berr);
 }
 
 extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
@@ -803,7 +629,6 @@ extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
   hb_ctx* c = s->ctx;
   const int N = s->N;
   const bool rbt = s->mode == HB_FACT_RBT_NOPIV;
-  cudaStream_t st = c->stream;
   HB_CUDA(cudaSetDevice(c->device));
   auto reserve = [&]() -> int {
     HB_CHECK(s->xw.reserve(c, (size_t)N * nrhs, "solve rows"));
@@ -818,9 +643,7 @@ extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
   };
   HB_CHECK(agree(c, reserve()));
   double* xw = s->xw;
-  const int tg = hb_grid(c, (long long)N * nrhs);
-  k_dist_to_rows<<<tg, 256, 0, st>>>(N, nrhs, x, xw, 0);
-  HB_LAUNCHED();
+  HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, xw, false));
   int ok = 1;
   if(rbt) {
     ok = rbt_solve(s, xw, nrhs);
@@ -828,7 +651,6 @@ extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
   } else {
     HB_CHECK(dist_sweeps(s, xw, nrhs));
   }
-  k_dist_to_rows<<<tg, 256, 0, st>>>(N, nrhs, x, xw, 1);
-  HB_LAUNCHED();
+  HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, xw, true));
   return ok;
 }

@@ -164,7 +164,7 @@ class LinSolverSymDense:
     """hiopLinSolverSymDense: owns the N x N row-major system matrix (upper triangle valid), `matrixChanged()` returns
     the number of negative eigenvalues or -1, `solve(x)` overwrites the rhs (src/LinAlg/hiopLinSolver.hpp:78-128)."""
 
-    BUNCH_KAUFMAN, NOPIV, CHOLESKY = _lib.HB_FACT_BUNCH_KAUFMAN, _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY
+    BUNCH_KAUFMAN, NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_BUNCH_KAUFMAN, _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
 
     def __init__(self, ctx: Context, n: int, mode: int = _lib.HB_FACT_BUNCH_KAUFMAN):
         self.ctx, self.n, self.mode = ctx, n, mode
@@ -214,6 +214,12 @@ class LinSolverSymDense:
         if rc < 0:
             check(rc, "hb_symdense_solve_host")
         return rc == 1
+
+    def rbt_stats(self):
+        """(corrections, backward error) of the last RBT_NOPIV solve and the transform time (ms) of the last RBT_NOPIV factorization"""
+        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
+        check(self.ctx.L.hb_symdense_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_rbt_stats")
+        return n.value, be.value, float(ms.value)
 
 
 class _DeviceArray:

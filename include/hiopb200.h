@@ -176,7 +176,7 @@ int hb_mat_add_upper_to_sym_upper(hb_ctx*, int n, const double* A, long long lda
 #define HB_FACT_BUNCH_KAUFMAN 0 /* pivoted LDL^T (DSYTRF / magma_dsytrf_gpu semantics), inertia from 1x1/2x2 pivots */
 #define HB_FACT_NOPIV 1         /* LDL^T without pivoting (magma_dsytrf_nopiv_gpu, linsol_mode=speculative) */
 #define HB_FACT_CHOLESKY 2      /* LL^T for SPD systems (DPOTRF; duals LSQ + condensed QN system) */
-#define HB_FACT_RBT_NOPIV 3     /* random butterfly transform, LDL^T without pivoting, refinement (hb_symdense_dist only; linsol_mode=stable) */
+#define HB_FACT_RBT_NOPIV 3     /* random butterfly transform, LDL^T without pivoting, refinement (safe mode of linsol_mode=stable) */
 
 int hb_symdense_create(hb_ctx* ctx, int N, hb_symdense** out);
 int hb_symdense_destroy(hb_symdense* s);
@@ -187,11 +187,35 @@ double* hb_symdense_matrix(hb_symdense* s);
  * -1 if a null pivot (|d| < 1e-14, hiopLinSolverSymDenseLapack.hpp:154-166) or a breakdown was met.
  * Values <= -2 are HB_ERR_* codes. */
 int hb_symdense_matrix_changed(hb_symdense* s, int mode);
+/* HB_FACT_RBT_NOPIV (the safe mode without Bunch-Kaufman): A' = U^T A U with the depth-2 random butterfly U of hb_symdense_dist (the same
+ * bits of A' as hb_symdense_dist at every P, oracle/rbt_model.py), formed in one pass over the upper triangle of M, then the
+ * HB_FACT_NOPIV factorization of A' (the same plan and bits as HB_FACT_NOPIV on A'). The return value and the inertia are those of A',
+ * which equal those of A (U is nonsingular). A' is kept for the refinement of hb_symdense_solve: the first RBT factorization allocates a
+ * second N x N matrix, 2 N butterfly diagonals and (N / 64 + 1) N doubles of row-sum scratch, so the handle's device memory doubles
+ * and the largest order this mode takes on one 80 GB card is about 70 000 instead of about 100 000 (hb_symdense_dist spreads both
+ * copies over the ranks). A handle that never sees this mode allocates none of it. */
 /* inertia of the last factorization (host ints): negative, null, positive */
 int hb_symdense_inertia(hb_symdense* s, int* n_neg, int* n_null, int* n_pos);
 /* solve(x): in-place solve with nrhs right-hand sides stored one after the other (each N doubles, device).
  * Returns 1 on success, 0 on failure (bool semantics of hiopLinSolver::solve), negative HB_ERR_* on misuse. */
 int hb_symdense_solve(hb_symdense* s, double* x, int nrhs);
+/* After HB_FACT_RBT_NOPIV, solve refines like hb_symdense_dist_solve: b' = U^T b, the sweeps of the no-pivot factor, refinement against
+ * the kept A' with omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf) (correct while omega > 2^-52,
+ * fewer than 3 corrections were made and omega is at most half its value before the last correction), x = U x'; 0 when omega is not
+ * finite. hb_symdense_rbt_stats: the last RBT solve's corrections and omega, and the last RBT factorization's transform time (ms,
+ * device events, every factorization). Every output may be NULL. */
+int hb_symdense_rbt_stats(hb_symdense* s, int* corrections, double* backward_error, float* transform_ms);
+/* diagnostics (tests): the RBT transform of the upper triangle of M without factoring (the handle then holds no factorization): A'
+ * (N x N row-major, full) and the factor buffer the factorization would read (N x N row-major, upper triangle = A', unpadded). Either
+ * output may be NULL. */
+int hb_debug_symdense_rbt(hb_symdense* s, double* Aprime_host, double* F_host);
+/* The tile schedule of the one-pass RBT transform (k_rbt_fused, hb_rbt.cu) for order N, run on the host (no device needed). dims4 =
+ * {tiles T, CTAs C, window rows W, output rows O}. CTA b takes the tile pair ctas_host[2b .. 2b+1] = {bi, bj}, bi <= bj, and computes
+ * A'(i, j) for i among the output rows of tile bi and j among those of tile bj from the entries A(r, c) (read as A(min, max)) with r
+ * among the window rows of tile bi and c among those of tile bj (on a diagonal tile only r <= c is read). Tile t: window_host[t W ..]
+ * (W global rows, -1 for none) and out_host[t O ..] (O global rows, -1 for none). Filled for the first min(cap, C) CTAs and
+ * min(cap, T) tiles. */
+int hb_rbt_schedule_view(int N, int cap, int* dims4, int* ctas_host, int* window_host, int* out_host);
 /* host-buffer convenience used by the C++ adapter when mem_space is host: uploads the upper triangle, factorizes */
 int hb_symdense_matrix_changed_host(hb_symdense* s, const double* M_host, int mode);
 int hb_symdense_solve_host(hb_symdense* s, double* x_host, int nrhs);

@@ -8,9 +8,10 @@ the factor time, the bytes one factorization broadcasts (from the shapes), the p
 over ranks: panel chain, broadcast including the wait for the owner, trailing update), hb_symdense's time on the same matrix on rank 0
 with its default dispatch and with its blocks never paired (K = 128 updates), max |x_dist - x_single| / |x|, and the card's name and power limit.
 Mode rbt (the safe mode, HB_FACT_RBT_NOPIV) adds the transform time of one profiled factorization, the corrections and backward error of
-the refined solve, and whether its inertia equals hb_symdense's Bunch-Kaufman on rank 0 on the same matrix. Then one line each for a mixed
-dense-sparse step in speculative mode (no-pivot LDL^T) and in stable mode (RBT; update + build + factor + solve) at bench.py's MDS size,
-distributed against the replicated single-GPU step, with the residual of the uncondensed system (must be <= 1e-8)."""
+the refined solve, and whether its inertia equals hb_symdense's Bunch-Kaufman on rank 0 on the same matrix, and the same for the one-GPU
+safe mode (hb_symdense with HB_FACT_RBT_NOPIV) on rank 0. Then one line each for a mixed dense-sparse step in speculative mode (no-pivot
+LDL^T) and in stable mode (RBT; update + build + factor + solve) at bench.py's MDS size, distributed against the replicated single-GPU step
+(stable: Bunch-Kaufman, and the one-GPU RBT step), with the residual of the uncondensed system (must be <= 1e-8)."""
 import argparse
 import json
 import os
@@ -219,19 +220,41 @@ def run_rbt(N, ctx, world, rank, rmax, timed, info):
     corr, berr, _ = s.rbt_stats()
     s.close()
     f_ms, s_ms, transform_ms = rmax(f_ms), rmax(s_ms), rmax(transform_ms)
-    same = None
+    same = single = None
     if rank == 0:
         ss = LinSolverSymDense(ctx, N, BK)
         ss.set_matrix(M)
         rc_bk = ss.matrixChanged()
-        same = rc_bk == N // 3 and ss.inertia() == inertia
+        in_bk = ss.inertia()
+        same = rc_bk == N // 3 and in_bk == inertia
         ss.close()
+        # the same safe mode on one GPU (hb_symdense): fused transform, NOPIV's plan on A', refined solve
+        su = LinSolverSymDense(ctx, N, RBT)
+
+        def sfactor():
+            su.set_matrix(M)
+            assert su.matrixChanged() == N // 3
+        sfactor()
+        c_ms = timed(lambda: su.set_matrix(M), 1)
+        sf_ms = timed(sfactor, 3) - c_ms
+        t_ms = su.rbt_stats()[2]
+
+        def ssolve():
+            with torch.cuda.stream(ctx.stream):
+                x.copy_(b)
+            assert su.solve(x)
+        ssolve()
+        ss_ms = timed(ssolve, 3)
+        scorr, sberr, _ = su.rbt_stats()
+        single = {"factor_ms": sf_ms, "transform_ms": t_ms, "solve_ms": ss_ms, "corrections": scorr, "backward_error": sberr,
+                  "inertia_equals_bunch_kaufman": rc_bk == N // 3 and su.inertia() == in_bk}
+        su.close()
     del M
     torch.cuda.empty_cache()
     if rank == 0:
         print(json.dumps({"N": N, "mode": "rbt", "P": world, "factor_ms": f_ms, "solve_ms": s_ms, "transform_ms": transform_ms,
                           "corrections": corr, "backward_error": berr, "inertia": list(inertia), "inertia_equals_bunch_kaufman_rank0": same,
-                          **info}), flush=True)
+                          "single_gpu_hb_symdense_rank0": single, **info}), flush=True)
 
 
 def run_mds(args, ctx, world, rank, rmax, timed, info, stable=False):
@@ -281,6 +304,12 @@ def run_mds(args, ctx, world, rank, rmax, timed, info, stable=False):
             sms = timed(step_single, args.steps)
             single = {"ms_per_step": sms, "resid": bench.mds_independent_residual(torch, T, nxs, nxd, neq, nineq, dx, dyc, dyd),
                       "max_rel_diff_dx": float((dxd - dx).abs().max() / dx.abs().max())}
+            if stable:       # the single-GPU stable step with the random-butterfly safe mode instead of Bunch-Kaufman
+                k.linSys.mode = k.linSys.RBT_NOPIV
+                step_single()
+                single["rbt_ms_per_step"] = timed(step_single, args.steps)
+                single["rbt_resid"] = bench.mds_independent_residual(torch, T, nxs, nxd, neq, nineq, dx, dyc, dyd)
+                single["rbt_transform_ms"] = k.linSys.rbt_stats()[2]
         k.close()
     assert resid <= 1e-8, resid
     if rank == 0:
