@@ -128,6 +128,7 @@ def lib() -> ctypes.CDLL:
     f("hb_debug_symdense_factor", c_i, c_vp, P(c_i), P(c_i), c_vp, c_vp, c_vp, c_vp)
     f("hb_symdense_rbt_stats", c_i, c_vp, P(c_i), P(ctypes.c_double), P(ctypes.c_float))
     f("hb_debug_symdense_rbt", c_i, c_vp, c_vp, c_vp)
+    f("hb_debug_symdense_rbt_solve", c_i, c_vp, c_dp, c_i, c_dp, c_d, P(c_i), P(c_i), *([c_vp] * 4))
     f("hb_rbt_schedule_view", c_i, c_i, c_i, P(c_i), c_vp, c_vp, c_vp)
     f("hb_debug_condensed_solve", c_i, c_vp, c_i, c_vp, c_vp, c_i, c_vp, c_vp, c_d, c_i, *([c_vp] * 6))
     f("hb_symdense_dist_create", c_i, c_vp, c_i, P(c_vp))
@@ -140,6 +141,7 @@ def lib() -> ctypes.CDLL:
     f("hb_symdense_dist_profile", c_i, c_vp, c_i, P(ctypes.c_float))
     f("hb_symdense_dist_rbt_stats", c_i, c_vp, P(c_i), P(ctypes.c_double), P(ctypes.c_float))
     f("hb_debug_symdense_dist_rbt", c_i, c_vp, c_i)
+    f("hb_debug_symdense_dist_rbt_solve", c_i, c_vp, c_dp, c_i, P(c_i), P(c_i), *([c_vp] * 4))
     f("hb_microbench_peak", c_i, c_vp, c_i, P(c_d))
     # lowrank
     f("hb_lowrank_create", c_i, c_vp, c_ll, c_i, c_i, c_i, P(c_vp))

@@ -204,12 +204,23 @@ int hb_rbt_rows(hb_ctx* c, int N, int P, int rank, int nrows, const double* A, l
 int hb_rbt_max1(hb_ctx* c, int n, const double* v, double* out);
 // The refined RBT solve on the row-major N x nrhs xw (b in, x out): b' = U^T b (kept in bp), sweeps(xw), then while the stopping rule
 // allows: residual(x', b', r) forms r = b' - A' x' in rw, sweeps(rw), x' += r; finally x = U x'. omega = max over the rhs of
-// ||r||_inf / (anorm ||x'||_inf + ||b'||_inf); correct while omega > HB_RBT_EPS, fewer than HB_RBT_MAX_CORR corrections were made and omega
-// is at most half its value before the last correction. rw: N nrhs + 3 nrhs doubles, nrm_host: 3 nrhs pinned doubles. Returns 1, 0 when
-// omega is not finite, or an HB_ERR_* code; *corr and *berr receive the corrections and the last omega.
+// ||r||_inf / (anorm ||x'||_inf + ||b'||_inf), NaN for a column where one of the three norms or anorm is not finite, +inf where the
+// denominator is 0 and r is not, 0 for a zero column (a NaN wins the max); correct while omega is finite, omega > HB_RBT_EPS, fewer than
+// HB_RBT_MAX_CORR corrections were made and omega is at most half its value before the last correction. rw: N nrhs + 3 nrhs doubles,
+// nrm_host: 3 nrhs pinned doubles. Returns 1, 0 when omega is not finite, or an HB_ERR_* code; *corr and *berr receive the corrections
+// and the last omega. trace (tests only, NULL otherwise) receives what the loop read: it adds copies to the host, never a kernel.
+struct hb_rbt_trace
+{
+  double anorm = 0.0;
+  std::vector<double> norms; // per pass: max |r|, max |x'|, max |b'| of every rhs (3 nrhs), then omega
+  std::vector<double> x;     // per pass: x' (row-major N x nrhs) before its residual
+  std::vector<double> b;     // b' (row-major N x nrhs)
+};
 int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, double* xw, double* bp, double* rw, double* nrm_host,
                  const std::function<int(double*)>& sweeps, const std::function<int(const double*, const double*, double*)>& residual, int* corr,
-                 double* berr);
+                 double* berr, hb_rbt_trace* trace = nullptr);
+// copies a trace into the host buffers of hb_debug_symdense_rbt_solve / hb_debug_symdense_dist_rbt_solve (every one may be NULL)
+void hb_rbt_trace_out(const hb_rbt_trace& t, int* passes, double* anorm, double* norms, double* xp, double* bp);
 // One GPU: A' from the upper triangle of A (ld lda; the other triangle is not read) in one pass (k_rbt_fused): the upper triangle of A'
 // into F (ldf; may be A itself when hb_rbt_in_place(N), NULL for none), the full A' into Ak (ldk), ||A'||_inf into nrm_dev[0].
 // part: hb_rbt_part_doubles(N) doubles of row-sum scratch.

@@ -14,6 +14,7 @@
 // the reads. The tile schedule is __host__ __device__ code that hb_rbt_schedule_view runs on the host for the tests.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
+#include <algorithm>
 
 namespace {
 
@@ -333,20 +334,34 @@ int hb_rbt_max1(hb_ctx* c, int n, const double* v, double* out)
 
 int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, double* xw, double* bp, double* rw, double* nrm_host,
                  const std::function<int(double*)>& sweeps, const std::function<int(const double*, const double*, double*)>& residual, int* corr_out,
-                 double* berr_out)
+                 double* berr_out, hb_rbt_trace* trace)
 {
   cudaStream_t st = c->stream;
   const int tg = hb_grid(c, (long long)N * nrhs);
-  double* nrm = rw + (size_t)N * nrhs; // per rhs: max |r|, max |x'|, max |b'|
+  const size_t n = (size_t)N * nrhs;
+  double* nrm = rw + n; // per rhs: max |r|, max |x'|, max |b'|
+  auto to_trace = [&](std::vector<double>& v, const double* d, size_t count) -> int {
+    const size_t at = v.size();
+    v.resize(at + count);
+    HB_CUDA(cudaMemcpyAsync(v.data() + at, d, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaStreamSynchronize(st));
+    return HB_OK;
+  };
   k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, f, xw, rw, 1);
   HB_LAUNCHED();
   k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 1, f, rw, bp, 1);
   HB_LAUNCHED();
-  HB_CUDA(cudaMemcpyAsync(xw, bp, sizeof(double) * N * nrhs, cudaMemcpyDeviceToDevice, st));
+  HB_CUDA(cudaMemcpyAsync(xw, bp, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
   HB_CHECK(sweeps(xw));
+  if(trace) {
+    *trace = hb_rbt_trace{};
+    trace->anorm = anorm;
+    HB_CHECK(to_trace(trace->b, bp, n));
+  }
   double om = 0.0, prev = INFINITY;
   int corr = 0;
   for(;;) {
+    if(trace) HB_CHECK(to_trace(trace->x, xw, n));
     HB_CHECK(residual(xw, bp, rw));
     k_rbt_max<<<nrhs, 256, 0, st>>>(N, nrhs, rw, xw, bp, nrm);
     HB_LAUNCHED();
@@ -356,10 +371,16 @@ int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, doub
     for(int q = 0; q < nrhs; q++) {
       const double* m3 = nrm_host + 3 * q;
       const double den = anorm * m3[1] + m3[2];
-      const double w = den > 0.0 ? m3[0] / den : (m3[0] == 0.0 ? 0.0 : INFINITY);
+      double w;
+      if(!std::isfinite(m3[0]) || !std::isfinite(m3[1]) || !std::isfinite(m3[2]) || !std::isfinite(anorm)) w = NAN;
+      else w = den > 0.0 ? m3[0] / den : (m3[0] == 0.0 ? 0.0 : INFINITY);
       om = (w > om || w != w) ? w : om;
     }
-    if(!(corr < HB_RBT_MAX_CORR && om > HB_RBT_EPS && om <= 0.5 * prev)) break;
+    if(trace) {
+      trace->norms.insert(trace->norms.end(), nrm_host, nrm_host + 3 * nrhs);
+      trace->norms.push_back(om);
+    }
+    if(!(std::isfinite(om) && corr < HB_RBT_MAX_CORR && om > HB_RBT_EPS && om <= 0.5 * prev)) break;
     HB_CHECK(sweeps(rw));
     HB_CHECK(hb_vec_axpy(c, (long long)N * nrhs, xw, 1.0, rw));
     corr++;
@@ -372,6 +393,15 @@ int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, doub
   k_rbt_vec<<<tg, 256, 0, st>>>(N, nrhs, 2, f, rw, xw, 0);
   HB_LAUNCHED();
   return std::isfinite(om) ? 1 : 0;
+}
+
+void hb_rbt_trace_out(const hb_rbt_trace& t, int* passes, double* anorm, double* norms, double* xp, double* bp)
+{
+  if(passes) *passes = (int)(t.b.empty() ? 0 : t.x.size() / t.b.size());
+  if(anorm) *anorm = t.anorm;
+  if(norms) std::copy(t.norms.begin(), t.norms.end(), norms);
+  if(xp) std::copy(t.x.begin(), t.x.end(), xp);
+  if(bp) std::copy(t.b.begin(), t.b.end(), bp);
 }
 
 bool hb_rbt_in_place(int N) { return rbt_quarters_of(N).closed; }

@@ -356,7 +356,8 @@ static int plan_sweeps(hb_symdense* s, double* x, int nrhs)
 }
 
 // RBT: hb_rbt_solve on the rows of x (row-major N x nrhs), the sweeps of the NOPIV plan on columns, the residual against the kept A'
-static int rbt_solve(hb_symdense* s, double* x, int nrhs)
+// with its ||A'||_inf, or (tests: hb_debug_symdense_rbt_solve) against a full N x N Aref with anorm
+static int rbt_solve(hb_symdense* s, double* x, int nrhs, hb_rbt_trace* trace = nullptr, const double* Aref = nullptr, double anorm = 0.0)
 {
   hb_ctx* c = s->ctx;
   const int N = s->N;
@@ -372,10 +373,11 @@ static int rbt_solve(hb_symdense* s, double* x, int nrhs)
     HB_CHECK(plan_sweeps(s, s->rbt_col, nrhs));
     return hb_rbt_to_rows(c, N, nrhs, s->rbt_col, v, false);
   };
-  auto residual = [&](const double* xr, const double* b, double* r) { return hb_rbt_rows(c, N, 1, 0, N, s->Ak, N, nrhs, xr, b, r); };
+  const double* Ar = Aref ? Aref : s->Ak.get();
+  auto residual = [&](const double* xr, const double* b, double* r) { return hb_rbt_rows(c, N, 1, 0, N, Ar, N, nrhs, xr, b, r); };
   HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, s->rbt_xw, false));
-  const int ok = hb_rbt_solve(c, N, nrhs, s->rbt_f, s->rbt_anorm, s->rbt_xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual, &s->rbt_corr,
-                              &s->rbt_berr);
+  const int ok = hb_rbt_solve(c, N, nrhs, s->rbt_f, Aref ? anorm : s->rbt_anorm, s->rbt_xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual,
+                              &s->rbt_corr, &s->rbt_berr, trace);
   if(ok < 0) return ok;
   HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, s->rbt_xw, true));
   return ok;
@@ -418,6 +420,23 @@ extern "C" int hb_debug_symdense_rbt(hb_symdense* s, double* Ak_host, double* F_
   if(F_host)
     HB_CUDA(cudaMemcpy2DAsync(F_host, sizeof(double) * N, s->F, sizeof(double) * s->ldf, sizeof(double) * N, N, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
+  return HB_OK;
+}
+
+// diagnostics (tests): one refined RBT solve of x, traced, with the residual and ||.||_inf of Aref / anorm instead of the kept A' when
+// Aref is given (the kept A' is not touched)
+extern "C" int hb_debug_symdense_rbt_solve(hb_symdense* s, double* x, int nrhs, const double* Aref, double anorm, int* ret_host, int* passes_host,
+                                           double* anorm_host, double* norms_host, double* xp_host, double* bp_host)
+{
+  HB_REQUIRE(s && x && nrhs > 0 && s->N > 0, "hb_debug_symdense_rbt_solve: bad arguments");
+  if(!s->factored || s->mode != HB_FACT_RBT_NOPIV)
+    return hb_fail(HB_ERR_STATE, "hb_debug_symdense_rbt_solve: no valid RBT factorization%s", "");
+  HB_CUDA(cudaSetDevice(s->ctx->device));
+  hb_rbt_trace t;
+  const int ok = rbt_solve(s, x, nrhs, &t, Aref, anorm);
+  if(ok < 0) return ok;
+  if(ret_host) *ret_host = ok;
+  hb_rbt_trace_out(t, passes_host, anorm_host, norms_host, xp_host, bp_host);
   return HB_OK;
 }
 

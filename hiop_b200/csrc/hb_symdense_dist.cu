@@ -604,7 +604,7 @@ static int dist_sweeps(hb_symdense_dist* s, double* xw, int nrhs)
 
 // RBT solve on the row-major xw (b in, x out): hb_rbt_solve with the sweeps above, and residual rows formed by the owner of each block
 // row and broadcast, so that the stopping rule reads only replicated values and every rank makes the same decisions.
-static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs)
+static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs, hb_rbt_trace* trace)
 {
   hb_ctx* c = s->ctx;
   const int N = s->N, P = s->P, rank = s->rank, nrows = s->nloc * DB;
@@ -617,15 +617,12 @@ static int rbt_solve(hb_symdense_dist* s, double* xw, int nrhs)
     }
     return HB_OK;
   };
-  return hb_rbt_solve(c, N, nrhs, s->rbt_f, s->rbt_anorm, xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual, &s->rbt_corr, &s->rbt_berr);
+  return hb_rbt_solve(c, N, nrhs, s->rbt_f, s->rbt_anorm, xw, s->rbt_b, s->rbt_r, s->rbt_nrm_host, sweeps, residual, &s->rbt_corr, &s->rbt_berr,
+                      trace);
 }
 
-extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
+static int dist_solve(hb_symdense_dist* s, double* x, int nrhs, hb_rbt_trace* trace)
 {
-  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_dist_solve: bad arguments");
-  if(s->N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_dist_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_dist_solve: no valid factorization (call hb_symdense_dist_matrix_changed)%s", "");
   hb_ctx* c = s->ctx;
   const int N = s->N;
   const bool rbt = s->mode == HB_FACT_RBT_NOPIV;
@@ -646,11 +643,35 @@ extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
   HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, xw, false));
   int ok = 1;
   if(rbt) {
-    ok = rbt_solve(s, xw, nrhs);
+    ok = rbt_solve(s, xw, nrhs, trace);
     if(ok < 0) return ok;
   } else {
     HB_CHECK(dist_sweeps(s, xw, nrhs));
   }
   HB_CHECK(hb_rbt_to_rows(c, N, nrhs, x, xw, true));
   return ok;
+}
+
+extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
+{
+  HB_REQUIRE(s && nrhs >= 0, "hb_symdense_dist_solve: bad arguments");
+  if(s->N == 0 || nrhs == 0) return 1;
+  HB_REQUIRE(x, "hb_symdense_dist_solve: null rhs");
+  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_dist_solve: no valid factorization (call hb_symdense_dist_matrix_changed)%s", "");
+  return dist_solve(s, x, nrhs, nullptr);
+}
+
+// diagnostics (tests): hb_symdense_dist_solve after HB_FACT_RBT_NOPIV, traced (collective)
+extern "C" int hb_debug_symdense_dist_rbt_solve(hb_symdense_dist* s, double* x, int nrhs, int* ret_host, int* passes_host, double* anorm_host,
+                                                double* norms_host, double* xp_host, double* bp_host)
+{
+  HB_REQUIRE(s && x && nrhs > 0 && s->N > 0, "hb_debug_symdense_dist_rbt_solve: bad arguments");
+  if(!s->factored || s->mode != HB_FACT_RBT_NOPIV)
+    return hb_fail(HB_ERR_STATE, "hb_debug_symdense_dist_rbt_solve: no valid RBT factorization%s", "");
+  hb_rbt_trace t;
+  const int ok = dist_solve(s, x, nrhs, &t);
+  if(ok < 0) return ok;
+  if(ret_host) *ret_host = ok;
+  hb_rbt_trace_out(t, passes_host, anorm_host, norms_host, xp_host, bp_host);
+  return HB_OK;
 }

@@ -200,15 +200,25 @@ int hb_symdense_inertia(hb_symdense* s, int* n_neg, int* n_null, int* n_pos);
  * Returns 1 on success, 0 on failure (bool semantics of hiopLinSolver::solve), negative HB_ERR_* on misuse. */
 int hb_symdense_solve(hb_symdense* s, double* x, int nrhs);
 /* After HB_FACT_RBT_NOPIV, solve refines like hb_symdense_dist_solve: b' = U^T b, the sweeps of the no-pivot factor, refinement against
- * the kept A' with omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf) (correct while omega > 2^-52,
- * fewer than 3 corrections were made and omega is at most half its value before the last correction), x = U x'; 0 when omega is not
- * finite. hb_symdense_rbt_stats: the last RBT solve's corrections and omega, and the last RBT factorization's transform time (ms,
- * device events, every factorization). Every output may be NULL. */
+ * the kept A' with omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf), x = U x'. A column's quotient is
+ * NaN when one of its three norms or ||A'||_inf is not finite, +inf when the denominator is 0 and the residual is not, 0 for a zero column;
+ * a NaN wins the max. Correct while omega is finite, omega > 2^-52, fewer than 3 corrections were made and omega is at most half its
+ * value before the last correction. Returns 0 when omega is not finite (no correction is made after such an omega). hb_symdense_rbt_stats:
+ * the last RBT solve's corrections and omega, and the last RBT factorization's transform time (ms, device events, every factorization).
+ * Every output may be NULL. */
 int hb_symdense_rbt_stats(hb_symdense* s, int* corrections, double* backward_error, float* transform_ms);
 /* diagnostics (tests): the RBT transform of the upper triangle of M without factoring (the handle then holds no factorization): A'
  * (N x N row-major, full) and the factor buffer the factorization would read (N x N row-major, upper triangle = A', unpadded). Either
  * output may be NULL. */
 int hb_debug_symdense_rbt(hb_symdense* s, double* Aprime_host, double* F_host);
+/* diagnostics (tests): one hb_symdense_solve of x (device, nrhs >= 1) after HB_FACT_RBT_NOPIV, traced. With Aref (device, N x N
+ * row-major, full) the refinement forms its residuals with Aref and its omegas with anorm instead of the kept A' and ||A'||_inf (which
+ * stay untouched); with Aref NULL, anorm is ignored. Synchronises the stream; every output may be NULL. ret_host: the solve's value (1 or
+ * 0). passes_host: residuals formed (corrections + 1). anorm_host: the ||A'||_inf used. norms_host: per pass, max |r|, max |x'|, max |b'| of
+ * every rhs, then omega (at most 4 (3 nrhs + 1) doubles). xp_host: per pass, x' before its residual (row-major N x nrhs, at most 4 N nrhs
+ * doubles). bp_host: b' (row-major N x nrhs). */
+int hb_debug_symdense_rbt_solve(hb_symdense* s, double* x, int nrhs, const double* Aref, double anorm, int* ret_host, int* passes_host,
+                                double* anorm_host, double* norms_host, double* xp_host, double* bp_host);
 /* The tile schedule of the one-pass RBT transform (k_rbt_fused, hb_rbt.cu) for order N, run on the host (no device needed). dims4 =
  * {tiles T, CTAs C, window rows W, output rows O}. CTA b takes the tile pair ctas_host[2b .. 2b+1] = {bi, bj}, bi <= bj, and computes
  * A'(i, j) for i among the output rows of tile bi and j among those of tile bj from the entries A(r, c) (read as A(min, max)) with r
@@ -273,8 +283,10 @@ int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_null, int* 
 /* x: N x nrhs (one rhs after the other, device), replicated on every rank in and out. 1 / 0 / HB_ERR_* like hb_symdense_solve.
  * After HB_FACT_RBT_NOPIV: b' = U^T b, the two sweeps of the factor, then refinement against the kept A' (the owner of each block row
  * forms its rows of b' - A' x' in a fixed order and broadcasts them), x = U x'. Stopping rule, on values every rank holds alike:
- * omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf); correct while omega > 2^-52, fewer than 3
- * corrections were made and omega is at most half its value before the last correction. Returns 0 when omega is not finite. */
+ * omega = max over the rhs of ||b' - A' x'||_inf / (||A'||_inf ||x'||_inf + ||b'||_inf), with the column quotients of hb_symdense_solve
+ * (NaN for a non-finite norm, +inf for a zero denominator under a non-zero residual, 0 for a zero column); correct while omega is finite,
+ * omega > 2^-52, fewer than 3 corrections were made and omega is at most half its value before the last correction. Returns 0 when omega
+ * is not finite, on every rank. */
 int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs);
 /* the last RBT solve's corrections and omega (above), and the last RBT factorization's mirror + butterfly time (ms, device events, only
  * while hb_symdense_dist_profile is on; 0 otherwise). Every output may be NULL. */
@@ -282,6 +294,10 @@ int hb_symdense_dist_rbt_stats(hb_symdense_dist* s, int* corrections, double* ba
 /* diagnostics (tests): the first `stages` steps of the RBT transform on the owned block rows, in place and without factoring (collective;
  * 0: the mirrored full rows, 1: B2^T A B2, 2: A'); the handle then holds no factorization. */
 int hb_debug_symdense_dist_rbt(hb_symdense_dist* s, int stages);
+/* diagnostics (tests): hb_symdense_dist_solve after HB_FACT_RBT_NOPIV, traced like hb_debug_symdense_rbt_solve (collective; the outputs
+ * are this rank's copies of the replicated values). */
+int hb_debug_symdense_dist_rbt_solve(hb_symdense_dist* s, double* x, int nrhs, int* ret_host, int* passes_host, double* anorm_host,
+                                     double* norms_host, double* xp_host, double* bp_host);
 /* diagnostics (tools/bench_dist_symdense.py): on != 0 times the phases of every following factorization with device events; on == 0
  * stops and returns this rank's sums (ms) over the steps of the last one: panel chain (owner's k_diag128 + k_trsm_panel + packing),
  * broadcast (including the wait for the owner), trailing update on the update stream. ms3 may be NULL. */

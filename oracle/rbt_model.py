@@ -145,19 +145,24 @@ def U_matrix(N: int) -> np.ndarray:
     return apply_U(np.eye(N))
 
 
-def nopiv_ldlt(A: np.ndarray):
+def nopiv_ldlt(A: np.ndarray, nb: int = 128):
     """LDL^T without pivoting of a full symmetric A: (L, d, ret) with ret the value hb_symdense_dist_matrix_changed gives (number of
-    negative pivots, -1 for a zero or non-finite pivot or |d| < 1e-14)"""
+    negative pivots, -1 for a zero or non-finite pivot or |d| < 1e-14). Right-looking in blocks of nb: the columns of a block one by one
+    (with the block's rows), then one product L S for the trailing matrix, S the block's rows of the Schur complement.""" 
     N = A.shape[0]
     S = np.array(A, dtype=np.float64)
     L = np.eye(N)
     d = np.zeros(N)
-    for k in range(N):
-        d[k] = S[k, k]
-        if d[k] == 0.0 or not np.isfinite(d[k]):
-            return L, d, -1
-        L[k + 1:, k] = S[k + 1:, k] / d[k]
-        S[k + 1:, k + 1:] -= np.outer(L[k + 1:, k], S[k, k + 1:])
+    for k0 in range(0, N, nb):
+        k1 = min(k0 + nb, N)
+        for k in range(k0, k1):
+            d[k] = S[k, k]
+            if d[k] == 0.0 or not np.isfinite(d[k]):
+                return L, d, -1
+            L[k + 1:, k] = S[k + 1:, k] / d[k]
+            S[k + 1:, k + 1:k1] -= np.outer(L[k + 1:, k], S[k, k + 1:k1])
+            S[k + 1:k1, k1:] -= np.outer(L[k + 1:k1, k], S[k, k1:])
+        S[k1:, k1:] -= L[k1:, k0:k1] @ S[k0:k1, k1:]
     return L, d, inertia_ret(d)
 
 
@@ -202,34 +207,66 @@ def dsytrf_inertia(A: np.ndarray):
     return neg, nul, pos
 
 
-def backward_error(A, x, b) -> float:
-    """||b - A x||_inf / (||A||_inf ||x||_inf + ||b||_inf), the largest over the columns of x, b"""
+def column_omegas(nA, num, xn, bn):
+    """the stopping rule's quotient per column from ||A||_inf and the per-column max |r|, max |x|, max |b|: num / (nA xn + bn), NaN where
+    one of the four is not finite, +inf where the denominator is 0 and num is not, 0 for a zero column"""
+    num, xn, bn = (np.asarray(v, dtype=np.float64) for v in (num, xn, bn))
+    finite = np.isfinite(num) & np.isfinite(xn) & np.isfinite(bn) & np.isfinite(nA)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        den = nA * xn + bn
+        w = np.where(den > 0, num / np.where(den > 0, den, 1.0), np.where(num == 0, 0.0, np.inf))
+    return np.where(finite, w, np.nan)
+
+
+def nan_max(w) -> float:
+    """the largest entry, NaN if there is one, 0 for none"""
+    w = np.asarray(w, dtype=np.float64)
+    return float(np.max(w)) if w.size else 0.0
+
+
+def backward_error(A, x, b, nA=None) -> float:
+    """||b - A x||_inf / (||A||_inf ||x||_inf + ||b||_inf), the largest over the columns of x, b (column_omegas; a NaN wins). nA replaces
+    ||A||_inf."""
     x2, b2 = x.reshape(A.shape[0], -1), b.reshape(A.shape[0], -1)
-    nA = np.abs(A).sum(axis=1).max(initial=0.0)
-    r = b2 - A @ x2
-    num = np.abs(r).max(axis=0)
-    den = nA * np.abs(x2).max(axis=0) + np.abs(b2).max(axis=0)
-    return float(np.max(num / np.where(den > 0, den, 1.0), initial=0.0))
+    if nA is None:
+        nA = np.abs(A).sum(axis=1).max(initial=0.0)
+    with np.errstate(invalid="ignore", over="ignore"):
+        r = b2 - A @ x2
+    return nan_max(column_omegas(nA, np.abs(r).max(axis=0), np.abs(x2).max(axis=0), np.abs(b2).max(axis=0)))
 
 
 def solve(A: np.ndarray, b: np.ndarray):
-    """A x = b through A' = U^T A U, its no-pivot LDL^T and refinement against A' with the rule of hb_symdense_dist_solve:
-    correct while the backward error exceeds EPS, fewer than MAX_CORRECTIONS corrections were made and the last correction at least
-    halved it. Returns (x, corrections, backward error against A')."""
-    Ap = transform(A)
-    L, d, ret = nopiv_ldlt(Ap)
+    """A x = b through A' = U^T A U, its no-pivot LDL^T and refinement against A' with the rule of hb_symdense_solve /
+    hb_symdense_dist_solve (refine). Returns (x, corrections, backward error against A')."""
+    return refine(A, b)[:3]
+
+
+def refine(A: np.ndarray, b: np.ndarray, Aref=None, anorm=None, Ap=None, factor=None):
+    """solve with every exit of the refinement visible: correct while omega is finite, omega > EPS, fewer than MAX_CORRECTIONS
+    corrections were made and the last correction at least halved it. The residuals and omegas are against A' and ||A'||_inf, or against
+    Aref (full, in the transformed basis) and anorm when given (anorm defaults to ||Aref||_inf). Ap, factor: A' and nopiv_ldlt(A') when the
+    caller has them already. Returns (x, corrections, omega, omegas, ret): omegas = every omega the rule read, ret = 1 when the last one
+    is finite, else 0."""
+    Ap = transform(A) if Ap is None else Ap
+    L, d, ret = nopiv_ldlt(Ap) if factor is None else factor
     assert ret >= 0, ret
     from scipy.linalg import solve_triangular
+    Ar = Ap if Aref is None else Aref
+    nA = np.abs(Ar).sum(axis=1).max(initial=0.0) if anorm is None else anorm
 
     def ldl_solve(v):
-        y = solve_triangular(L, v, lower=True, unit_diagonal=True)
-        return solve_triangular(L.T, y / (d if y.ndim == 1 else d[:, None]), lower=False, unit_diagonal=True)
+        y = solve_triangular(L, v, lower=True, unit_diagonal=True, check_finite=False)
+        return solve_triangular(L.T, y / (d if y.ndim == 1 else d[:, None]), lower=False, unit_diagonal=True, check_finite=False)
 
     bp = apply_UT(b)
-    xp = ldl_solve(bp)
-    om, prev, corr = backward_error(Ap, xp, bp), np.inf, 0
-    while corr < MAX_CORRECTIONS and om > EPS and om <= 0.5 * prev:
-        xp = xp + ldl_solve(bp - Ap @ xp)
-        corr += 1
-        prev, om = om, backward_error(Ap, xp, bp)
-    return apply_U(xp), corr, om
+    with np.errstate(invalid="ignore", over="ignore"):
+        xp = ldl_solve(bp)
+        om, prev, corr = backward_error(Ar, xp, bp, nA), np.inf, 0
+        oms = [om]
+        while np.isfinite(om) and corr < MAX_CORRECTIONS and om > EPS and om <= 0.5 * prev:
+            xp = xp + ldl_solve(bp - Ar @ xp)
+            corr += 1
+            prev, om = om, backward_error(Ar, xp, bp, nA)
+            oms.append(om)
+        x = apply_U(xp)
+    return x, corr, om, oms, int(np.isfinite(om))

@@ -123,3 +123,107 @@ def test_model_solve_reaches_the_refinement_rule(name):
     assert corr <= rbt.MAX_CORRECTIONS
     assert om <= 4 * rbt.EPS, (corr, om)
     assert rbt.backward_error(A, x, b) <= 1e-14
+
+
+@pytest.mark.parametrize("name", list(FAMILIES))
+def test_model_refine_records_what_solve_returns(name):
+    """refine's omega history ends in solve's omega after solve's corrections, and its x is solve's, bit for bit"""
+    A = FAMILIES[name]
+    N = A.shape[0]
+    b = np.random.default_rng(N).standard_normal((N, 2))
+    x, corr, om = rbt.solve(A, b)
+    x2, corr2, om2, oms, ret = rbt.refine(A, b)
+    assert np.array_equal(x.view(np.uint64), x2.view(np.uint64)) and (corr2, om2) == (corr, om)
+    assert ret == 1 and len(oms) == corr + 1 and oms[-1] == om
+
+
+# ---- the stopping rule of the refinement on non-finite values and at every exit --------------------------------------------------------
+def test_column_omegas_on_non_finite_and_zero_columns():
+    nan, inf = np.nan, np.inf
+    w = rbt.column_omegas(2.0, [1.0, 0.0, nan, 1.0, 1.0, 1.0, inf, 3.0], [1.0, 0.0, 1.0, nan, inf, 1.0, 1.0, 0.0],
+                          [2.0, 0.0, 1.0, 1.0, 1.0, inf, 1.0, 0.0])
+    assert w[0] == 0.25 and w[1] == 0.0                                # a finite column; a zero column stays 0
+    assert np.isnan(w[2:7]).all()                                      # any non-finite norm: NaN, never 0 or +inf
+    assert w[7] == np.inf                                              # zero denominator under a non-zero residual
+    assert np.isnan(rbt.column_omegas(inf, [1.0, 0.0], [1.0, 0.0], [1.0, 0.0])).all()   # ||A||_inf overflowed: NaN, not "converged"
+    assert np.isnan(rbt.nan_max([0.5, nan, 1.0])) and rbt.nan_max([0.5, inf]) == inf and rbt.nan_max([]) == 0.0
+    A = np.eye(3)
+    assert np.isnan(rbt.backward_error(A, np.array([1.0, nan, 0.0]), np.ones(3)))
+    assert rbt.backward_error(A, np.zeros((3, 2)), np.zeros((3, 2))) == 0.0
+
+
+CAP_RATIO = 1.0 + 2.0 ** -8       # Aref = A' (1 + 2^-8): each correction contracts the error by 2^-8
+DIVERGE_RATIO = 2.0 + 2.0 ** -4   # Aref = A' (2 + 2^-4): the error grows by 17/16, and omega by about 17 in the first correction
+PLACED_MIN_N = 129                # below, ||A'|| ||x'|| / ||b'|| is too small for stagnation and divergence to clear 0.5 omega by 10x
+
+
+def placed_reference(Ap, case):
+    """(Aref, anorm) of a placed exit on the model's A': anorm is ||Aref||_inf, or +inf for the overflow case"""
+    if case == "overflow":
+        return Ap, np.inf
+    Aref = Ap * {"cap": CAP_RATIO, "stagnation": 2.0, "divergence": DIVERGE_RATIO}[case]
+    return Aref, float(np.abs(Aref).sum(axis=1).max())
+
+
+def placed_rhs(N, nrhs, case, seed):
+    """the right-hand side of a placed exit: zero; a NaN or +Inf in column 1 of a 3-column b; else standard normal"""
+    b = np.random.default_rng(seed).standard_normal((N, nrhs))
+    if case == "zero":
+        return np.zeros((N, nrhs))
+    if case in ("nan", "inf"):
+        b[N // 2, 1] = np.nan if case == "nan" else np.inf
+    return b
+
+
+# every placed exit: corrections, return value, and what the last omega is
+PLACED = {"zero": (0, 1, "zero"), "cap": (3, 1, "finite"), "stagnation": (1, 1, "finite"), "divergence": (1, 1, "finite"),
+          "nan": (0, 0, "nan"), "inf": (0, 0, "nan"), "overflow": (0, 0, "nan")}
+
+
+def assert_placed(case, corr, ret, oms):
+    """the exit of `case` from a solve's corrections, return value and omega sequence, with the sequence at least a factor 10 away from
+    EPS and from 0.5 omega_prev wherever the rule compares them"""
+    want_corr, want_ret, last = PLACED[case]
+    assert (corr, ret, len(oms)) == (want_corr, want_ret, want_corr + 1), (case, corr, ret, oms)
+    if last == "zero":
+        assert oms == [0.0]
+    elif last == "nan":
+        assert np.isnan(oms[-1])
+    for k, om in enumerate(oms if last == "finite" else []):
+        assert om >= 10 * rbt.EPS, (case, k, oms)
+        if k:
+            assert om >= 10 * 0.5 * oms[k - 1] or om <= 0.1 * 0.5 * oms[k - 1], (case, k, oms)
+    if case == "cap":
+        assert all(oms[k] <= 0.1 * 0.5 * oms[k - 1] for k in (1, 2, 3))
+    if case in ("stagnation", "divergence"):
+        assert oms[1] > 10 * 0.5 * oms[0] and oms[1] > oms[0]
+
+
+@pytest.mark.parametrize("case,N", [(c, N) for c in PLACED for N in (1, 2, 3, 129, 1000)
+                                    if N >= PLACED_MIN_N or c not in ("stagnation", "divergence")])
+def test_model_places_every_exit(case, N):
+    A = known_matrix(N)
+    Ap = rbt.transform(A)
+    nrhs = 3 if case in ("nan", "inf") else 1 + (N % 2) * 2
+    b = placed_rhs(N, nrhs, case, seed=N)
+    Aref, anorm = placed_reference(Ap, case) if case in ("cap", "stagnation", "divergence", "overflow") else (None, None)
+    x, corr, om, oms, ret = rbt.refine(A, b, Aref=Aref, anorm=anorm, Ap=Ap)
+    assert_placed(case, corr, ret, oms)
+    assert om == oms[-1] or (np.isnan(om) and np.isnan(oms[-1]))
+    if case == "zero":
+        assert np.array_equal(x, np.zeros_like(x))
+    if case == "divergence":
+        assert_corrected_x(A, b, x)
+
+
+def assert_corrected_x(A, b, x):
+    """divergence returns the corrected x: x'_1 = x'_0 + A'^-1 (b' - c A' x'_0) = (2 - c) x'_0, 16 times smaller than the first solve's.
+    The first solve is ~1e-8 from A^-1 b (the growth of the no-pivot factor of A'); an uncorrected x would be 15/16 of |x| away."""
+    xs = np.linalg.solve(A, b)
+    assert np.abs(x - (2.0 - DIVERGE_RATIO) * xs).max() <= 1e-6 * np.abs(xs).max()
+
+
+def known_matrix(N):
+    """the matrix of order N of the placed exits and the GPU refinement tests"""
+    from oracle import bounds
+    return bounds.known_inertia_matrix(N, N // 8, N // 3, seed=N)[0].numpy()
