@@ -190,6 +190,19 @@ __device__ __forceinline__ double rbt_entry(double all, double ahh, double alh, 
   return __dmul_rn(__dmul_rn(fi, fj), __dmul_rn(t, w));
 }
 
+// ---- the per-block kernels of hb_symdense_dist (hb_symdense_dist.cu), shared with the host-resident handle (hb_symdense_host.cu) ----
+// Ak addresses block row k like the factor: Ak[(k0 + p) * ld + i] = L(i, k0 + p) for the rows i >= k0 of column k0 + p.
+int hb_dist_init_attrs();
+// L[c * ldb + i] = W[c * ldb + i] * hdr[c] (i < rows, c < 128: k_trsm_panel's L = W D^-1, bit for bit); folds the int at hdr + 128 into
+// *info when it is non-zero and *info is still 0
+int hb_dist_form_l(hb_ctx* c, const double* hdr, const double* W, long long ldb, int rows, double* L, int* info, cudaStream_t st);
+// out3 = {neg, null, pos} of the diagonal entries A[e * ld + k0 + t] (e = q * 128 + t of the nloc owned blocks) with the +-1e-14 rule
+int hb_dist_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st);
+// the forward step of block k on the row-major N x nrhs xw (y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, LDL^T: z_k = y_k / d_k), and the
+// backward step (x_k = L_kk^-T (z_k - L_>k,k^T x_>k)); ybuf, tdot: 128 nrhs doubles
+int hb_dist_fwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* ybuf, cudaStream_t st);
+int hb_dist_bwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* tdot, cudaStream_t st);
+
 // global row of local row y of rank `rank` in the block-cyclic layout (P = 1: y)
 __host__ __device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / HB_DIST_DB) * P + rank) * HB_DIST_DB + y % HB_DIST_DB; }
 

@@ -221,6 +221,52 @@ int agree(hb_ctx* c, int rc)
 
 } // namespace
 
+// ---- the per-block kernels above, for this file and the host-resident handle (hb_symdense_host.cu) ----
+int hb_dist_init_attrs()
+{
+  HB_CUDA(cudaFuncSetAttribute(k_dist_fwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
+  HB_CUDA(cudaFuncSetAttribute(k_dist_bwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
+  return HB_OK;
+}
+
+int hb_dist_form_l(hb_ctx* c, const double* hdr, const double* W, long long ldb, int rows, double* L, int* info, cudaStream_t st)
+{
+  k_dist_recv<<<hb_grid(c, DB * ldb), 256, 0, st>>>(hdr, W, ldb, rows, 1, L, info);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+int hb_dist_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st)
+{
+  k_dist_inertia<<<1, 1024, 0, st>>>(A, ld, N, P, rank, nloc, out3);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+int hb_dist_fwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* ybuf, cudaStream_t st)
+{
+  const int nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb, ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
+  k_dist_fwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, ybuf);
+  HB_LAUNCHED();
+  if(rows > 0) {
+    k_dist_fwd_panel<<<(rows + 255) / 256, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, ybuf);
+    HB_LAUNCHED();
+  }
+  return HB_OK;
+}
+
+int hb_dist_bwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* tdot, cudaStream_t st)
+{
+  const int nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb, ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
+  if(rows > 0) {
+    k_dist_bwd_dots<<<nb, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, tdot);
+    HB_LAUNCHED();
+  }
+  k_dist_bwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, rows > 0 ? tdot : nullptr);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
 struct hb_symdense_dist
 {
   hb_ctx* ctx = nullptr;
@@ -307,8 +353,7 @@ extern "C" int hb_symdense_dist_create(hb_ctx* c, int N, hb_symdense_dist** out)
       HB_CHECK(s->ev_free[b].create(cudaEventDisableTiming));
     }
     HB_CHECK(s->ev_join.create(cudaEventDisableTiming));
-    HB_CUDA(cudaFuncSetAttribute(k_dist_fwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
-    HB_CUDA(cudaFuncSetAttribute(k_dist_bwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
+    HB_CHECK(hb_dist_init_attrs());
     HB_CUDA(cudaStreamSynchronize(c->stream));
     return HB_OK;
   };
@@ -533,8 +578,7 @@ extern "C" int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode)
   }
   HB_CUDA(cudaEventRecord(s->ev_join, sp));
   HB_CUDA(cudaStreamWaitEvent(su, s->ev_join, 0));
-  k_dist_inertia<<<1, 1024, 0, su>>>(A, ld, N, P, rank, s->nloc, s->red);
-  HB_LAUNCHED();
+  HB_CHECK(hb_dist_inertia(A, ld, N, P, rank, s->nloc, s->red, su));
   HB_CHECK(hb_allreduce_op(c, s->red, 3, HB_SUM));
   HB_CUDA(cudaMemcpyAsync(s->red_host, s->red, sizeof(double) * 3, cudaMemcpyDeviceToHost, su));
   HB_CUDA(cudaMemcpyAsync(s->info_host, s->info, sizeof(int), cudaMemcpyDeviceToHost, su));
@@ -572,31 +616,14 @@ static int dist_sweeps(hb_symdense_dist* s, double* xw, int nrhs)
   const bool ldl = s->mode != HB_FACT_CHOLESKY;
   const long long ld = s->ld;
   cudaStream_t st = c->stream;
-  const int ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
   for(int k = 0; k < s->nblk; k++) {
-    const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb;
-    if(owner == rank) {
-      const double* Ak = s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld;
-      k_dist_fwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, s->ybuf);
-      HB_LAUNCHED();
-      if(rows > 0) {
-        k_dist_fwd_panel<<<(rows + 255) / 256, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, s->ybuf);
-        HB_LAUNCHED();
-      }
-    }
+    const int owner = k % P, k0 = k * DB;
+    if(owner == rank) HB_CHECK(hb_dist_fwd_block(s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld, ld, N, k0, ldl, xw, nrhs, s->ybuf, st));
     HB_CHECK(hb_broadcast(c, xw + (size_t)k0 * nrhs, (long long)(N - k0) * nrhs, owner, st));
   }
   for(int k = s->nblk - 1; k >= 0; k--) {
-    const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb;
-    if(owner == rank) {
-      const double* Ak = s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld;
-      if(rows > 0) {
-        k_dist_bwd_dots<<<nb, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, s->tdot);
-        HB_LAUNCHED();
-      }
-      k_dist_bwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, rows > 0 ? s->tdot.get() : nullptr);
-      HB_LAUNCHED();
-    }
+    const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
+    if(owner == rank) HB_CHECK(hb_dist_bwd_block(s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld, ld, N, k0, ldl, xw, nrhs, s->tdot, st));
     HB_CHECK(hb_broadcast(c, xw + (size_t)k0 * nrhs, (long long)nb * nrhs, owner, st));
   }
   return HB_OK;

@@ -305,6 +305,68 @@ class LinSolverSymDenseDist:
         return n.value, be.value, float(ms.value)
 
 
+class LinSolverSymDenseHost:
+    """The dense symmetric solver of one GPU with the matrix in page-locked host memory (hb_symdense_host): Cholesky or no-pivot LDL^T,
+    streamed through at most `device_bytes` of device memory (0: what is free, less a margin) in slabs of 128-row block rows. It owns
+    a pinned n x n host tensor, matrix(); the caller fills its upper triangle, matrixChanged(mode) overwrites that triangle with the
+    factor and returns what LinSolverSymDense.matrixChanged does, solve(x) solves in place on the device. Bunch-Kaufman and RBT_NOPIV
+    are refused (use LinSolverSymDense, or LinSolverSymDenseDist for the safe mode)."""
+
+    NOPIV, CHOLESKY = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY
+
+    def __init__(self, ctx: Context, n: int, device_bytes: int = 0):
+        self.ctx, self.n = ctx, n
+        self.h = ctypes.c_void_p()
+        check(ctx.L.hb_symdense_host_create(ctx.h, n, device_bytes, ctypes.byref(self.h)), "hb_symdense_host_create")
+        self._M = torch.empty((n, n), dtype=torch.float64, pin_memory=True)
+        check(ctx.L.hb_symdense_host_set_matrix(self.h, ctypes.c_void_p(self._M.data_ptr() if n else None), max(n, 1)),
+              "hb_symdense_host_set_matrix")
+
+    def close(self):
+        if self.h:
+            self.ctx.L.hb_symdense_host_destroy(self.h)
+            self.h = None
+            self._M = None
+
+    def matrix(self) -> torch.Tensor:
+        """the pinned n x n row-major host matrix the handle factors in place (upper triangle)"""
+        return self._M
+
+    def matrixChanged(self, mode: int) -> int:
+        if mode not in (self.NOPIV, self.CHOLESKY):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
+            raise EngineError("LinSolverSymDenseHost: only CHOLESKY and NOPIV stream from host memory; use LinSolverSymDense for "
+                              "Bunch-Kaufman, LinSolverSymDenseDist for RBT_NOPIV")
+        rc = self.ctx.L.hb_symdense_host_matrix_changed(self.h, mode)
+        if rc < -1:
+            check(rc, "hb_symdense_host_matrix_changed")
+        return rc
+
+    def inertia(self):
+        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        check(self.ctx.L.hb_symdense_host_inertia(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "hb_symdense_host_inertia")
+        return a.value, b.value, c.value
+
+    def solve(self, x: torch.Tensor) -> bool:
+        nrhs = x.numel() // max(self.n, 1) if self.n else 0
+        rc = self.ctx.L.hb_symdense_host_solve(self.h, _ptr(x), nrhs)
+        if rc < 0:
+            check(rc, "hb_symdense_host_solve")
+        return rc == 1
+
+    @staticmethod
+    def plan_view(n: int, device_bytes: int) -> dict:
+        """the slab plan of a handle of order n under device_bytes (host only): slabs, block rows, block rows per slab, the first block
+        row of each slab (and the count at the end), peak device bytes, and the bytes one factorization / solve copies"""
+        L = _lib.lib()
+        dims = (ctypes.c_int * 3)()
+        nblk = (n + 127) // 128
+        first = (ctypes.c_int * (nblk + 1))()
+        b = (ctypes.c_longlong * 5)()
+        check(L.hb_symdense_host_plan_view(n, device_bytes, dims, first, b), "hb_symdense_host_plan_view")
+        return {"slabs": dims[0], "blocks": dims[1], "slab_blocks": dims[2], "first": [first[i] for i in range(dims[0] + 1)],
+                "peak_bytes": b[0], "h2d_bytes": b[1], "d2h_bytes_cholesky": b[2], "d2h_bytes_ldlt": b[3], "solve_h2d_bytes": b[4]}
+
+
 class KKTLinSysLowRank:
     """hiopKKTLinSysLowRank with the hiopHessianLowRank state it drives.
 

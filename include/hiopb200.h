@@ -39,6 +39,7 @@ typedef struct hb_lowrank hb_lowrank;
 typedef struct hb_symdense hb_symdense;
 typedef struct hb_mds hb_mds;
 typedef struct hb_symdense_dist hb_symdense_dist;
+typedef struct hb_symdense_host hb_symdense_host;
 
 /* ------------------------------------------------------------------------------------------------------------
  * Context, memory, streams
@@ -302,6 +303,48 @@ int hb_debug_symdense_dist_rbt_solve(hb_symdense_dist* s, double* x, int nrhs, i
  * stops and returns this rank's sums (ms) over the steps of the last one: panel chain (owner's k_diag128 + k_trsm_panel + packing),
  * broadcast (including the wait for the owner), trailing update on the update stream. ms3 may be NULL. */
 int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3);
+
+/* ---- the same system on one GPU with the matrix in page-locked host memory (hb_symdense_host.cu) ----
+ * For orders whose N x N matrix does not fit the device (about 100 000 on an 80 GB card): the matrix stays in the caller's page-locked
+ * buffer and is streamed through HBM. Cholesky and no-pivot LDL^T on the 128-row block rows of hb_symdense_dist at P = 1, left-looking
+ * over slabs (runs of consecutive block rows): each slab is copied in, the block rows factored before it are streamed through a ring of
+ * two panel buffers and applied in ascending order with the same K = 128 update kernel, the slab's own block rows are factored as the
+ * P = 1 distributed loop does, and the slab is copied back. The factor, the return value and the inertia are bit-identical to
+ * hb_symdense_dist at P = 1 (hence to hb_symdense with unpaired blocks) for every slab plan, and so are the solutions.
+ * Bunch-Kaufman (its pivot search needs up-to-date columns) and HB_FACT_RBT_NOPIV (the butterfly needs partner rows and both triangles)
+ * are refused with HB_ERR_INVALID and the handle stays usable; for the safe mode beyond one GPU use hb_symdense_dist.
+ *
+ * device_bytes: the device memory the handle may hold: the slab, the ring (4 x 128 ld doubles, ld = N rounded up to 8), 1/d and the
+ * 16 x 16 inverses, the factor's diagonal and the scratch of a solve of 16 right-hand sides. The slab height is the largest multiple of 128
+ * rows that fits (all N rows: one slab); 0 takes what is free less 5 % (at least 256 MiB). The handle makes one device allocation of that
+ * many bytes at create (the driver rounds it up to its allocation granularity); HB_ERR_INVALID below one block row plus the rest,
+ * HB_ERR_ALLOC when the allocation fails. */
+int hb_symdense_host_create(hb_ctx* ctx, int N, size_t device_bytes, hb_symdense_host** out);
+int hb_symdense_host_destroy(hb_symdense_host* s);
+/* M_host: the caller's N x N row-major buffer (leading dimension ld >= N), borrowed until the next call: page-locked (hb_malloc_host or
+ * hb_host_register; HB_ERR_INVALID otherwise, checked at both ends). The caller fills its upper triangle before each factorization; the
+ * factorization overwrites the upper triangle in place with the factor, stored as hb_symdense stores it. No kernel reads or writes the
+ * strictly lower triangle; the strictly lower entries of the 128 x 128 diagonal blocks make the round trip through the device with the
+ * copies of their block rows and come back unchanged. Drops the factorization. */
+int hb_symdense_host_set_matrix(hb_symdense_host* s, double* M_host, long long ld);
+/* HB_FACT_CHOLESKY or HB_FACT_NOPIV; returns what hb_symdense_dist_matrix_changed returns (>= 0: negative eigenvalues, -1: null pivot
+ * or breakdown; the factorization runs to its last block either way). Synchronous: the factor is in the host buffer on return.
+ * Traffic per factorization (hb_symdense_host_plan_view): the matrix in and the factor out once, plus per slab starting at block b0 the
+ * 128 b0 (N - 128 b0) doubles of the block rows before it; LDL^T with several slabs streams W = L D instead of L and keeps it in pinned
+ * host memory the handle allocates on its first such factorization (about 4 N^2 bytes; HB_ERR_ALLOC leaves the handle usable). */
+int hb_symdense_host_matrix_changed(hb_symdense_host* s, int mode);
+int hb_symdense_host_inertia(hb_symdense_host* s, int* n_neg, int* n_null, int* n_pos);
+/* x: N x nrhs (one rhs after the other, device), in place on the context stream; 1 / 0 / HB_ERR_* like hb_symdense_solve (HB_ERR_STATE
+ * without a valid factorization). The per-block kernels of hb_symdense_dist_solve, so the solutions are bit-identical to it at P = 1 for
+ * every nrhs. With a one-slab plan the factor stays on the device and the solve reads it there. Otherwise every group of up to 16
+ * right-hand sides streams the factor's block rows from the host buffer twice (forward and backward sweep): about 8 N^2 bytes of H2D
+ * traffic, and the call returns after its last read of the buffer. */
+int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs);
+/* The plan of hb_symdense_host_create(N, device_bytes > 0), made on the host (no device needed). dims: {slabs, block rows, block rows per
+ * slab}. slab_first_block_host: slabs + 1 entries, the first block row of each slab and then the number of block rows. bytes_host: {peak
+ * device bytes, H2D bytes per factorization, D2H bytes per Cholesky factorization, D2H bytes per LDL^T factorization, H2D bytes per
+ * solve of up to 16 right-hand sides (0 with one slab)}. Every output may be NULL. */
+int hb_symdense_host_plan_view(int N, size_t device_bytes, int* dims, int* slab_first_block_host, long long* bytes_host);
 
 /* ------------------------------------------------------------------------------------------------------------
  * hiopKKTLinSysLowRank + hiopHessianLowRank (B2; src/Optimization/hiopKKTLinSys.cpp:1031-1350,
