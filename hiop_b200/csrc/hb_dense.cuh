@@ -119,7 +119,7 @@ int hb_big_init(hb_ctx* c, hb_big* b);
 int hb_big_reserve(hb_ctx* c, hb_big* b, int N, bool need_w);
 // pairs: factor the 128-column blocks in pairs (K = 256 trailing updates)
 int hb_big_factor(hb_ctx* c, hb_big* b, int N, double* A, long long lda, bool ldl, bool pairs, int* info_dev);
-// the per-block pieces of hb_big_factor, for the distributed factorization (hb_symdense_dist.cu): one panel step (k_diag128 +
+// the per-block pieces of hb_big_factor, for the block-row step loop (hb_blockrow.cu): one panel step (k_diag128 +
 // k_trsm_panel) and the K = 128 trailing update on a block-cyclic matrix
 int hb_big_panel(int N, double* A, long long lda, int k0, bool ldl, double* inv16, double* dinv, double* W, long long ldw, int* info_dev, cudaStream_t st);
 int hb_big_update_cyclic(int N, const double* P, long long ldp, const double* Q, long long ldq, int qsub, double* C, long long ldc, int nranks, int rank,
@@ -149,7 +149,6 @@ int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int*
 constexpr double HB_RBT_C = 0.7071067811865476; // the double nearest 1/sqrt(2)
 constexpr double HB_RBT_EPS = 0x1p-52;          // refinement target of the backward error
 constexpr int HB_RBT_MAX_CORR = 3;
-constexpr int HB_DIST_DB = 128;                 // block size of the block-cyclic layout of hb_symdense_dist (rows of one block)
 
 // the entries of column i of a level's butterfly: rows lo and hi (lo = hi = i when unpaired), sign s of the hi side (+1 on the lo side)
 struct rbt_pos
@@ -190,21 +189,54 @@ __device__ __forceinline__ double rbt_entry(double all, double ahh, double alh, 
   return __dmul_rn(__dmul_rn(fi, fj), __dmul_rn(t, w));
 }
 
-// ---- the per-block kernels of hb_symdense_dist (hb_symdense_dist.cu), shared with the host-resident handle (hb_symdense_host.cu) ----
-// Ak addresses block row k like the factor: Ak[(k0 + p) * ld + i] = L(i, k0 + p) for the rows i >= k0 of column k0 + p.
-int hb_dist_init_attrs();
-// L[c * ldb + i] = W[c * ldb + i] * hdr[c] (i < rows, c < 128: k_trsm_panel's L = W D^-1, bit for bit); folds the int at hdr + 128 into
-// *info when it is non-zero and *info is still 0
-int hb_dist_form_l(hb_ctx* c, const double* hdr, const double* W, long long ldb, int rows, double* L, int* info, cudaStream_t st);
+// ---- block rows (hb_blockrow.cu): the step loop and the solve sweeps of hb_symdense_dist and hb_symdense_host ----
+// Block row k (rows k0 = 128 k .. of the row-major upper triangle) is block column k of the lower view. A handle holds some on the device;
+// the others reach it through its transport (another rank's broadcast, or a copy from page-locked host memory).
+constexpr int HB_ROWS_DB = 128;  // block size (hb_big_factor's)
+constexpr int HB_ROWS_HDR = 136; // step header: 1/d (128 doubles), the breakdown word as the int at slot 128, pad to 16 bytes
+enum { HB_ROWS_PH_PANEL = 0, HB_ROWS_PH_MOVE, HB_ROWS_PH_UPDATE, HB_ROWS_PH_COUNT }; // profiled: panel chain, transport + fold, update
+int hb_rows_init_attrs();
+
+// What a block-row handle owns for the loop, and the outcome of its last factorization. The update stream is the context's.
+struct hb_rows
+{
+  hb_stream sp;                                     // panel stream (high priority)
+  hb_event ev_bc[2], ev_free[2], ev_ahead, ev_join; // per step parity: panel ready, operands free; look-ahead done; panel stream joined
+  int mode = -1;
+  bool factored = false;
+  int n_neg = 0, n_null = 0, n_pos = 0;
+  int create();
+  // the end of matrix_changed: the counts {neg, null, pos}; -1 after a breakdown (info != 0); else factored, -1 with a null pivot, n_neg
+  int finish(const double* counts, int info);
+};
+
+// Where step k's panel lives on this rank: its header, and its rows from `sub` on (pan[p * ldp + i - sub]: row i of column k0 + p). A
+// local panel's rows >= k0 + 128 go there unless pan is null (LDL^T: W = L D; Cholesky: L, copied from A); a received one arrives there
+// (LDL^T: W, and L is formed into L with the same layout; Cholesky: L).
+struct hb_rows_panel { double* hdr; double* pan; long long ldp; int sub; double* L; };
+
+// Steps 0 .. nsteps-1 of the factorization of the local block columns, hb_big_factor's K = 128 schedule. Block k is local iff k % P ==
+// rank and k / P >= q0; local block q = k / P holds global columns k0 .. at A + q * 128 * ld. Per step k:
+//   panel stream : wait for ev_free[k & 1]; at(k, local, b); local: zero the header's breakdown word, the panel into b; move(k, local,
+//                  b) makes the panel's operands ready; fold the breakdown into *info; received LDL^T: form L (k_trsm_panel's
+//                  multiplication; a local panel's L is read from A); ev_bc[k & 1]; block k+1 first when it is local (look-ahead)
+//   update stream: behind ev_bc[k & 1], the other local blocks beyond k; then behind the look-ahead, ev_free[k & 1]
+// So ev_free[k & 1] is recorded only when every reader of step k's operands, on both streams, is done: a transport reuses its buffers
+// of parity k & 1 by waiting for ev_free[k & 1] on the stream that writes them. Every entry of A gets the panels 0, 1, ... in ascending
+// order, from the same kernel on the same operand bits. prof: null, or 2 * HB_ROWS_PH_COUNT events per step (begin, end of each phase).
+int hb_rows_factor(hb_ctx* c, hb_rows& r, int N, double* A, long long ld, int P, int rank, int q0, int nsteps, bool ldl, double* inv16, int* info,
+                   const std::function<int(int k, bool local, hb_rows_panel& b)>& at,
+                   const std::function<int(int k, bool local, const hb_rows_panel& b)>& move, hb_event* prof = nullptr);
 // out3 = {neg, null, pos} of the diagonal entries A[e * ld + k0 + t] (e = q * 128 + t of the nloc owned blocks) with the +-1e-14 rule
-int hb_dist_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st);
-// the forward step of block k on the row-major N x nrhs xw (y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, LDL^T: z_k = y_k / d_k), and the
-// backward step (x_k = L_kk^-T (z_k - L_>k,k^T x_>k)); ybuf, tdot: 128 nrhs doubles
-int hb_dist_fwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* ybuf, cudaStream_t st);
-int hb_dist_bwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* tdot, cudaStream_t st);
+int hb_rows_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st);
+// The forward steps on the row-major N x nrhs xw (y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, LDL^T: z_k = y_k / d_k) in ascending block order,
+// then the backward steps (x_k = L_kk^-T (z_k - L_>k,k^T x_>k)) in descending order. rows(k, &Ak): block row k addressed like the factor
+// (Ak[(k0 + p) * ld + i] = L(i, k0 + p)), or null when another rank computes it; after(k, forward) runs after each. ybuf, tdot: 128 nrhs.
+int hb_rows_sweeps(int N, long long ld, bool ldl, double* xw, int nrhs, double* ybuf, double* tdot, cudaStream_t st,
+                   const std::function<int(int k, const double** Ak)>& rows, const std::function<int(int k, bool forward)>& after);
 
 // global row of local row y of rank `rank` in the block-cyclic layout (P = 1: y)
-__host__ __device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / HB_DIST_DB) * P + rank) * HB_DIST_DB + y % HB_DIST_DB; }
+__host__ __device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / HB_ROWS_DB) * P + rank) * HB_ROWS_DB + y % HB_ROWS_DB; }
 
 // f[(level - 1) * N + i]: the diagonal entry of column i at level 1 (B1) and 2 (B2), a function of N alone (2 N doubles)
 int hb_rbt_table(hb_ctx* c, int N, double* f);

@@ -94,6 +94,7 @@ int hb_dense_init(hb_ctx* c)
 {
   HB_CHECK(hb_dense_init_attrs(c));
   HB_CHECK(hb_big_init_attrs(c));
+  HB_CHECK(hb_rows_init_attrs());
   HB_CHECK(hb_bkc_init_attrs(c));
   HB_CHECK(hb_chol_coop_init(c));
   // Thresholds of the symdense caller, with the environment overrides benchmarks use (a negative order keeps the default).

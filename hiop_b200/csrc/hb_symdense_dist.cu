@@ -1,24 +1,17 @@
 // The dense symmetric system factored across the ranks of the context's communicator: Cholesky LL^T and no-pivot LDL^T on a 1-D
 // block-cyclic layout, with NCCL broadcasts of the panels (hb_symdense_dist_*, include/hiopb200.h).
 //
-// Layout. Block size 128 (that of hb_big_factor). Block row k of the N x N row-major upper triangle (rows k*128 .. min(N, k*128+128)-1,
-// full width) is block column k of the column-major lower view the kernels use (hb_dense.cuh). It belongs to rank k mod P and is
-// stored as local block q = k div P: the owned block rows are stacked in order, each 128 rows of ld doubles.
+// Layout. The block rows of hb_blockrow.cu: block row k belongs to rank k mod P and is stored as local block q = k div P, the owned
+// block rows stacked in order, each 128 rows of ld doubles.
 //
-// Factorization, step k (all ranks run the same host sequence, so every rank issues the same collectives in the same order):
-//   owner of k, panel stream : k_diag128 + k_trsm_panel of block k (hb_big_panel) into the broadcast buffer: header [1/d (128), info]
-//                              + the panel rows >= (k+1)*128 (Cholesky: L; LDL^T: W = L D, as hb_big_factor uses them)
-//   every rank, panel stream : ncclBroadcast of that buffer from the owner; fold the header's info word; LDL^T: L = W * (1/d)
-//   owner of k+1, panel stream: look-ahead, the panel applied to block k+1 first, so that its panel chain runs under the others' update
-//   every rank, update stream: the panel applied to every other owned block column beyond k (k_gemm_pq, block-cyclic epilogue)
-// Each entry sees the same k_diag128 / k_trsm_panel / k_gemm_pq arithmetic in the same k order as hb_big_factor with K = 128, so the
-// factor is bit-identical to hb_symdense's look-ahead path (unpaired blocks) for every P. Broadcast buffers are double-buffered across
-// steps. A breakdown (the first failing column, like hb_big_factor's info word) travels in the header of its step, so every rank
-// returns the same value; like the single-GPU path, the factorization runs to its last block either way.
+// Factorization: the step loop of hb_blockrow.cu over every block. All ranks run the same host sequence, so every rank issues the same
+// collectives in the same order. Step k's transport: the owner's panel (the header [1/d, breakdown word] and the rows >= (k+1)*128,
+// Cholesky: L, LDL^T: W = L D) is broadcast from buffer k & 1, where the others receive it. The loop's look-ahead lets the owner of block
+// k+1 run its panel chain and broadcast under the others' update. The factor is bit-identical to hb_symdense's look-ahead path
+// (unpaired blocks) for every P. The breakdown travels in its step's header, so every rank returns the same value.
 //
-// Solves (x replicated on every rank): forward sweep, owner of block k: y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, z_k = y_k (/ d_k), then
-// the broadcast of rows k*128 .. N; backward sweep, owner of block k: x_k = L_kk^-T (z_k - L_>k,k^T x_>k), broadcast of its rows. Every
-// block is computed by its owner in the same order for every P, so the solution does not depend on P.
+// Solves (x replicated on every rank): the sweeps of hb_blockrow.cu, block k computed by its owner, which broadcasts the rows it changed
+// (forward: rows k*128 .. N, backward: its block). Every block is computed in the same order for every P, so x does not depend on P.
 //
 // Safe mode (HB_FACT_RBT_NOPIV): A' = U^T A U with a depth-2 random butterfly U = B2 B1 (rbt_transform: the mirror of the upper
 // triangle, then one pass per level, each output row formed from its row and its partner row), the no-pivot LDL^T above on A', and
@@ -29,126 +22,7 @@
 
 namespace {
 
-constexpr int DB = HB_DIST_DB;   // block size = hb_big_factor's
-constexpr int HDR = 136;         // broadcast header: 1/d (128 doubles), info word (as the first int of slot 128), pad to 16 bytes
-constexpr int SOLVE_RHS = 4;     // right-hand sides per CTA of the diagonal-block solves
-constexpr int DLD = DB + 1;      // shared-memory stride of the diagonal block
-constexpr size_t DIAG_SMEM = sizeof(double) * ((size_t)DB * DLD + SOLVE_RHS * DB);
-
-// fold the breakdown of a received step into the factorization's info word (the first one stays, as in hb_big_factor); LDL^T: form
-// L = W * (1/d) of the received panel with the operation k_trsm_panel uses, so that L is bit-identical to the owner's
-__global__ void k_dist_recv(const double* __restrict__ hdr, const double* __restrict__ W, long long ldb, int rows, int ldl, double* __restrict__ L,
-                            int* __restrict__ info)
-{
-  if(blockIdx.x == 0 && threadIdx.x == 0) {
-    const int step = *reinterpret_cast<const int*>(hdr + DB);
-    if(*info == 0 && step != 0) *info = step;
-  }
-  if(!ldl) return;
-  const long long total = (long long)DB * ldb;
-  for(long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(e / ldb), i = (int)(e % ldb);
-    if(i < rows) L[e] = W[e] * hdr[c];
-  }
-}
-
-// {neg, null, pos} of the owned diagonal entries with the +-1e-14 rule of the I_DIAG sweep (hb_dense_inertia_diag)
-__global__ void __launch_bounds__(1024) k_dist_inertia(const double* __restrict__ A, long long ld, int N, int P, int rank, int nloc, double* __restrict__ out3)
-{
-  __shared__ int cnt[3];
-  if(threadIdx.x < 3) cnt[threadIdx.x] = 0;
-  __syncthreads();
-  int neg = 0, nul = 0, pos = 0;
-  for(int e = threadIdx.x; e < nloc * DB; e += blockDim.x) {
-    const int q = e / DB, t = e % DB, k0 = (q * P + rank) * DB;
-    if(k0 + t >= N) continue;
-    const double d = A[(size_t)e * ld + k0 + t];
-    if(d < -1e-14) neg++; else if(d < 1e-14) nul++; else pos++;
-  }
-  atomicAdd(&cnt[0], neg); atomicAdd(&cnt[1], nul); atomicAdd(&cnt[2], pos);
-  __syncthreads();
-  if(threadIdx.x < 3) out3[threadIdx.x] = (double)cnt[threadIdx.x];
-}
-
-// the nb x nb diagonal block of block column k0 into shared memory: S[j * DLD + i] = L(k0 + i, k0 + j), i >= j
-__device__ __forceinline__ void load_diag(const double* __restrict__ A, long long ld, int k0, int nb, double* S)
-{
-  for(int e = threadIdx.x; e < nb * nb; e += blockDim.x) {
-    const int j = e / nb, i = e % nb;
-    if(i >= j) S[j * DLD + i] = A[(size_t)(k0 + j) * ld + k0 + i];
-  }
-  __syncthreads();
-}
-
-// forward: y = L_kk^-1 b_k for SOLVE_RHS rhs per CTA (thread = row i, rhs cl); y -> ybuf, z = y (LDL^T: y / d) -> xw
-__global__ void __launch_bounds__(DB * SOLVE_RHS) k_dist_fwd_diag(const double* __restrict__ A, long long ld, int k0, int nb, int ldl, double* __restrict__ xw,
-                                                                  int nrhs, double* __restrict__ ybuf)
-{
-  extern __shared__ double dsm[];
-  double* S = dsm;
-  double* ys = dsm + DB * DLD;
-  load_diag(A, ld, k0, nb, S);
-  const int i = threadIdx.x % DB, cl = threadIdx.x / DB, c = blockIdx.x * SOLVE_RHS + cl;
-  const bool live = i < nb && c < nrhs;
-  double b = live ? xw[(size_t)(k0 + i) * nrhs + c] : 0.0;
-  for(int j = 0; j < nb; j++) {
-    if(i == j) ys[cl * DB + j] = ldl ? b : b / S[j * DLD + j];
-    __syncthreads();
-    if(i > j) b -= S[j * DLD + i] * ys[cl * DB + j];
-  }
-  if(live) {
-    const double y = ys[cl * DB + i];
-    ybuf[(size_t)i * nrhs + c] = y;
-    xw[(size_t)(k0 + i) * nrhs + c] = ldl ? y / S[i * DLD + i] : y;
-  }
-}
-
-// forward: b_i -= sum_p L(i, k0 + p) y_p for the rows i >= k0 + 128
-__global__ void k_dist_fwd_panel(const double* __restrict__ A, long long ld, int N, int k0, double* __restrict__ xw, int nrhs, const double* __restrict__ ybuf)
-{
-  const int i = k0 + DB + blockIdx.x * blockDim.x + threadIdx.x;
-  if(i >= N) return;
-  for(int c = 0; c < nrhs; c++) {
-    double acc = 0.0;
-    for(int p = 0; p < DB; p++) acc += A[(size_t)(k0 + p) * ld + i] * ybuf[(size_t)p * nrhs + c];
-    xw[(size_t)i * nrhs + c] -= acc;
-  }
-}
-
-// backward: t[p][c] = sum_{i >= k0 + 128} L(i, k0 + p) x_i (one CTA per p, fixed-order block reduction)
-__global__ void __launch_bounds__(256) k_dist_bwd_dots(const double* __restrict__ A, long long ld, int N, int k0, const double* __restrict__ xw, int nrhs,
-                                                       double* __restrict__ t)
-{
-  __shared__ double red[8];
-  const int p = blockIdx.x;
-  const double* col = A + (size_t)(k0 + p) * ld;
-  for(int c = 0; c < nrhs; c++) {
-    double acc = 0.0;
-    for(int i = k0 + DB + threadIdx.x; i < N; i += 256) acc += col[i] * xw[(size_t)i * nrhs + c];
-    acc = hb_block_sum<256>(acc, red);
-    if(threadIdx.x == 0) t[(size_t)p * nrhs + c] = acc;
-  }
-}
-
-// backward: x_k = L_kk^-T (z_k - t) (unit diagonal for LDL^T) in place in xw
-__global__ void __launch_bounds__(DB * SOLVE_RHS) k_dist_bwd_diag(const double* __restrict__ A, long long ld, int k0, int nb, int ldl, double* __restrict__ xw,
-                                                                  int nrhs, const double* __restrict__ t)
-{
-  extern __shared__ double dsm[];
-  double* S = dsm;
-  double* xs = dsm + DB * DLD;
-  load_diag(A, ld, k0, nb, S);
-  const int i = threadIdx.x % DB, cl = threadIdx.x / DB, c = blockIdx.x * SOLVE_RHS + cl;
-  const bool live = i < nb && c < nrhs;
-  double v = live ? xw[(size_t)(k0 + i) * nrhs + c] : 0.0;
-  if(live && t) v -= t[(size_t)i * nrhs + c];
-  for(int j = nb - 1; j >= 0; j--) {
-    if(i == j) xs[cl * DB + j] = ldl ? v : v / S[j * DLD + j];
-    __syncthreads();
-    if(i < j) v -= S[i * DLD + j] * xs[cl * DB + j];
-  }
-  if(live) xw[(size_t)(k0 + i) * nrhs + c] = xs[cl * DB + i];
-}
+constexpr int DB = HB_ROWS_DB, HDR = HB_ROWS_HDR;
 
 // ---- random butterfly transform (HB_FACT_RBT_NOPIV): A' = U^T A U, U = B2 B1 (oracle/rbt_model.py states every expression; the
 // diagonals, the vector and row kernels and the refined solve are shared with hb_symdense in hb_rbt.cu) ------------------------------
@@ -201,8 +75,6 @@ __global__ void __launch_bounds__(256) k_rbt_level(int N, int level, const doubl
   }
 }
 
-enum { PH_PANEL = 0, PH_BCAST, PH_UPDATE, PH_COUNT };
-
 // Every rank's local result rc (HB_OK or an HB_ERR_* code) made common before the next collective, so that a rank whose allocation
 // failed never leaves the others waiting in a broadcast: all ranks return the most severe code (their own when they failed).
 int agree(hb_ctx* c, int rc)
@@ -221,53 +93,7 @@ int agree(hb_ctx* c, int rc)
 
 } // namespace
 
-// ---- the per-block kernels above, for this file and the host-resident handle (hb_symdense_host.cu) ----
-int hb_dist_init_attrs()
-{
-  HB_CUDA(cudaFuncSetAttribute(k_dist_fwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
-  HB_CUDA(cudaFuncSetAttribute(k_dist_bwd_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DIAG_SMEM));
-  return HB_OK;
-}
-
-int hb_dist_form_l(hb_ctx* c, const double* hdr, const double* W, long long ldb, int rows, double* L, int* info, cudaStream_t st)
-{
-  k_dist_recv<<<hb_grid(c, DB * ldb), 256, 0, st>>>(hdr, W, ldb, rows, 1, L, info);
-  HB_LAUNCHED();
-  return HB_OK;
-}
-
-int hb_dist_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st)
-{
-  k_dist_inertia<<<1, 1024, 0, st>>>(A, ld, N, P, rank, nloc, out3);
-  HB_LAUNCHED();
-  return HB_OK;
-}
-
-int hb_dist_fwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* ybuf, cudaStream_t st)
-{
-  const int nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb, ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
-  k_dist_fwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, ybuf);
-  HB_LAUNCHED();
-  if(rows > 0) {
-    k_dist_fwd_panel<<<(rows + 255) / 256, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, ybuf);
-    HB_LAUNCHED();
-  }
-  return HB_OK;
-}
-
-int hb_dist_bwd_block(const double* Ak, long long ld, int N, int k0, bool ldl, double* xw, int nrhs, double* tdot, cudaStream_t st)
-{
-  const int nb = N - k0 < DB ? N - k0 : DB, rows = N - k0 - nb, ctas = (nrhs + SOLVE_RHS - 1) / SOLVE_RHS;
-  if(rows > 0) {
-    k_dist_bwd_dots<<<nb, 256, 0, st>>>(Ak, ld, N, k0, xw, nrhs, tdot);
-    HB_LAUNCHED();
-  }
-  k_dist_bwd_diag<<<ctas, DB * SOLVE_RHS, DIAG_SMEM, st>>>(Ak, ld, k0, nb, ldl ? 1 : 0, xw, nrhs, rows > 0 ? tdot : nullptr);
-  HB_LAUNCHED();
-  return HB_OK;
-}
-
-struct hb_symdense_dist
+struct hb_symdense_dist : hb_rows // the panel stream, the step loop's events, mode, factored and the inertia counts
 {
   hb_ctx* ctx = nullptr;
   int N = 0, P = 1, rank = 0, nblk = 0, nloc = 0;
@@ -281,15 +107,10 @@ struct hb_symdense_dist
   hb_pinned<double> red_host;
   hb_pinned<int> info_host;
   hb_dev<double> xw, ybuf, tdot; // solve
-  hb_stream sp;               // panel stream
-  hb_event ev_bc[2], ev_free[2], ev_join;
   // per-phase timing (hb_symdense_dist_profile): begin / end events of each phase of each step
   bool profile = false;
   std::unique_ptr<hb_event[]> ev_prof;
-  float phase_ms[PH_COUNT] = {0.f, 0.f, 0.f};
-  int mode = -1;
-  bool factored = false;
-  int n_neg = 0, n_null = 0, n_pos = 0;
+  float phase_ms[HB_ROWS_PH_COUNT] = {0.f, 0.f, 0.f};
   // HB_FACT_RBT_NOPIV, allocated by the first RBT factorization: A' (full rows, owned like A), the butterfly diagonals (2 N), the row
   // sums of |A'| and norm scratch; the solve adds b', the residual and the per-rhs norms
   bool rbt_ready = false;
@@ -345,15 +166,7 @@ extern "C" int hb_symdense_dist_create(hb_ctx* c, int N, hb_symdense_dist** out)
     HB_CHECK(s->info_host.reserve(c, 4, "info words"));
     HB_CHECK(s->red.reserve(c, 4, "inertia counts"));
     HB_CHECK(s->red_host.reserve(c, 4, "inertia counts"));
-    int lo = 0, hi = 0;
-    HB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    HB_CHECK(s->sp.create(cudaStreamNonBlocking, hi));
-    for(int b = 0; b < 2; b++) {
-      HB_CHECK(s->ev_bc[b].create(cudaEventDisableTiming));
-      HB_CHECK(s->ev_free[b].create(cudaEventDisableTiming));
-    }
-    HB_CHECK(s->ev_join.create(cudaEventDisableTiming));
-    HB_CHECK(hb_dist_init_attrs());
+    HB_CHECK(s->create());
     HB_CUDA(cudaStreamSynchronize(c->stream));
     return HB_OK;
   };
@@ -387,8 +200,8 @@ extern "C" int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3)
   HB_REQUIRE(s, "null handle");
   if(on) {
     if(!s->ev_prof) {
-      s->ev_prof.reset(new hb_event[(size_t)2 * PH_COUNT * (s->nblk > 0 ? s->nblk : 1)]);
-      for(int e = 0; e < 2 * PH_COUNT * s->nblk; e++) HB_CHECK(s->ev_prof[e].create(cudaEventDefault));
+      s->ev_prof.reset(new hb_event[(size_t)2 * HB_ROWS_PH_COUNT * (s->nblk > 0 ? s->nblk : 1)]);
+      for(int e = 0; e < 2 * HB_ROWS_PH_COUNT * s->nblk; e++) HB_CHECK(s->ev_prof[e].create(cudaEventDefault));
     }
     for(float& m : s->phase_ms) m = 0.f;
     s->profile = true;
@@ -396,7 +209,7 @@ extern "C" int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3)
   }
   s->profile = false;
   if(ms3)
-    for(int p = 0; p < PH_COUNT; p++) ms3[p] = s->phase_ms[p];
+    for(int p = 0; p < HB_ROWS_PH_COUNT; p++) ms3[p] = s->phase_ms[p];
   return HB_OK;
 }
 
@@ -520,83 +333,38 @@ extern "C" int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode)
   const bool ldl = mode != HB_FACT_CHOLESKY;
   s->mode = mode;
   s->factored = false;
-  if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
+  if(N == 0) { const double none[3] = {0.0, 0.0, 0.0}; return s->finish(none, 0); }
   HB_CUDA(cudaSetDevice(c->device));
   if(mode == HB_FACT_RBT_NOPIV) {
     HB_CHECK(agree(c, rbt_reserve(s)));
     HB_CHECK(rbt_transform(s, 2));
   }
-  cudaStream_t su = c->stream, sp = s->sp;
+  cudaStream_t su = c->stream;
   const long long ld = s->ld;
-  double* A = s->A;
   HB_CUDA(cudaMemsetAsync(s->info, 0, sizeof(int) * 4, su));
-  HB_CUDA(cudaEventRecord(s->ev_free[0], su));
-  HB_CUDA(cudaEventRecord(s->ev_free[1], su));
-  auto mark = [&](int k, int ph, int end, cudaStream_t st) -> int {
-    if(s->profile) HB_CUDA(cudaEventRecord(s->ev_prof[((size_t)k * PH_COUNT + ph) * 2 + end], st));
+  // the transport: the owner's panel goes out from the header and panel rows of broadcast buffer k & 1, the others receive it there
+  auto at = [&](int k, bool, hb_rows_panel& b) -> int { // the slack of ld doubles in front keeps pan - r0 inside the allocation
+    const int r0 = (k + 1) * DB < N ? (k + 1) * DB : N;
+    b = {s->bbuf[k & 1] + ld, s->bbuf[k & 1] + ld + HDR, (N - r0 + 1) & ~1, r0, s->Lbuf[k & 1]};
     return HB_OK;
   };
-  for(int k = 0; k < s->nblk; k++) {
-    const int owner = k % P, sl = k & 1;
-    const int k0 = k * DB, r0 = k0 + DB < N ? k0 + DB : N, rows = N - r0;
-    const long long ldb = (rows + 1) & ~1;
-    double* hdr = s->bbuf[sl] + ld; // the slack in front keeps pan - r0 inside the allocation
-    double* pan = hdr + HDR;
-    int* info_step = reinterpret_cast<int*>(hdr + DB);
-    HB_CUDA(cudaStreamWaitEvent(sp, s->ev_free[sl], 0)); // the update of step k-2 (this buffer, and block k's last update) is done
-    HB_CHECK(mark(k, PH_PANEL, 0, sp));
-    if(owner == rank) {
-      double* Ak = A + (ptrdiff_t)((k / P) * DB - k0) * ld; // LC(Ak, ld, i, j) = element (i, j) for the columns of block k
-      HB_CUDA(cudaMemsetAsync(info_step, 0, sizeof(double), sp));
-      HB_CHECK(hb_big_panel(N, Ak, ld, k0, ldl, s->inv16, hdr, ldl ? pan - r0 : nullptr, ldb, info_step, sp));
-      if(!ldl && rows > 0)
-        HB_CUDA(cudaMemcpy2DAsync(pan, sizeof(double) * ldb, Ak + (size_t)k0 * ld + r0, sizeof(double) * ld, sizeof(double) * rows, DB,
-                                  cudaMemcpyDeviceToDevice, sp));
-    }
-    HB_CHECK(mark(k, PH_PANEL, 1, sp));
-    HB_CHECK(mark(k, PH_BCAST, 0, sp));
-    HB_CHECK(hb_broadcast(c, hdr, HDR + DB * ldb, owner, sp));
-    k_dist_recv<<<ldl ? hb_grid(c, DB * ldb) : 1, 256, 0, sp>>>(hdr, pan, ldb, rows, ldl ? 1 : 0, ldl ? s->Lbuf[sl].get() : nullptr, s->info);
-    HB_LAUNCHED();
-    HB_CHECK(mark(k, PH_BCAST, 1, sp));
-    HB_CUDA(cudaEventRecord(s->ev_bc[sl], sp));
-    if(rows == 0) continue;
-    const double* Pop = pan - r0;                     // P[p * ldb + i], absolute row i
-    const double* Qop = ldl ? s->Lbuf[sl].get() : pan; // Q[p * ldb + j - r0]
-    const bool ahead = k + 1 < s->nblk && (k + 1) % P == rank;
-    if(ahead) {
-      HB_CUDA(cudaStreamWaitEvent(sp, s->ev_free[sl ^ 1], 0)); // block k+1 has received the panels up to k-1
-      HB_CHECK(hb_big_update_cyclic(N, Pop, ldb, Qop, ldb, r0, A, ld, P, rank, (k + 1) / P, 1, sp));
-    }
-    const int first = ahead ? k + 2 : k + 1;         // first global block the update stream takes
-    const int qa = first <= rank ? 0 : (first - rank + P - 1) / P;
-    HB_CUDA(cudaStreamWaitEvent(su, s->ev_bc[sl], 0));
-    HB_CHECK(mark(k, PH_UPDATE, 0, su));
-    HB_CHECK(hb_big_update_cyclic(N, Pop, ldb, Qop, ldb, r0, A, ld, P, rank, qa, s->nloc - qa, su));
-    HB_CHECK(mark(k, PH_UPDATE, 1, su));
-    HB_CUDA(cudaEventRecord(s->ev_free[sl], su));
-  }
-  HB_CUDA(cudaEventRecord(s->ev_join, sp));
-  HB_CUDA(cudaStreamWaitEvent(su, s->ev_join, 0));
-  HB_CHECK(hb_dist_inertia(A, ld, N, P, rank, s->nloc, s->red, su));
+  auto move = [&](int k, bool, const hb_rows_panel& b) { return hb_broadcast(c, b.hdr, HDR + DB * b.ldp, k % P, s->sp); };
+  HB_CHECK(hb_rows_factor(c, *s, N, s->A, ld, P, rank, 0, s->nblk, ldl, s->inv16, s->info, at, move, s->profile ? s->ev_prof.get() : nullptr));
+  HB_CHECK(hb_rows_inertia(s->A, ld, N, P, rank, s->nloc, s->red, su));
   HB_CHECK(hb_allreduce_op(c, s->red, 3, HB_SUM));
   HB_CUDA(cudaMemcpyAsync(s->red_host, s->red, sizeof(double) * 3, cudaMemcpyDeviceToHost, su));
   HB_CUDA(cudaMemcpyAsync(s->info_host, s->info, sizeof(int), cudaMemcpyDeviceToHost, su));
   HB_CUDA(cudaStreamSynchronize(su));
   if(s->profile) {
     for(int k = 0; k < s->nblk; k++)
-      for(int ph = 0; ph < PH_COUNT; ph++) {
-        if(ph == PH_UPDATE && k + 1 == s->nblk) continue; // the last block has no trailing update
+      for(int ph = 0; ph < HB_ROWS_PH_COUNT; ph++) {
+        if(ph == HB_ROWS_PH_UPDATE && k + 1 == s->nblk) continue; // the last block has no trailing update
         float ms = 0.f;
-        HB_CUDA(cudaEventElapsedTime(&ms, s->ev_prof[((size_t)k * PH_COUNT + ph) * 2], s->ev_prof[((size_t)k * PH_COUNT + ph) * 2 + 1]));
+        HB_CUDA(cudaEventElapsedTime(&ms, s->ev_prof[((size_t)k * HB_ROWS_PH_COUNT + ph) * 2], s->ev_prof[((size_t)k * HB_ROWS_PH_COUNT + ph) * 2 + 1]));
         s->phase_ms[ph] += ms;
       }
   }
-  s->n_neg = (int)s->red_host[0]; s->n_null = (int)s->red_host[1]; s->n_pos = (int)s->red_host[2];
-  if(s->info_host[0] != 0) return -1; // zero pivot / not SPD, as hb_symdense_matrix_changed
-  s->factored = true;
-  if(s->n_null > 0) return -1;
-  return s->n_neg;
+  return s->finish(s->red_host, s->info_host[0]);
 }
 
 extern "C" int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_null, int* n_pos)
@@ -608,25 +376,20 @@ extern "C" int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_
   return HB_OK;
 }
 
-// the forward and backward sweeps of the factor on the replicated row-major N x nrhs vectors xw, in place
+// the forward and backward sweeps of the factor on the replicated row-major N x nrhs vectors xw, in place: the owner of block k computes
+// it, then broadcasts the rows it changed (forward: k0 .. N-1, backward: its block)
 static int dist_sweeps(hb_symdense_dist* s, double* xw, int nrhs)
 {
-  hb_ctx* c = s->ctx;
-  const int N = s->N, P = s->P, rank = s->rank;
-  const bool ldl = s->mode != HB_FACT_CHOLESKY;
-  const long long ld = s->ld;
-  cudaStream_t st = c->stream;
-  for(int k = 0; k < s->nblk; k++) {
-    const int owner = k % P, k0 = k * DB;
-    if(owner == rank) HB_CHECK(hb_dist_fwd_block(s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld, ld, N, k0, ldl, xw, nrhs, s->ybuf, st));
-    HB_CHECK(hb_broadcast(c, xw + (size_t)k0 * nrhs, (long long)(N - k0) * nrhs, owner, st));
-  }
-  for(int k = s->nblk - 1; k >= 0; k--) {
-    const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
-    if(owner == rank) HB_CHECK(hb_dist_bwd_block(s->A.get() + (ptrdiff_t)((k / P) * DB - k0) * ld, ld, N, k0, ldl, xw, nrhs, s->tdot, st));
-    HB_CHECK(hb_broadcast(c, xw + (size_t)k0 * nrhs, (long long)nb * nrhs, owner, st));
-  }
-  return HB_OK;
+  const int N = s->N, P = s->P;
+  auto rows = [&](int k, const double** Ak) {
+    *Ak = k % P == s->rank ? s->A.get() + (ptrdiff_t)((k / P) * DB - k * DB) * s->ld : nullptr;
+    return HB_OK;
+  };
+  auto after = [&](int k, bool forward) {
+    const int k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
+    return hb_broadcast(s->ctx, xw + (size_t)k0 * nrhs, (long long)(forward ? N - k0 : nb) * nrhs, k % P, s->ctx->stream);
+  };
+  return hb_rows_sweeps(N, s->ld, s->mode != HB_FACT_CHOLESKY, xw, nrhs, s->ybuf, s->tdot, s->ctx->stream, rows, after);
 }
 
 // RBT solve on the row-major xw (b in, x out): hb_rbt_solve with the sweeps above, and residual rows formed by the owner of each block

@@ -2,40 +2,31 @@
 // LL^T and no-pivot LDL^T of matrices larger than the device memory, streamed through HBM. A block row kept in host memory is to time
 // what a block row of another rank is to space in hb_symdense_dist.
 //
-// Layout. The block rows of hb_symdense_dist at P = 1: block row k is rows k*128 .. min(N, k*128+128)-1 of the caller's N x N row-major
+// Layout. The block rows of hb_blockrow.cu at one rank: block row k is rows k*128 .. min(N, k*128+128)-1 of the caller's N x N row-major
 // matrix (upper triangle valid), i.e. block column k of the column-major lower view the kernels use (hb_dense.cuh). A slab is a run of
 // H consecutive block rows; H comes from the device budget alone (make_plan). On the device, slab rows keep their full width ld, so the
 // kernels address an entry of the slab by its global (row, column) through a shifted base pointer.
 //
-// Factorization, left-looking over the slabs; slab s holds the block rows b0 .. b1-1 (rows c0 = b0*128 ..):
-//   copy stream   : the slab in, one copy per block row from its diagonal column to N - 1 (the strictly lower entries of the 128 x 128
-//                   diagonal blocks ride along and go back unchanged; no kernel reads or writes them)
-//   for every block k < b0, ascending:
-//     copy stream   : columns c0 .. N-1 of block row k into a ring slot (LDL^T: of W = L D, which the slab of block k left in pinned host
-//                     memory), once the slot's last reader is done
-//     compute stream: LDL^T: L = W (1/d) with the multiplication of hb_symdense_dist's k_dist_recv; the K = 128 update of every block
-//                     column of the slab (hb_big_update_cyclic at one rank)
-//   for every block k of the slab, ascending, with hb_symdense_dist's look-ahead:
-//     panel stream  : hb_big_panel (k_diag128 + k_trsm_panel; LDL^T: W into a ring slot, and from there to the host when a later slab
-//                     streams it), then the K = 128 update of block column k+1
-//     compute stream: the K = 128 update of the slab's block columns beyond k+1
-//     copy stream   : block row k, now final, back to the host
-// Every entry thus receives the updates of blocks 0, 1, ... in ascending order, from the same kernel, on the same operand bits as in
-// hb_symdense_dist at P = 1 (L of an in-slab panel is read from the slab, where k_trsm_panel wrote the same W * (1/d)). The factor, the
-// return value and the inertia are bit-identical to it for every slab plan. H2D traffic per factorization: the matrix once plus, per
-// slab, 128 b0 (N - c0) doubles of panels; D2H: the factor once (LDL^T with several slabs: plus the W rows of every block a later slab
-// streams).
+// Factorization, left-looking over the slabs; slab s holds the block rows b0 .. b1-1 (rows c0 = b0*128 ..). The copy stream brings the
+// slab in, one copy per block row from its diagonal column to N - 1 (the strictly lower entries of the diagonal blocks ride along and go
+// back unchanged). Then the step loop of hb_blockrow.cu runs steps 0 .. b1-1, the slab's blocks local, ring slot k & 1 the transport:
+//   k < b0 : the copy stream, behind the slot's ev_free, brings columns c0 .. N-1 of block row k into the slot (LDL^T: of W = L D,
+//            which the slab of block k left in pinned host memory)
+//   k >= b0: the panel writes W into the slot (LDL^T), and the copy stream takes block row k, now final, back to the host, and W to
+//            pinned host memory when a later slab streams it
+// So the factor, the return value and the inertia are bit-identical to hb_symdense_dist at P = 1 for every slab plan. H2D traffic per
+// factorization: the matrix once plus, per slab, 128 b0 (N - c0) doubles of panels; D2H: the factor once (LDL^T with several slabs:
+// plus the W rows of every block a later slab streams).
 //
-// Solves: hb_symdense_dist's per-block kernels, forward in ascending and backward in descending block order, on row-major groups of at
-// most RHS right-hand sides. With one slab the factor stays resident and the sweeps read it there; otherwise every sweep streams block
-// row k (columns k0 .. N-1) through the ring, about 8 N^2 bytes per group.
+// Solves: the sweeps of hb_blockrow.cu (hb_rows_sweeps) on row-major groups of at most RHS right-hand sides. With one slab the factor
+// stays resident and the sweeps read it there; otherwise every sweep streams block row k (columns k0 .. N-1) through the ring, about
+// 8 N^2 bytes per group.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
 
 namespace {
 
-constexpr int DB = HB_DIST_DB;  // block rows of 128, those of hb_symdense_dist
-constexpr int HDR = 136;        // per block: 1/d (128 doubles) and the zero info word hb_dist_form_l reads at slot 128
+constexpr int DB = HB_ROWS_DB, HDR = HB_ROWS_HDR; // one step header per block: its 1/d are read again by every later slab
 constexpr int RHS = 16;         // right-hand sides per pass of a solve (the size of the solve scratch)
 constexpr size_t ALIGN_D = 32;  // every part of the device allocation starts on a 256-byte boundary
 enum { B_PEAK = 0, B_H2D, B_D2H_CHOL, B_D2H_LDL, B_SOLVE_H2D, B_COUNT };
@@ -116,7 +107,7 @@ bool page_locked(const void* p)
 
 } // namespace
 
-struct hb_symdense_host
+struct hb_symdense_host : hb_rows // the panel stream, the step loop's events, mode, factored and the inertia counts
 {
   hb_ctx* ctx = nullptr;
   plan_t p;
@@ -126,11 +117,9 @@ struct hb_symdense_host
   hb_pinned<double> host;      // landing slots: inertia counts (3 doubles), info word
   double* M = nullptr;         // the caller's page-locked matrix (borrowed)
   long long ldh = 0;
-  hb_stream sc, sp;            // copy stream; panel stream (the look-ahead inside a slab)
-  hb_event ev_in[2], ev_read[2], ev_out[2], ev_a, ev_b, ev_free[2], ev_bc[2], ev_join;
-  int mode = -1;
-  bool factored = false, resident = false;
-  int n_neg = 0, n_null = 0, n_pos = 0;
+  hb_stream sc;                // copy stream
+  hb_event ev_in[2], ev_read[2], ev_out[2], ev_a, ev_b, ev_panel;
+  bool resident = false;
   double* at(size_t off) const { return mem.get() + off; }
   double* slot(int j) const { return mem.get() + p.ring + (size_t)j * 2 * DB * p.ld; } // W or L rows; the formed L follows at + 128 ld
   ~hb_symdense_host()
@@ -175,14 +164,11 @@ extern "C" int hb_symdense_host_create(hb_ctx* c, int N, size_t device_bytes, hb
   HB_CHECK(make_plan(N, device_bytes, s->p));
   if(N > 0) HB_CHECK(s->mem.reserve(c, s->p.total, "slab, panel ring and scratch"));
   HB_CHECK(s->host.reserve(c, 4, "inertia counts and info word"));
-  int lo = 0, hi = 0;
-  HB_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+  HB_CHECK(s->create());
   HB_CHECK(s->sc.create(cudaStreamNonBlocking));
-  HB_CHECK(s->sp.create(cudaStreamNonBlocking, hi));
   for(int j = 0; j < 2; j++)
-    for(hb_event* e : {&s->ev_in[j], &s->ev_read[j], &s->ev_out[j], &s->ev_free[j], &s->ev_bc[j]}) HB_CHECK(e->create(cudaEventDisableTiming));
-  for(hb_event* e : {&s->ev_a, &s->ev_b, &s->ev_join}) HB_CHECK(e->create(cudaEventDisableTiming));
-  HB_CHECK(hb_dist_init_attrs());
+    for(hb_event* e : {&s->ev_in[j], &s->ev_read[j], &s->ev_out[j]}) HB_CHECK(e->create(cudaEventDisableTiming));
+  for(hb_event* e : {&s->ev_a, &s->ev_b, &s->ev_panel}) HB_CHECK(e->create(cudaEventDisableTiming));
   *out = s.release();
   return HB_OK;
 }
@@ -231,15 +217,15 @@ int slab_copy(hb_symdense_host* s, int b0, int kb, int ke, bool in)
   return HB_OK;
 }
 
-// `rows` rows of `width` doubles from the host (pitch hld) into ring slot j (pitch ld) on the copy stream, once the slot's last reader on
-// the compute stream is done; the compute stream then waits for the copy
-int ring_in(hb_symdense_host* s, int j, const double* src, long long hld, long long width, long long rows)
+// `rows` rows of `width` doubles from the host (pitch hld) into ring slot j (pitch ld) on the copy stream, once `free` (the slot's last
+// reader is done) has passed; the stream `use` then waits for the copy
+int ring_in(hb_symdense_host* s, int j, const double* src, long long hld, long long width, long long rows, cudaEvent_t free, cudaStream_t use)
 {
-  cudaStream_t su = s->ctx->stream, sc = s->sc;
-  HB_CUDA(cudaStreamWaitEvent(sc, s->ev_read[j], 0));
+  cudaStream_t sc = s->sc;
+  HB_CUDA(cudaStreamWaitEvent(sc, free, 0));
   HB_CUDA(cudaMemcpy2DAsync(s->slot(j), sizeof(double) * s->p.ld, src, sizeof(double) * hld, sizeof(double) * width, rows, cudaMemcpyHostToDevice, sc));
   HB_CUDA(cudaEventRecord(s->ev_in[j], sc));
-  HB_CUDA(cudaStreamWaitEvent(su, s->ev_in[j], 0));
+  HB_CUDA(cudaStreamWaitEvent(use, s->ev_in[j], 0));
   return HB_OK;
 }
 
@@ -265,68 +251,43 @@ int factor(hb_symdense_host* s, bool ldl)
   int* info = reinterpret_cast<int*>(s->at(p.info));
   const int wlast = (p.nslab - 1) * p.H; // the blocks before this one are streamed by a later slab
   HB_CUDA(cudaMemsetAsync(info, 0, sizeof(int), su));
-  HB_CUDA(cudaMemsetAsync(hdr, 0, sizeof(double) * p.nblk * HDR, su));
   HB_CHECK(order(s, true)); // the slab and the ring may still be read by an earlier solve
-  long long t = 0;          // ring uses
   for(int sl = 0; sl < p.nslab; sl++) {
     const int b0 = sl * p.H, b1 = b0 + p.H < p.nblk ? b0 + p.H : p.nblk, c0 = b0 * DB, c1 = b1 * DB < N ? b1 * DB : N;
-    double* Sb = S - (ptrdiff_t)c0 * ld; // LC(Sb, ld, i, j) = entry (i, j) for the columns j of the slab
     HB_CHECK(slab_copy(s, b0, b0, b1, true));
     HB_CHECK(order(s, false));
-    for(int k = 0; k < b0; k++) {
-      const int j = (int)(t++ & 1), r0 = (k + 1) * DB;
-      double* R = s->slot(j);
-      double* RL = R + (size_t)DB * ld;
-      if(ldl) HB_CHECK(ring_in(s, j, s->Wh.get() + s->woff[k] + (c0 - r0), N - r0, N - c0, DB));
-      else HB_CHECK(ring_in(s, j, s->M + (size_t)k * DB * s->ldh + c0, s->ldh, N - c0, DB));
-      if(ldl) HB_CHECK(hb_dist_form_l(c, hdr + (size_t)k * HDR, R, ld, N - c0, RL, info, su));
-      HB_CHECK(hb_big_update_cyclic(N, R - c0, ld, ldl ? RL : R, ld, c0, Sb, ld, 1, 0, b0, b1 - b0, su));
-      HB_CUDA(cudaEventRecord(s->ev_read[j], su));
-    }
-    // the slab's own block rows, with the look-ahead of hb_symdense_dist: panel k and its update of block k+1 on the panel stream, the
-    // update of the blocks beyond on the compute stream. ev_free[k & 1]: the compute stream's update of step k is done.
-    HB_CUDA(cudaEventRecord(s->ev_free[0], su));
-    HB_CUDA(cudaEventRecord(s->ev_free[1], su));
-    for(int k = b0; k < b1; k++) {
-      const int k0 = k * DB, r0 = k0 + DB < N ? k0 + DB : N, sl = k & 1;
-      const double* Lk = Sb + (size_t)k0 * ld; // Lk[p * ld + i] = L(i, k0 + p)
-      const bool wpanel = ldl && r0 < N;
-      int j = 0;
-      double* W = nullptr;
-      HB_CUDA(cudaStreamWaitEvent(sp, s->ev_free[sl], 0)); // block k has its update of step k-2
-      if(wpanel) {
-        j = (int)(t++ & 1);
-        HB_CUDA(cudaStreamWaitEvent(sp, s->ev_read[j], 0)); // the slot's last reader on the compute stream is done
-        HB_CUDA(cudaStreamWaitEvent(sp, s->ev_out[j], 0));  // and its last copy to the host
-        W = s->slot(j) - r0;
-      }
-      HB_CHECK(hb_big_panel(N, Sb, ld, k0, ldl, s->at(p.inv16), hdr + (size_t)k * HDR, W, ld, info, sp));
-      HB_CUDA(cudaEventRecord(s->ev_bc[sl], sp));
+    // the transport of step k, ring slot k & 1: a block before the slab arrives from the host (its columns c0 .. N-1; LDL^T: of W);
+    // a block of the slab writes W there (LDL^T, when a block follows) and goes back to the host once its panel is done
+    auto at = [&](int k, bool local, hb_rows_panel& b) -> int {
+      const int r0 = (k + 1) * DB < N ? (k + 1) * DB : N;
+      double* R = s->slot(k & 1);
+      b = local ? hb_rows_panel{hdr + (size_t)k * HDR, ldl && r0 < N ? R : nullptr, ld, r0, nullptr}
+                : hb_rows_panel{hdr + (size_t)k * HDR, R, ld, c0, R + (size_t)DB * ld};
+      if(local && b.pan) HB_CUDA(cudaStreamWaitEvent(sp, s->ev_out[k & 1], 0)); // W goes into the slot once its last copy to the host is done
+      return HB_OK;
+    };
+    auto move = [&](int k, bool local, const hb_rows_panel&) -> int {
+      const int j = k & 1, r0 = (k + 1) * DB < N ? (k + 1) * DB : N;
+      if(!local && ldl) return ring_in(s, j, s->Wh.get() + s->woff[k] + (c0 - r0), N - r0, N - c0, DB, s->ev_free[j], sp);
+      if(!local) return ring_in(s, j, s->M + (size_t)k * DB * s->ldh + c0, s->ldh, N - c0, DB, s->ev_free[j], sp);
       // block row k is final: back to the host under the rest of the slab's updates
-      HB_CUDA(cudaStreamWaitEvent(sc, s->ev_bc[sl], 0));
+      HB_CUDA(cudaEventRecord(s->ev_panel, sp));
+      HB_CUDA(cudaStreamWaitEvent(sc, s->ev_panel, 0));
       HB_CHECK(slab_copy(s, b0, k, k + 1, false));
-      if(wpanel && k < wlast) {
+      if(ldl && r0 < N && k < wlast) {
         HB_CUDA(cudaMemcpy2DAsync(s->Wh.get() + s->woff[k], sizeof(double) * (N - r0), s->slot(j), sizeof(double) * ld, sizeof(double) * (N - r0), DB,
                                   cudaMemcpyDeviceToHost, sc));
         HB_CUDA(cudaEventRecord(s->ev_out[j], sc));
       }
-      if(k + 1 >= b1) continue;
-      const double* P = wpanel ? W : Lk;
-      HB_CUDA(cudaStreamWaitEvent(sp, s->ev_free[sl ^ 1], 0)); // block k+1 has its update of step k-1
-      HB_CHECK(hb_big_update_cyclic(N, P, ld, Lk, ld, 0, Sb, ld, 1, 0, k + 1, 1, sp));
-      HB_CUDA(cudaStreamWaitEvent(su, s->ev_bc[sl], 0));
-      HB_CHECK(hb_big_update_cyclic(N, P, ld, Lk, ld, 0, Sb, ld, 1, 0, k + 2, b1 - k - 2, su));
-      HB_CUDA(cudaEventRecord(s->ev_free[sl], su));
-      if(wpanel) HB_CUDA(cudaEventRecord(s->ev_read[j], su));
-    }
-    HB_CUDA(cudaEventRecord(s->ev_join, sp));
-    HB_CUDA(cudaStreamWaitEvent(su, s->ev_join, 0));
+      return HB_OK;
+    };
+    HB_CHECK(hb_rows_factor(c, *s, N, S - (ptrdiff_t)c0 * ld, ld, 1, 0, b0, b1, ldl, s->at(p.inv16), info, at, move));
     // the slab's diagonal (inertia); the next slab's copy waits for the compute stream to be done with this one
     HB_CUDA(cudaMemcpy2DAsync(s->at(p.diag) + c0, sizeof(double), S + c0, sizeof(double) * (ld + 1), sizeof(double), c1 - c0, cudaMemcpyDeviceToDevice, su));
     HB_CHECK(order(s, true));
   }
   HB_CHECK(order(s, false));
-  HB_CHECK(hb_dist_inertia(s->at(p.diag), 0, N, 1, 0, p.nblk, s->at(p.red), su));
+  HB_CHECK(hb_rows_inertia(s->at(p.diag), 0, N, 1, 0, p.nblk, s->at(p.red), su));
   HB_CUDA(cudaMemcpyAsync(s->host, s->at(p.red), sizeof(double) * 3, cudaMemcpyDeviceToHost, su));
   HB_CUDA(cudaMemcpyAsync(s->host.get() + 3, info, sizeof(int), cudaMemcpyDeviceToHost, su));
   HB_CUDA(cudaStreamSynchronize(su));
@@ -350,7 +311,7 @@ extern "C" int hb_symdense_host_matrix_changed(hb_symdense_host* s, int mode)
   if(N > 0 && !s->M) return hb_fail(HB_ERR_STATE, "hb_symdense_host_matrix_changed: no matrix (call hb_symdense_host_set_matrix)%s", "");
   s->mode = mode;
   s->factored = s->resident = false;
-  if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
+  if(N == 0) { const double none[3] = {0.0, 0.0, 0.0}; return s->finish(none, 0); }
   HB_CUDA(cudaSetDevice(s->ctx->device));
   if(ldl && p.nslab > 1 && !s->Wh) {
     const int wlast = (p.nslab - 1) * p.H;
@@ -365,11 +326,7 @@ extern "C" int hb_symdense_host_matrix_changed(hb_symdense_host* s, int mode)
   }
   HB_CHECK(factor(s, ldl));
   s->resident = p.nslab == 1;
-  s->n_neg = (int)s->host[0]; s->n_null = (int)s->host[1]; s->n_pos = (int)s->host[2];
-  if(*reinterpret_cast<const int*>(s->host.get() + 3) != 0) return -1; // zero pivot / not SPD, as hb_symdense_dist_matrix_changed
-  s->factored = true;
-  if(s->n_null > 0) return -1;
-  return s->n_neg;
+  return s->finish(s->host, *reinterpret_cast<const int*>(s->host.get() + 3));
 }
 
 extern "C" int hb_symdense_host_inertia(hb_symdense_host* s, int* n_neg, int* n_null, int* n_pos)
@@ -396,36 +353,29 @@ extern "C" int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs)
   const long long ld = p.ld;
   double* xw = s->at(p.xw);
   long long t = 0;
-  // block row k on the device: the resident factor, or columns k0 .. N-1 of the host's block row streamed into a ring slot (*j)
-  auto block = [&](int k, const double** Ak, int* j) -> int {
+  int j = 0;
+  // block row k on the device: the resident factor, or columns k0 .. N-1 of the host's block row streamed into ring slot j, which is
+  // free again once the block's step is done
+  auto rows = [&](int k, const double** Ak) -> int {
     const long long k0 = (long long)k * DB;
     if(s->resident) {
       *Ak = s->at(p.slab);
       return HB_OK;
     }
-    *j = (int)(t++ & 1);
-    HB_CHECK(ring_in(s, *j, s->M + (size_t)k0 * s->ldh + k0, s->ldh, N - k0, N - k0 < DB ? N - k0 : DB));
-    *Ak = s->slot(*j) - (ptrdiff_t)(k0 * ld + k0);
+    j = (int)(t++ & 1);
+    HB_CHECK(ring_in(s, j, s->M + (size_t)k0 * s->ldh + k0, s->ldh, N - k0, N - k0 < DB ? N - k0 : DB, s->ev_read[j], su));
+    *Ak = s->slot(j) - (ptrdiff_t)(k0 * ld + k0);
+    return HB_OK;
+  };
+  auto after = [&](int, bool) -> int {
+    if(!s->resident) HB_CUDA(cudaEventRecord(s->ev_read[j], su));
     return HB_OK;
   };
   for(int g0 = 0; g0 < nrhs; g0 += RHS) {
     const int ng = nrhs - g0 < RHS ? nrhs - g0 : RHS;
     double* xg = x + (size_t)g0 * N;
     HB_CHECK(hb_rbt_to_rows(c, N, ng, xg, xw, false));
-    for(int k = 0; k < p.nblk; k++) {
-      const double* Ak = nullptr;
-      int j = 0;
-      HB_CHECK(block(k, &Ak, &j));
-      HB_CHECK(hb_dist_fwd_block(Ak, ld, N, k * DB, ldl, xw, ng, s->at(p.ybuf), su));
-      if(!s->resident) HB_CUDA(cudaEventRecord(s->ev_read[j], su));
-    }
-    for(int k = p.nblk - 1; k >= 0; k--) {
-      const double* Ak = nullptr;
-      int j = 0;
-      HB_CHECK(block(k, &Ak, &j));
-      HB_CHECK(hb_dist_bwd_block(Ak, ld, N, k * DB, ldl, xw, ng, s->at(p.tdot), su));
-      if(!s->resident) HB_CUDA(cudaEventRecord(s->ev_read[j], su));
-    }
+    HB_CHECK(hb_rows_sweeps(N, ld, ldl, xw, ng, s->at(p.ybuf), s->at(p.tdot), su, rows, after));
     HB_CHECK(hb_rbt_to_rows(c, N, ng, xg, xw, true));
   }
   if(!s->resident) HB_CUDA(cudaStreamSynchronize(s->sc)); // the last read of the host matrix is done when the solve returns

@@ -1,7 +1,7 @@
 """The dense symmetric solver with the matrix in page-locked host memory (hb_symdense_host, LinSolverSymDenseHost): the factor, the
-return value, the inertia and the solutions bit for bit against hb_symdense_dist at P = 1 for one slab, two slabs and one block row per
-slab; the backward-error bounds of test_gpu_symdense_dist.py; the strictly lower triangle left alone; failure, misuse, device footprint
-and resources."""
+return value, the inertia and the solutions bit for bit against hb_symdense_dist at P = 1 for one slab, two slabs, one block row per
+slab and three slabs with a shorter last one; the backward-error bounds of test_gpu_symdense_dist.py; the strictly lower triangle left
+alone; failure, misuse, device footprint and resources."""
 import ctypes
 import threading
 
@@ -35,14 +35,34 @@ def budget_for(N, slabs):
     return hi
 
 
+def budget_for_height(N, H):
+    """the smallest budget whose plan puts at least H block rows in a slab"""
+    lo, hi = 1, 1 << 40
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        try:
+            ok = plan(N, mid)["slab_blocks"] >= H
+        except Exception:
+            ok = False
+        hi, lo = (mid, lo) if ok else (hi, mid)
+    return hi
+
+
 def budgets(N):
-    """{one slab, two slabs, one block row per slab}, each once"""
+    """{one slab, two slabs, one block row per slab, three slabs with a shorter last one}, each once"""
     nblk = -(-N // 128)
     out = {}
     for name, n in (("one_slab", 1), ("two_slabs", 2), ("row_per_slab", nblk)):
         b = budget_for(N, n)
         if all(plan(N, b)["slabs"] != plan(N, v)["slabs"] for v in out.values()):
             out[name] = b
+    # the first slab height that gives three slabs with a remainder, so that the last slab has fewer block rows
+    H = next((h for h in range(1, nblk) if -(-nblk // h) == 3 and nblk % h), None)
+    if H is not None:
+        b = budget_for_height(N, H)
+        p = plan(N, b)
+        assert p["slabs"] == 3 and p["first"][3] - p["first"][2] < p["first"][1] - p["first"][0], p
+        out["three_slabs_short_last"] = b
     return out
 
 

@@ -25,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 CHOL, NOPIV, RBT, BK = 2, 1, 3, 0
-BLOCK, HDR = 128, 136   # hb_symdense_dist.cu: block size, broadcast header (doubles)
+BLOCK, HDR = 128, 136   # hb_blockrow.cu (HB_ROWS_DB, HB_ROWS_HDR): block size, broadcast step header (doubles)
 
 
 def card(local_rank):
