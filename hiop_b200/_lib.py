@@ -149,6 +149,10 @@ def lib() -> ctypes.CDLL:
     f("hb_symdense_host_inertia", c_i, c_vp, P(c_i), P(c_i), P(c_i))
     f("hb_symdense_host_solve", c_i, c_vp, c_dp, c_i)
     f("hb_symdense_host_plan_view", c_i, c_i, ctypes.c_size_t, P(c_i), c_vp, c_vp)
+    f("hb_symdense_host_set_rbt_copy", c_i, c_vp, c_vp, c_ll)
+    f("hb_symdense_host_rbt_stats", c_i, c_vp, P(c_i), P(ctypes.c_double), P(ctypes.c_float))
+    f("hb_symdense_host_rbt_plan_view", c_i, c_i, ctypes.c_size_t, P(c_i), c_vp, c_vp)
+    f("hb_rbt_strip_view", c_i, c_i, c_i, c_i, P(c_i), c_vp, c_vp)
     f("hb_microbench_peak", c_i, c_vp, c_i, P(c_d))
     # lowrank
     f("hb_lowrank_create", c_i, c_vp, c_ll, c_i, c_i, c_i, P(c_vp))

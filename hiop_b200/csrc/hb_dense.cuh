@@ -238,6 +238,30 @@ int hb_rows_sweeps(int N, long long ld, bool ldl, double* xw, int nrhs, double* 
 // global row of local row y of rank `rank` in the block-cyclic layout (P = 1: y)
 __host__ __device__ __forceinline__ int rbt_global_row(int y, int P, int rank) { return ((y / HB_ROWS_DB) * P + rank) * HB_ROWS_DB + y % HB_ROWS_DB; }
 
+// Which rows of A a handle holds for the transform: local row y is global row global(y) (-1: none), global row g is local row local(g)
+// (-1: not held). rows == nullptr: the block-cyclic rows of rank `rank` of P (hb_symdense_dist); else the explicit map rows[y], pos[g]
+// (hb_symdense_host: the window of a strip).
+struct hb_rbt_rowmap
+{
+  const int* rows;
+  const int* pos;
+  int P, rank;
+  __device__ __forceinline__ int global(int y) const { return rows ? rows[y] : rbt_global_row(y, P, rank); }
+  __device__ __forceinline__ int local(int g) const
+  {
+    if(pos) return pos[g];
+    return (g / HB_ROWS_DB) % P == rank ? (g / HB_ROWS_DB / P) * HB_ROWS_DB + g % HB_ROWS_DB : -1;
+  }
+};
+// the mirror of the upper triangle: every local row y >= ybeg (of nrows) with global row r gets dst(y, j) = src(j, r) for the columns
+// q0 <= j < q0 + nq, j < r, where src holds rows q0 .. (ld doubles each, column r at src[(j - q0) * ld + r])
+int hb_rbt_mirror(hb_ctx* c, int N, hb_rbt_rowmap m, int nrows, int ybeg, const double* src, long long ld, int q0, int nq, double* dst);
+// one level B^T A B on full rows (ld): for each of the nsrc source rows q (local row x of `in`, global m.global(x); or, with src, global
+// row q0 + x held at src + x ld), its partner r, when held (m.local(r) >= 0), gets its whole output row from rows r and q in `out`, at
+// the same local row as in `in`. Every output entry is rbt_entry on the model's operands, so it does not depend on the map.
+int hb_rbt_level(hb_ctx* c, int N, int level, const double* f, const double* in, long long ld, hb_rbt_rowmap m, int nsrc, const double* src, int q0,
+                 double* out);
+
 // f[(level - 1) * N + i]: the diagonal entry of column i at level 1 (B1) and 2 (B2), a function of N alone (2 N doubles)
 int hb_rbt_table(hb_ctx* c, int N, double* f);
 // x (N x nrhs, one rhs after the other) -> xw (row-major N x nrhs), or back
@@ -273,3 +297,18 @@ bool hb_rbt_in_place(int N);
 size_t hb_rbt_part_doubles(int N);
 int hb_rbt_fused(hb_ctx* c, int N, const double* f, const double* A, long long lda, double* F, long long ldf, double* Ak, long long ldk, double* part,
                  double* nrm_dev);
+// The strips of the out-of-core transform (hb_symdense_host): strip [s0, s1) of the butterfly slots produces the rows at those slots in
+// each of the four quarters of k_rbt_fused's schedule, and reads its window: the same slots (N != 1 mod 4), or one slot more on each side
+// plus the three fixed rows (N = 1 mod 4), laid out as k_rbt_fused lays out a tile's window with s1 - s0 slots per quarter.
+struct hb_rbt_window
+{
+  int N, slots, s0, s1, W, wr; // slots: of the longest quarter; W: window slots per quarter; wr: window positions
+  int ext, qs[4], qlen[4], sp[3];
+};
+hb_rbt_window hb_rbt_window_of(int N, int s0, int s1);
+// the window's positions: rows[k] = the global row held at position k (-1: none, or held at an earlier position); pos_win[g] = the
+// position of global row g (-1: outside), pos_out[g] = the same for the strip's own rows only (-1 elsewhere)
+int hb_rbt_window_map(hb_ctx* c, const hb_rbt_window& w, int* rows, int* pos_win, int* pos_out);
+// host side of the same: position k of the window (-1: none or a repeat), and whether global row g is one of the strip's rows
+int hb_rbt_window_row(const hb_rbt_window& w, int k);
+bool hb_rbt_window_out(const hb_rbt_window& w, int g);

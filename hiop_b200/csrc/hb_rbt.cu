@@ -1,6 +1,8 @@
-// The random butterfly transform of the safe mode (HB_FACT_RBT_NOPIV), shared by hb_symdense (one GPU) and hb_symdense_dist: the
-// butterfly diagonals, U^T b and U x on row-major N x nrhs vectors, the rows of b' - A' x' and of |A'|, the refined solve, and the
-// one-pass transform of the one-GPU handle (k_rbt_fused). oracle/rbt_model.py states every expression.
+// The random butterfly transform of the safe mode (HB_FACT_RBT_NOPIV), shared by hb_symdense (one GPU), hb_symdense_dist and
+// hb_symdense_host: the butterfly diagonals, U^T b and U x on row-major N x nrhs vectors, the rows of b' - A' x' and of |A'|, the
+// refined solve, the row-wise transform of the distributed and host-resident handles (k_rbt_mirror, k_rbt_level on a row map: the
+// block-cyclic rows of a rank, or the window of a strip), the strips' windows, and the one-pass transform of the one-GPU handle
+// (k_rbt_fused). oracle/rbt_model.py states every expression.
 //
 // k_rbt_fused. A'(i, j) reads B2^T A B2 at rows {i, p1(i)} and columns {j, p1(j)}, which reads A at rows {i, p2(i), p1(i), p2(p1(i))}
 // (p1, p2: the level-1 and level-2 partners), and alike for j. Split [0, N) into four quarters Q0 = [0, ha), Q1 = [ha, h), Q2 = [h, h + hb),
@@ -115,6 +117,56 @@ __global__ void __launch_bounds__(256) k_rbt_max(int N, int ncols, const double*
   }
 }
 
+// ---- the row-wise transform of the distributed and host-resident handles: the mirror, then one pass per level ----------------------
+constexpr int RBT_COLS = 1024; // columns per CTA of k_rbt_level (256 threads x 4)
+
+// mirror: every held row r gets dst(y, j) = src(j, r) for the columns q0 <= j < q0 + nq, j < r, where src holds the rows q0 .. of the
+// upper triangle (ld doubles each). 32 x 32 tiles through shared memory: local rows y0 .., starting at local row ybeg.
+__global__ void __launch_bounds__(256) k_rbt_mirror(int N, hb_rbt_rowmap m, int nrows, int ybeg, const double* __restrict__ src, long long ld, int q0,
+                                                    int nq, double* __restrict__ dst)
+{
+  __shared__ double tile[32][33];
+  const int y0 = ybeg + blockIdx.y * 32, j0 = q0 + blockIdx.x * 32, tx = threadIdx.x % 32, ty = threadIdx.x / 32;
+  for(int jj = ty; jj < 32; jj += 8) {
+    const int y = y0 + tx, j = j0 + jj;
+    const int r = y < nrows ? m.global(y) : N;
+    tile[jj][tx] = (r < N && j < q0 + nq && j < r) ? src[(size_t)(j - q0) * ld + r] : 0.0;
+  }
+  __syncthreads();
+  for(int yy = ty; yy < 32; yy += 8) {
+    const int y = y0 + yy, j = j0 + tx;
+    const int r = y < nrows ? m.global(y) : N;
+    if(r < N && j < q0 + nq && j < r) dst[(size_t)y * ld + j] = tile[tx][yy];
+  }
+}
+
+// one level B^T A B on full rows. CTA x = a source row q: local row x of `in` (src == nullptr: every partner is held) or row x of src
+// (global rows q0 .. q0 + nq, the owner's broadcast). Its partner r (q itself when unpaired), when held, gets its whole output row from
+// rows r and q: out(r, j) = (f_r f_j) (t w) with t and w of oracle/rbt_model.py, in that operation order.
+__global__ void __launch_bounds__(256) k_rbt_level(int N, int level, const double* __restrict__ f, const double* __restrict__ in, long long ld,
+                                                   hb_rbt_rowmap m, const double* __restrict__ src, int q0, double* __restrict__ out)
+{
+  const int q = src ? q0 + blockIdx.x : m.global(blockIdx.x);
+  if(q < 0 || q >= N) return;
+  const double* rowq = src ? src + (size_t)blockIdx.x * ld : in + (size_t)blockIdx.x * ld;
+  const rbt_pos pq = rbt_at(N, level, q);
+  const int r = pq.lo == q ? pq.hi : pq.lo;
+  const int lr = m.local(r);
+  if(lr < 0) return;
+  const double* rowr = in + (size_t)lr * ld;
+  const rbt_pos pr = rbt_at(N, level, r);
+  const double* RL = pr.lo == r ? rowr : rowq;
+  const double* RH = pr.hi == r ? rowr : rowq;
+  const double* fl = f + (size_t)(level - 1) * N;
+  const double fi = fl[r];
+  double* o = out + (size_t)lr * ld;
+  const int jend = min(N, (int)(blockIdx.y + 1) * RBT_COLS);
+  for(int j = blockIdx.y * RBT_COLS + threadIdx.x; j < jend; j += 256) {
+    const rbt_pos pj = rbt_at(N, level, j);
+    o[j] = rbt_entry(RL[pj.lo], RH[pj.hi], RL[pj.hi], RH[pj.lo], pr, pj, fi, fl[j]);
+  }
+}
+
 // ---- the one-pass transform of the one-GPU handle ----------------------------------------------------------------------------------
 constexpr int RBT_T = 16;                        // slots per tile: 4 RBT_T output rows
 constexpr int RBT_OR = 4 * RBT_T;                // output rows of a tile
@@ -163,34 +215,34 @@ __host__ __device__ inline int rbt_out_row(const rbt_quarters& q, int b, int k)
   return slot < q.len[a] ? q.s[a] + slot : -1;
 }
 
-// window row k (0 .. q.wr-1) of tile b: the slots b RBT_T - ext .. (b + 1) RBT_T + ext - 1 of each quarter, then the three fixed rows
-// of N = 1 (mod 4); -1 where there is none
-__host__ __device__ inline int rbt_window_row(const rbt_quarters& q, int b, int k)
+// window row k (0 .. q.wr-1) of the tile or strip whose first slot is `first`: the slots first - ext .. first + q.W - ext - 1 of each
+// quarter, then the three fixed rows of N = 1 (mod 4); -1 where there is none
+__host__ __device__ inline int rbt_window_row(const rbt_quarters& q, int first, int k)
 {
   if(k < 4 * q.W) {
-    const int a = k / q.W, slot = b * RBT_T - q.ext + k % q.W;
+    const int a = k / q.W, slot = first - q.ext + k % q.W;
     return slot >= 0 && slot < q.len[a] ? q.s[a] + slot : -1;
   }
   k -= 4 * q.W;
   return k < 3 ? q.sp[k] : -1;
 }
 
-// the first window position of tile b that holds row g, -1 if none
-__host__ __device__ inline int rbt_window_pos(const rbt_quarters& q, int b, int g)
+// the first window position of the tile or strip starting at slot `first` that holds row g, -1 if none
+__host__ __device__ inline int rbt_window_pos(const rbt_quarters& q, int first, int g)
 {
   const int a = g >= q.s[3] ? 3 : g >= q.s[2] ? 2 : g >= q.s[1] ? 1 : 0;
-  const int w = g - q.s[a] - (b * RBT_T - q.ext);
+  const int w = g - q.s[a] - (first - q.ext);
   if(w >= 0 && w < q.W) return a * q.W + w;
   for(int e = 0; e < 3; e++)
     if(q.sp[e] == g) return 4 * q.W + e;
   return -1;
 }
 
-// the row the kernel reads into window position k of tile b: rbt_window_row unless an earlier position holds it already (-1)
-__host__ __device__ inline int rbt_window_held(const rbt_quarters& q, int b, int k)
+// the row the kernel reads into window position k: rbt_window_row unless an earlier position holds it already (-1)
+__host__ __device__ inline int rbt_window_held(const rbt_quarters& q, int first, int k)
 {
-  const int g = k < q.wr ? rbt_window_row(q, b, k) : -1;
-  return g >= 0 && rbt_window_pos(q, b, g) == k ? g : -1;
+  const int g = k < q.wr ? rbt_window_row(q, first, k) : -1;
+  return g >= 0 && rbt_window_pos(q, first, g) == k ? g : -1;
 }
 
 __global__ void __launch_bounds__(256) k_rbt_fused(int N, const double* __restrict__ f, const double* A, long long lda, double* F, long long ldf,
@@ -207,8 +259,8 @@ __global__ void __launch_bounds__(256) k_rbt_fused(int N, const double* __restri
   const int wr = q.wr, tid = threadIdx.x;
   const bool diag = bi == bj;
   for(int k = tid; k < wr; k += 256) {
-    rw[k] = rbt_window_held(q, bi, k);
-    cw[k] = rbt_window_held(q, bj, k);
+    rw[k] = rbt_window_held(q, bi * RBT_T, k);
+    cw[k] = rbt_window_held(q, bj * RBT_T, k);
   }
   __syncthreads();
   // the window of A from its upper triangle: entries on or above the diagonal along rows, the others along columns (coalesced both)
@@ -236,7 +288,7 @@ __global__ void __launch_bounds__(256) k_rbt_fused(int N, const double* __restri
     if(r < 0 || c < 0) continue;
     const rbt_pos pr = rbt_at(N, 2, r), pc = rbt_at(N, 2, c);
     if(pr.lo != r || pc.lo != c) continue;
-    const int k2 = pr.paired ? rbt_window_pos(q, bi, pr.hi) : k, l2 = pc.paired ? rbt_window_pos(q, bj, pc.hi) : l;
+    const int k2 = pr.paired ? rbt_window_pos(q, bi * RBT_T, pr.hi) : k, l2 = pc.paired ? rbt_window_pos(q, bj * RBT_T, pc.hi) : l;
     if(k2 < 0 || l2 < 0) continue;
     const double all = S[k * RBT_SLD + l], ahh = S[k2 * RBT_SLD + l2], alh = S[k * RBT_SLD + l2], ahl = S[k2 * RBT_SLD + l];
     const rbt_pos ph = rbt_at(N, 2, pr.hi), qh = rbt_at(N, 2, pc.hi);
@@ -256,15 +308,15 @@ __global__ void __launch_bounds__(256) k_rbt_fused(int N, const double* __restri
     int x1 = -1, x2 = -1;
     if(x >= 0) {
       px = rbt_at(N, 1, x);
-      x1 = rbt_window_pos(q, bx, px.lo);
-      x2 = rbt_window_pos(q, bx, px.hi);
+      x1 = rbt_window_pos(q, bx * RBT_T, px.lo);
+      x2 = rbt_window_pos(q, bx * RBT_T, px.hi);
     }
     for(int ro = ty; ro < RBT_OR; ro += 256 / RBT_OR) {
       const int y = rbt_out_row(q, bo, ro);
       double v = 0.0;
       if(x >= 0 && y >= 0) {
         const rbt_pos py = rbt_at(N, 1, y);
-        const int y1 = rbt_window_pos(q, bo, py.lo), y2 = rbt_window_pos(q, bo, py.hi);
+        const int y1 = rbt_window_pos(q, bo * RBT_T, py.lo), y2 = rbt_window_pos(q, bo * RBT_T, py.hi);
         // S is indexed [row of tile bi][column of tile bj]
         const int i = pass ? x : y, j = pass ? y : x;
         const int k1 = pass ? x1 : y1, k2 = pass ? x2 : y2, l1 = pass ? y1 : x1, l2 = pass ? y2 : x2;
@@ -300,7 +352,72 @@ __global__ void k_rbt_rowsum(int N, int nt, const double* __restrict__ part, dou
   }
 }
 
+// the quarters of order N with the window of a strip of `slots` slots per quarter (k_rbt_fused's layout with RBT_T -> slots)
+__host__ __device__ inline rbt_quarters rbt_strip_quarters(int N, int slots)
+{
+  rbt_quarters q = rbt_quarters_of(N);
+  q.W = slots + 2 * q.ext;
+  q.wr = 4 * q.W + (q.closed ? 0 : 3);
+  return q;
+}
+
+__global__ void k_rbt_window_map(rbt_quarters q, int s0, int s1, int* __restrict__ rows, int* __restrict__ pos_win, int* __restrict__ pos_out)
+{
+  const int n = q.N > q.wr ? q.N : q.wr;
+  for(int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+    if(e < q.wr) rows[e] = rbt_window_held(q, s0, e);
+    if(e < q.N) {
+      const int w = rbt_window_pos(q, s0, e), a = e >= q.s[3] ? 3 : e >= q.s[2] ? 2 : e >= q.s[1] ? 1 : 0, slot = e - q.s[a];
+      pos_win[e] = w;
+      pos_out[e] = slot >= s0 && slot < s1 ? w : -1;
+    }
+  }
+}
+
 } // namespace
+
+int hb_rbt_mirror(hb_ctx* c, int N, hb_rbt_rowmap m, int nrows, int ybeg, const double* src, long long ld, int q0, int nq, double* dst)
+{
+  if(nrows <= ybeg || nq <= 0) return HB_OK;
+  k_rbt_mirror<<<dim3((nq + 31) / 32, (nrows - ybeg + 31) / 32), 256, 0, c->stream>>>(N, m, nrows, ybeg, src, ld, q0, nq, dst);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+int hb_rbt_level(hb_ctx* c, int N, int level, const double* f, const double* in, long long ld, hb_rbt_rowmap m, int nsrc, const double* src, int q0,
+                 double* out)
+{
+  if(nsrc <= 0) return HB_OK;
+  k_rbt_level<<<dim3(nsrc, (N + RBT_COLS - 1) / RBT_COLS), 256, 0, c->stream>>>(N, level, f, in, ld, m, src, q0, out);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+hb_rbt_window hb_rbt_window_of(int N, int s0, int s1)
+{
+  const rbt_quarters q = rbt_strip_quarters(N, s1 - s0);
+  hb_rbt_window w{};
+  w.N = N; w.slots = q.len[0]; w.s0 = s0; w.s1 = s1; w.W = q.W; w.wr = q.wr; w.ext = q.ext;
+  for(int a = 0; a < 4; a++) { w.qs[a] = q.s[a]; w.qlen[a] = q.len[a]; }
+  for(int e = 0; e < 3; e++) w.sp[e] = q.sp[e];
+  return w;
+}
+
+int hb_rbt_window_map(hb_ctx* c, const hb_rbt_window& w, int* rows, int* pos_win, int* pos_out)
+{
+  const rbt_quarters q = rbt_strip_quarters(w.N, w.s1 - w.s0);
+  k_rbt_window_map<<<hb_grid(c, w.N > w.wr ? w.N : w.wr), 256, 0, c->stream>>>(q, w.s0, w.s1, rows, pos_win, pos_out);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+int hb_rbt_window_row(const hb_rbt_window& w, int k) { return rbt_window_held(rbt_strip_quarters(w.N, w.s1 - w.s0), w.s0, k); }
+
+bool hb_rbt_window_out(const hb_rbt_window& w, int g)
+{
+  const int a = g >= w.qs[3] ? 3 : g >= w.qs[2] ? 2 : g >= w.qs[1] ? 1 : 0, slot = g - w.qs[a];
+  return slot >= w.s0 && slot < w.s1;
+}
 
 int hb_rbt_table(hb_ctx* c, int N, double* f)
 {
@@ -431,8 +548,23 @@ extern "C" int hb_rbt_schedule_view(int N, int cap, int* dims4, int* ctas_host, 
   dims4[0] = q.nt; dims4[1] = nctas; dims4[2] = RBT_WMAX; dims4[3] = RBT_OR;
   for(int b = 0; b < nctas && b < cap; b++) rbt_cta_tiles(b, ctas_host[2 * b], ctas_host[2 * b + 1]);
   for(int t = 0; t < q.nt && t < cap; t++) {
-    for(int k = 0; k < RBT_WMAX; k++) window_host[(size_t)t * RBT_WMAX + k] = rbt_window_held(q, t, k);
+    for(int k = 0; k < RBT_WMAX; k++) window_host[(size_t)t * RBT_WMAX + k] = rbt_window_held(q, t * RBT_T, k);
     for(int k = 0; k < RBT_OR; k++) out_host[(size_t)t * RBT_OR + k] = rbt_out_row(q, t, k);
   }
+  return HB_OK;
+}
+
+// One strip of the out-of-core transform of order N, run on the host: see hiopb200.h.
+extern "C" int hb_rbt_strip_view(int N, int s0, int s1, int* wr_host, int* window_host, int* out_host)
+{
+  HB_REQUIRE(N >= 1 && s0 >= 0 && s1 > s0 && wr_host, "hb_rbt_strip_view: bad arguments");
+  const hb_rbt_window w = hb_rbt_window_of(N, s0, s1);
+  HB_REQUIRE(s1 <= w.slots, "hb_rbt_strip_view: the strip ends past the last slot");
+  *wr_host = w.wr;
+  if(window_host)
+    for(int k = 0; k < w.wr; k++) window_host[k] = hb_rbt_window_row(w, k);
+  if(out_host)
+    for(int a = 0; a < 4; a++)
+      for(int t = s0; t < s1; t++) out_host[a * (s1 - s0) + t - s0] = t < w.qlen[a] ? w.qs[a] + t : -1;
   return HB_OK;
 }

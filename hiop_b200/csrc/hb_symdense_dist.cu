@@ -14,8 +14,8 @@
 // (forward: rows k*128 .. N, backward: its block). Every block is computed in the same order for every P, so x does not depend on P.
 //
 // Safe mode (HB_FACT_RBT_NOPIV): A' = U^T A U with a depth-2 random butterfly U = B2 B1 (rbt_transform: the mirror of the upper
-// triangle, then one pass per level, each output row formed from its row and its partner row), the no-pivot LDL^T above on A', and
-// solves refined against a kept copy of A' (rbt_solve, the refinement loop of hb_rbt.cu). Every entry of A' is a fixed expression of oracle/rbt_model.py and the random
+// triangle, then one pass per level, each output row formed from its row and its partner row; the kernels live in hb_rbt.cu), the
+// no-pivot LDL^T above on A', and solves refined against a kept copy of A' (rbt_solve, the refinement loop of hb_rbt.cu). Every entry of A' is a fixed expression of oracle/rbt_model.py and the random
 // diagonals depend on N alone, so A', the factor and the solution do not depend on P either.
 #include "hb_common.cuh"
 #include "hb_dense.cuh"
@@ -23,57 +23,6 @@
 namespace {
 
 constexpr int DB = HB_ROWS_DB, HDR = HB_ROWS_HDR;
-
-// ---- random butterfly transform (HB_FACT_RBT_NOPIV): A' = U^T A U, U = B2 B1 (oracle/rbt_model.py states every expression; the
-// diagonals, the vector and row kernels and the refined solve are shared with hb_symdense in hb_rbt.cu) ------------------------------
-constexpr int RBT_COLS = 1024;               // columns per CTA of k_rbt_level (256 threads x 4)
-
-// mirror: every owned row r gets dst(r, j) = src(j, r) for the columns q0 <= j < q0 + nq, j < r, where src holds the rows q0 .. of the
-// upper triangle (ld doubles each). 32 x 32 tiles through shared memory: rows y0 .. of the owned rows, starting at local row ybeg.
-__global__ void __launch_bounds__(256) k_rbt_mirror(int N, int P, int rank, int nrows, int ybeg, const double* __restrict__ src, long long ld, int q0,
-                                                    int nq, double* __restrict__ dst)
-{
-  __shared__ double tile[32][33];
-  const int y0 = ybeg + blockIdx.y * 32, j0 = q0 + blockIdx.x * 32, tx = threadIdx.x % 32, ty = threadIdx.x / 32;
-  for(int jj = ty; jj < 32; jj += 8) {
-    const int y = y0 + tx, j = j0 + jj;
-    const int r = rbt_global_row(y, P, rank);
-    tile[jj][tx] = (y < nrows && r < N && j < q0 + nq && j < r) ? src[(size_t)(j - q0) * ld + r] : 0.0;
-  }
-  __syncthreads();
-  for(int yy = ty; yy < 32; yy += 8) {
-    const int y = y0 + yy, j = j0 + tx;
-    const int r = rbt_global_row(y, P, rank);
-    if(y < nrows && r < N && j < q0 + nq && j < r) dst[(size_t)y * ld + j] = tile[tx][yy];
-  }
-}
-
-// one level B^T A B on full rows. CTA x = a source row q: local row x of `in` (src == nullptr: every partner is local) or row x of src
-// (global rows q0 .. q0 + nq, the owner's broadcast). Its partner r (q itself when unpaired), when this rank owns it, gets its whole
-// output row from rows r and q: out(r, j) = (f_r f_j) (t w) with t and w of oracle/rbt_model.py, in that operation order.
-__global__ void __launch_bounds__(256) k_rbt_level(int N, int level, const double* __restrict__ f, const double* __restrict__ in, long long ld, int P,
-                                                   int rank, const double* __restrict__ src, int q0, double* __restrict__ out)
-{
-  const int q = src ? q0 + blockIdx.x : rbt_global_row(blockIdx.x, P, rank);
-  if(q >= N) return;
-  const double* rowq = src ? src + (size_t)blockIdx.x * ld : in + (size_t)blockIdx.x * ld;
-  const rbt_pos pq = rbt_at(N, level, q);
-  const int r = pq.lo == q ? pq.hi : pq.lo;
-  if((r / DB) % P != rank) return;
-  const size_t lr = (size_t)(r / DB / P) * DB + r % DB;
-  const double* rowr = in + lr * ld;
-  const rbt_pos pr = rbt_at(N, level, r);
-  const double* RL = pr.lo == r ? rowr : rowq;
-  const double* RH = pr.hi == r ? rowr : rowq;
-  const double* fl = f + (size_t)(level - 1) * N;
-  const double fi = fl[r];
-  double* o = out + lr * ld;
-  const int jend = min(N, (int)(blockIdx.y + 1) * RBT_COLS);
-  for(int j = blockIdx.y * RBT_COLS + threadIdx.x; j < jend; j += 256) {
-    const rbt_pos pj = rbt_at(N, level, j);
-    o[j] = rbt_entry(RL[pj.lo], RH[pj.hi], RL[pj.hi], RH[pj.lo], pr, pj, fi, fl[j]);
-  }
-}
 
 // Every rank's local result rc (HB_OK or an HB_ERR_* code) made common before the next collective, so that a rank whose allocation
 // failed never leaves the others waiting in a broadcast: all ranks return the most severe code (their own when they failed).
@@ -251,6 +200,7 @@ static int rbt_transform(hb_symdense_dist* s, int stages)
   const long long ld = s->ld;
   cudaStream_t st = c->stream;
   double* recv = s->bbuf[0];
+  const hb_rbt_rowmap cyclic{nullptr, nullptr, P, rank};
   if(s->profile) HB_CUDA(cudaEventRecord(s->ev_rbt[0], st));
   // mirror
   for(int k = 0; k < s->nblk; k++) {
@@ -260,30 +210,24 @@ static int rbt_transform(hb_symdense_dist* s, int stages)
     const int q0 = P == 1 ? 0 : k0, nq = P == 1 ? N : nb;
     const int qa = k <= rank ? 0 : (k - rank + P - 1) / P; // first owned block at or after k
     if(nrows > qa * DB) {
-      k_rbt_mirror<<<dim3((nq + 31) / 32, (nrows - qa * DB + 31) / 32), 256, 0, st>>>(N, P, rank, nrows, qa * DB, src, ld, q0, nq, s->A);
-      HB_LAUNCHED();
+      HB_CHECK(hb_rbt_mirror(c, N, cyclic, nrows, qa * DB, src, ld, q0, nq, s->A));
     }
     if(P == 1) break;
   }
   // the two levels: A -> Ak (B2), Ak -> A (B1)
-  const int chunks = (N + RBT_COLS - 1) / RBT_COLS;
   for(int st_i = 0; st_i < stages; st_i++) {
     const int level = st_i == 0 ? 2 : 1;
     const double* in = st_i == 0 ? s->A.get() : s->Ak.get();
     double* out = st_i == 0 ? s->Ak.get() : s->A.get();
     if(rbt_level_local(N, P, level)) {
-      if(nrows > 0) {
-        k_rbt_level<<<dim3(nrows, chunks), 256, 0, st>>>(N, level, s->rbt_f, in, ld, P, rank, nullptr, 0, out);
-        HB_LAUNCHED();
-      }
+      HB_CHECK(hb_rbt_level(c, N, level, s->rbt_f, in, ld, cyclic, nrows, nullptr, 0, out));
       continue;
     }
     for(int k = 0; k < s->nblk; k++) {
       const int owner = k % P, k0 = k * DB, nb = N - k0 < DB ? N - k0 : DB;
       double* src = owner == rank ? const_cast<double*>(in) + (size_t)(k / P) * DB * ld : recv;
       HB_CHECK(hb_broadcast(c, src, (long long)nb * ld, owner, st));
-      k_rbt_level<<<dim3(nb, chunks), 256, 0, st>>>(N, level, s->rbt_f, in, ld, P, rank, src, k0, out);
-      HB_LAUNCHED();
+      HB_CHECK(hb_rbt_level(c, N, level, s->rbt_f, in, ld, cyclic, nb, src, k0, out));
     }
   }
   if(stages == 1) HB_CUDA(cudaMemcpyAsync(s->A, s->Ak, sizeof(double) * nrows * ld, cudaMemcpyDeviceToDevice, st));

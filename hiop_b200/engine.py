@@ -309,33 +309,47 @@ class LinSolverSymDenseHost:
     """The dense symmetric solver of one GPU with the matrix in page-locked host memory (hb_symdense_host): Cholesky or no-pivot LDL^T,
     streamed through at most `device_bytes` of device memory (0: what is free, less a margin) in slabs of 128-row block rows. It owns
     a pinned n x n host tensor, matrix(); the caller fills its upper triangle, matrixChanged(mode) overwrites that triangle with the
-    factor and returns what LinSolverSymDense.matrixChanged does, solve(x) solves in place on the device. Bunch-Kaufman and RBT_NOPIV
-    are refused (use LinSolverSymDense, or LinSolverSymDenseDist for the safe mode)."""
+    factor and returns what LinSolverSymDense.matrixChanged does, solve(x) solves in place on the device. Bunch-Kaufman is refused (use
+    LinSolverSymDense). With rbt=True the handle also owns a second pinned n x n tensor for the kept A' of the safe mode, kept(), and
+    accepts RBT_NOPIV; without it RBT_NOPIV is refused (use LinSolverSymDenseDist, or pass rbt=True)."""
 
-    NOPIV, CHOLESKY = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY
+    NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
 
-    def __init__(self, ctx: Context, n: int, device_bytes: int = 0):
-        self.ctx, self.n = ctx, n
+    def __init__(self, ctx: Context, n: int, device_bytes: int = 0, rbt: bool = False):
+        self.ctx, self.n, self.rbt = ctx, n, rbt
         self.h = ctypes.c_void_p()
         check(ctx.L.hb_symdense_host_create(ctx.h, n, device_bytes, ctypes.byref(self.h)), "hb_symdense_host_create")
         self._M = torch.empty((n, n), dtype=torch.float64, pin_memory=True)
+        self._K = None
         check(ctx.L.hb_symdense_host_set_matrix(self.h, ctypes.c_void_p(self._M.data_ptr() if n else None), max(n, 1)),
               "hb_symdense_host_set_matrix")
+        if rbt:
+            self._K = torch.empty((n, n), dtype=torch.float64, pin_memory=True)
+            rc = ctx.L.hb_symdense_host_set_rbt_copy(self.h, ctypes.c_void_p(self._K.data_ptr() if n else None), max(n, 1))
+            if rc != 0:
+                self.close()
+                check(rc, "hb_symdense_host_set_rbt_copy")
 
     def close(self):
         if self.h:
             self.ctx.L.hb_symdense_host_destroy(self.h)
             self.h = None
             self._M = None
+            self._K = None
 
     def matrix(self) -> torch.Tensor:
         """the pinned n x n row-major host matrix the handle factors in place (upper triangle)"""
         return self._M
 
+    def kept(self) -> torch.Tensor:
+        """rbt=True: the pinned n x n host tensor that receives A' = U^T A U, both triangles, on each RBT_NOPIV factorization"""
+        return self._K
+
     def matrixChanged(self, mode: int) -> int:
-        if mode not in (self.NOPIV, self.CHOLESKY):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
-            raise EngineError("LinSolverSymDenseHost: only CHOLESKY and NOPIV stream from host memory; use LinSolverSymDense for "
-                              "Bunch-Kaufman, LinSolverSymDenseDist for RBT_NOPIV")
+        if mode not in (self.NOPIV, self.CHOLESKY) and not (self.rbt and mode == self.RBT_NOPIV):
+            # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
+            raise EngineError("LinSolverSymDenseHost: only CHOLESKY and NOPIV stream from host memory, and RBT_NOPIV with rbt=True; use "
+                              "LinSolverSymDense for Bunch-Kaufman")
         rc = self.ctx.L.hb_symdense_host_matrix_changed(self.h, mode)
         if rc < -1:
             check(rc, "hb_symdense_host_matrix_changed")
@@ -365,6 +379,28 @@ class LinSolverSymDenseHost:
         check(L.hb_symdense_host_plan_view(n, device_bytes, dims, first, b), "hb_symdense_host_plan_view")
         return {"slabs": dims[0], "blocks": dims[1], "slab_blocks": dims[2], "first": [first[i] for i in range(dims[0] + 1)],
                 "peak_bytes": b[0], "h2d_bytes": b[1], "d2h_bytes_cholesky": b[2], "d2h_bytes_ldlt": b[3], "solve_h2d_bytes": b[4]}
+
+    def rbt_stats(self):
+        """(largest corrections, largest backward error) over the groups of the last RBT solve, and the transform time (ms) of the last
+        RBT factorization"""
+        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
+        check(self.ctx.L.hb_symdense_host_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_host_rbt_stats")
+        return n.value, be.value, float(ms.value)
+
+    @staticmethod
+    def rbt_plan_view(n: int, device_bytes: int) -> dict:
+        """the plan of an RBT_NOPIV factorization of order n under device_bytes (host only): the transform's strips (their first slots,
+        and the number of slots at the end), slots per strip, window positions, the slab plan, peak device bytes and the bytes the
+        transform, the factorization and one residual pass copy"""
+        L = _lib.lib()
+        dims = (ctypes.c_int * 6)()
+        h = (n + 1) // 2
+        first = (ctypes.c_int * ((h + 1) // 2 + 2))()
+        b = (ctypes.c_longlong * 5)()
+        check(L.hb_symdense_host_rbt_plan_view(n, device_bytes, dims, first, b), "hb_symdense_host_rbt_plan_view")
+        return {"strips": dims[0], "strip_slots": dims[1], "slots": dims[2], "window": dims[3], "slabs": dims[4], "slab_blocks": dims[5],
+                "first": [first[i] for i in range(dims[0] + 1)], "peak_bytes": b[0], "transform_h2d_bytes": b[1],
+                "transform_d2h_bytes": b[2], "factor_h2d_bytes": b[3], "residual_h2d_bytes": b[4]}
 
 
 class KKTLinSysLowRank:

@@ -311,8 +311,9 @@ int hb_symdense_dist_profile(hb_symdense_dist* s, int on, float* ms3);
  * two panel buffers and applied in ascending order with the same K = 128 update kernel, the slab's own block rows are factored as the
  * P = 1 distributed loop does, and the slab is copied back. The factor, the return value and the inertia are bit-identical to
  * hb_symdense_dist at P = 1 (hence to hb_symdense with unpaired blocks) for every slab plan, and so are the solutions.
- * Bunch-Kaufman (its pivot search needs up-to-date columns) and HB_FACT_RBT_NOPIV (the butterfly needs partner rows and both triangles)
- * are refused with HB_ERR_INVALID and the handle stays usable; for the safe mode beyond one GPU use hb_symdense_dist.
+ * Bunch-Kaufman (its pivot search needs up-to-date columns) is refused with HB_ERR_INVALID and the handle stays usable. The safe mode
+ * HB_FACT_RBT_NOPIV keeps A' = U^T A U in a second page-locked buffer the caller registers (hb_symdense_host_set_rbt_copy); without
+ * one it is refused the same way.
  *
  * device_bytes: the device memory the handle may hold: the slab, the ring (4 x 128 ld doubles, ld = N rounded up to 8), 1/d and the
  * 16 x 16 inverses, the factor's diagonal and the scratch of a solve of 16 right-hand sides. The slab height is the largest multiple of 128
@@ -345,6 +346,44 @@ int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs);
  * device bytes, H2D bytes per factorization, D2H bytes per Cholesky factorization, D2H bytes per LDL^T factorization, H2D bytes per
  * solve of up to 16 right-hand sides (0 with one slab)}. Every output may be NULL. */
 int hb_symdense_host_plan_view(int N, size_t device_bytes, int* dims, int* slab_first_block_host, long long* bytes_host);
+/* The safe mode. K_host: the caller's N x N row-major buffer (ld >= N) for the kept A', borrowed like M_host: page-locked (checked at
+ * both ends) and apart from M_host, HB_ERR_INVALID otherwise; NULL unregisters it. Drops the factorization. The safe mode doubles the host
+ * memory of the system, so it is the caller's choice: without a registered copy hb_symdense_host_matrix_changed refuses
+ * HB_FACT_RBT_NOPIV with HB_ERR_INVALID.
+ *
+ * With a copy, hb_symdense_host_matrix_changed(s, HB_FACT_RBT_NOPIV) returns what hb_symdense_dist_matrix_changed returns in that mode,
+ * synchronously:
+ *   1. the transform, in strips of butterfly slots: the rows at those slots of the four quarters of the one-GPU transform's schedule,
+ *      read with their window (their level-2 and level-1 partners; for N = 1 mod 4 one slot more on each side and three fixed rows).
+ *      Each window row is assembled on the device from its upper part (copied from M_host) and its lower part (the window's columns of
+ *      the block rows above it, streamed through the ring and mirrored); then level 2 on the window rows and level 1 on the strip's rows,
+ *      each output row from its row and its partner row, with the distributed handle's kernels. M_host is only read. A' is written to
+ *      K_host in full, both triangles, bit-identical to oracle/rbt_model.py and to hb_symdense_dist's A'; ||A'||_inf is the same bits too.
+ *   2. the factorization above on A': each slab is copied in from K_host, and the strictly lower part of each 128 x 128 diagonal block
+ *      from M_host, so that M_host's strictly lower triangle comes back unchanged. The factor (in M_host's upper triangle), the return
+ *      value and the inertia are bit-identical to hb_symdense_dist at P = 1 in RBT mode for every slab plan.
+ * The transform needs no device memory beyond the handle's allocation (see hb_symdense_host_rbt_plan_view). Traffic: about 8 N^2 bytes
+ * H2D (the upper triangle once as rows and once as mirrored columns) and 8 N^2 bytes D2H (A') for the transform, then the plain
+ * factorization's traffic plus the diagonal blocks.
+ * hb_symdense_host_solve after it: per group of at most 16 right-hand sides, hb_symdense_dist_solve's refined solve (b' = U^T b, the
+ * sweeps above, residuals b' - A' x' formed block row by block row on block rows of K_host streamed through the ring, x = U x'), each
+ * group with its own stopping rule. So each group's x, corrections and omega are bit-identical to hb_symdense_dist_solve of that group.
+ * Returns 1 when every group's omega is finite, 0 otherwise. Each refinement pass reads K_host once (8 N^2 bytes). */
+int hb_symdense_host_set_rbt_copy(hb_symdense_host* s, double* K_host, long long ld);
+/* After an RBT factorization: the largest number of corrections and the largest backward error (a NaN wins) over the groups of the last
+ * solve, and the transform's time (ms, device events, every factorization). Every output may be NULL. */
+int hb_symdense_host_rbt_stats(hb_symdense_host* s, int* corrections, double* backward_error, float* transform_ms);
+/* The RBT plan of hb_symdense_host_create(N, device_bytes > 0), on the host. dims (6): {strips, slots per strip, slots (of the longest
+ * quarter), window positions per strip, slabs, block rows per slab}. strip_first_slot_host: strips + 1 entries, the first slot of each
+ * strip, then the number of slots. bytes_host (5): {peak device bytes (the handle's one allocation), transform H2D, transform D2H,
+ * factorization H2D, H2D of one residual pass}. The strips' X and Y buffers (2 x window positions x ld doubles) take the allocation from the
+ * factor's 1/d headers on; the row sums, the diagonals, the window's row maps and a solve's b' and residual take the second halves of
+ * the ring slots. So the slab plan is hb_symdense_host_plan_view's, and HB_ERR_INVALID exactly where that refuses. */
+int hb_symdense_host_rbt_plan_view(int N, size_t device_bytes, int* dims, int* strip_first_slot_host, long long* bytes_host);
+/* diagnostics (tests): strip [s0, s1) of the butterfly slots of order N, on the host. *wr_host: window positions; window_host (wr): the
+ * row read into each position (-1: none, or held at an earlier position); out_host (4 (s1 - s0), may be NULL): the rows the strip
+ * produces, quarter by quarter (-1 past a quarter's end). */
+int hb_rbt_strip_view(int N, int s0, int s1, int* wr_host, int* window_host, int* out_host);
 
 /* ------------------------------------------------------------------------------------------------------------
  * hiopKKTLinSysLowRank + hiopHessianLowRank (B2; src/Optimization/hiopKKTLinSys.cpp:1031-1350,

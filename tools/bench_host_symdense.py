@@ -1,6 +1,6 @@
 """Measures the dense symmetric solver with the matrix in page-locked host memory (hb_symdense_host) against hb_symdense in HBM.
 
-    python tools/bench_host_symdense.py [--sizes 22000] [--budget-gib 4,80] [--modes cholesky] [--repeats 3] [--warmup 1]
+    python tools/bench_host_symdense.py [--sizes 22000] [--budget-gib 4,80] [--modes cholesky,nopiv_ldlt,rbt] [--repeats 3] [--warmup 1]
 
 First line: the rate of plain pinned-host <-> device copies of 1 GiB (device events), the ceiling of the streaming. Then one JSON line
 per (N, budget, mode): factor ms (host clock around the synchronous call; the median, min and max of the repeats), solve ms for one
@@ -11,7 +11,13 @@ way and alternating with the host-resident runs, with max |x_host - x_hbm| (the 
 different kernels). The card's name and power limit are read in the same run.
 
 The matrix: uniform [0, 1) entries above the diagonal and 2 N on it (diagonally dominant; the no-pivot LDL^T gets -2 N on the first
-N / 3 diagonal entries, hence N / 3 negative eigenvalues). Only the upper triangle is filled; the factorization reads nothing else."""
+N / 3 diagonal entries, hence N / 3 negative eigenvalues). Only the upper triangle is filled; the factorization reads nothing else.
+
+--modes rbt (the safe mode, LinSolverSymDenseHost(rbt=True) on the no-pivot matrix): factor ms (host clock, transform included), the
+transform's ms (device events) and its share of the factor, its H2D + D2H bytes from the plan over its time, solve ms of one right-hand
+side with its corrections and omega, the strips and slabs, and the bytes of the plan; then the same matrix through hb_symdense_dist RBT
+at P = 1 (whose x the host handle reproduces bit for bit: max |x_host - x_dist| is reported) and, when it fits next to the device copy,
+through hb_symdense RBT in HBM, timed the same way."""
 import argparse
 import json
 import os
@@ -25,8 +31,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-CHOL, NOPIV = 2, 1
-MODES = {"cholesky": CHOL, "nopiv_ldlt": NOPIV}
+CHOL, NOPIV, RBT = 2, 1, 3
+MODES = {"cholesky": CHOL, "nopiv_ldlt": NOPIV, "rbt": RBT}
 
 
 def card():
@@ -69,6 +75,80 @@ def spread(v):
     return {"median": statistics.median(v), "min": min(v), "max": max(v)}
 
 
+def timed(call, sync):
+    sync()
+    t0 = time.perf_counter()
+    out = call()
+    sync()
+    return (time.perf_counter() - t0) * 1e3, out
+
+
+def run_rbt(ctx, N, gibs, args, info):
+    """one JSON line per budget: the safe mode on the host-resident handle against hb_symdense_dist (P = 1) and hb_symdense in HBM"""
+    from hiop_b200.engine import LinSolverSymDense, LinSolverSymDenseDist, LinSolverSymDenseHost
+    dev = ctx.device
+    src = torch.empty((N, N), dtype=torch.float64, pin_memory=True)
+    fill(src, NOPIV, seed=N + RBT)
+    b = torch.randn(N, generator=torch.Generator().manual_seed(7), dtype=torch.float64).to(dev)
+    sync = ctx.sync
+
+    def measure(setup, factor, solve, stats):
+        f_ms, s_ms = [], []
+        x = torch.empty_like(b)
+        for it in range(args.warmup + args.repeats):
+            setup()
+            ms, rc = timed(factor, sync)
+            with torch.cuda.stream(ctx.stream):
+                x.copy_(b)
+            ms_s, ok = timed(lambda: solve(x), sync)
+            if it >= args.warmup:
+                f_ms.append(ms)
+                s_ms.append(ms_s)
+        corr, om, t_ms = stats()
+        return {"rc": rc, "solve_ok": bool(ok), "factor_ms": spread(f_ms), "solve_ms": spread(s_ms), "corrections": corr, "omega": om,
+                "transform_ms": t_ms}, x
+
+    ref = {}
+    # hb_symdense_dist at P = 1 (A and A' on the device) and hb_symdense (the matrix, A' and the device copy it is filled from)
+    free = torch.cuda.mem_get_info(dev)[0]
+    if 3.3 * 8 * N * N < free:
+        Md = src.to(dev)
+        d = LinSolverSymDenseDist(ctx, N)
+        d.profile(True)
+        r, xd = measure(lambda: d.set_matrix(Md), lambda: d.matrixChanged(RBT), d.solve, d.rbt_stats)
+        d.profile(False)
+        d.close()
+        ref["hb_symdense_dist_p1"] = r
+        torch.cuda.empty_cache()
+        ss = LinSolverSymDense(ctx, N, RBT)
+
+        def sset():
+            ss.set_matrix(Md)
+            sync()
+        r, _ = measure(sset, ss.matrixChanged, ss.solve, ss.rbt_stats)
+        ss.close()
+        ref["hb_symdense_in_hbm"] = r
+        del Md
+        torch.cuda.empty_cache()
+    else:
+        xd = None
+    for gib in gibs:
+        budget = int(gib * (1 << 30))
+        p = LinSolverSymDenseHost.rbt_plan_view(N, budget)
+        s = LinSolverSymDenseHost(ctx, N, budget, rbt=True)
+        r, x = measure(lambda: s.matrix().copy_(src), lambda: s.matrixChanged(RBT), s.solve, s.rbt_stats)
+        s.close()
+        tx = r["transform_ms"]
+        print(json.dumps({"N": N, "mode": "rbt", "budget_gib": gib, "strips": p["strips"], "strip_slots": p["strip_slots"], "slabs": p["slabs"],
+                          "slab_block_rows": p["slab_blocks"], "peak_device_bytes": p["peak_bytes"], **r,
+                          "transform_share_of_factor": tx / r["factor_ms"]["median"],
+                          "transform_h2d_bytes": p["transform_h2d_bytes"], "transform_d2h_bytes": p["transform_d2h_bytes"],
+                          "transform_h2d_plus_d2h_GBps": (p["transform_h2d_bytes"] + p["transform_d2h_bytes"]) / (tx * 1e-3) / 1e9 if tx else None,
+                          "factor_h2d_bytes": p["factor_h2d_bytes"], "residual_h2d_bytes_per_pass": p["residual_h2d_bytes"],
+                          "max_abs_diff_x_vs_dist": float((x - xd).abs().max()) if xd is not None else None, **ref, **info}), flush=True)
+    del src
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sizes", default="22000")
@@ -90,6 +170,9 @@ def main():
     for N in [int(v) for v in args.sizes.split(",")]:
         for mname in args.modes.split(","):
             mode = MODES[mname]
+            if mode == RBT:
+                run_rbt(ctx, N, [float(v) for v in args.budget_gib.split(",")], args, info)
+                continue
             want = N // 3 if mode == NOPIV else 0
             src = torch.empty((N, N), dtype=torch.float64, pin_memory=True)
             fill(src, mode, seed=N + mode)
