@@ -552,9 +552,8 @@ __global__ void k_bk_dsolve(const double* __restrict__ F, long long ldf, int N, 
   x[k + 1] = (akm1 * bk - bkm1) / denom;
 }
 
-// inertia from the block diagonal with the reference's dsidi rule and thresholds (hiopLinSolverSymDenseLapack.hpp:127-167), all rows in
-// parallel: a 1x1 pivot contributes the sign of d; the first row of a 2x2 block (dsub != 0) contributes (d_k/t) d_k+1 - t and t = |dsub|.
-// ipiv == NULL: plain diagonal (no-pivot LDL^T / Cholesky factors).
+// inertia from the block diagonal with the reference's dsidi rule (hb_inertia_count), all rows in parallel: a 1x1 pivot contributes d;
+// the first row of a 2x2 block (dsub != 0) contributes (d_k/t) d_k+1 - t and t = |dsub|.
 __global__ void __launch_bounds__(1024)
 k_inertia_par(const double* __restrict__ F, long long ldf, int N, const int* __restrict__ ipiv, const double* __restrict__ dsub, int* __restrict__ out)
 {
@@ -564,15 +563,15 @@ k_inertia_par(const double* __restrict__ F, long long ldf, int N, const int* __r
   int neg = 0, nul = 0, pos = 0;
   for(int k = threadIdx.x; k < N; k += blockDim.x) {
     const double dk = LC(F, ldf, k, k);
-    if(!ipiv || ipiv[k] > 0) {
-      if(dk < -1e-14) neg++; else if(dk < 1e-14) nul++; else pos++;
+    if(ipiv[k] > 0) {
+      hb_inertia_count(dk, neg, nul, pos);
     } else {
       const double s = dsub[k];
       if(s != 0.0) {
         const double t = fabs(s);
         const double d1 = (dk / t) * LC(F, ldf, k + 1, k + 1) - t;
-        if(d1 < -1e-14) neg++; else if(d1 < 1e-14) nul++; else pos++;
-        if(t < 1e-14) nul++; else pos++;
+        hb_inertia_count(d1, neg, nul, pos);
+        hb_inertia_count(t, neg, nul, pos);
       }
     }
   }
@@ -670,11 +669,6 @@ int hb_dense_inertia_blockdiag(hb_ctx* c, int N, const double* F, long long ldf,
   k_inertia_par<<<1, 1024, 0, c->stream>>>(F, ldf, N, ipiv_dev, dsub_dev, out3_dev);
   HB_LAUNCHED();
   return HB_OK;
-}
-
-int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev)
-{
-  return hb_dense_inertia_blockdiag(c, N, F, ldf, nullptr, nullptr, out3_dev);
 }
 
 int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, double* x)

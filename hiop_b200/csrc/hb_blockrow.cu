@@ -29,8 +29,9 @@ __global__ void k_rows_recv(const double* __restrict__ hdr, const double* __rest
   }
 }
 
-// {neg, null, pos} of the owned diagonal entries with the +-1e-14 rule of the I_DIAG sweep (hb_dense_inertia_diag)
-__global__ void __launch_bounds__(1024) k_rows_inertia(const double* __restrict__ A, long long ld, int N, int P, int rank, int nloc, double* __restrict__ out3)
+// {neg, null, pos} of the owned diagonal entries (hb_rows_inertia): doubles for the block-row handles, ints for hb_symdense's info words
+template <typename T>
+__global__ void __launch_bounds__(1024) k_rows_inertia(const double* __restrict__ A, long long ld, int N, int P, int rank, int nloc, T* __restrict__ out3)
 {
   __shared__ int cnt[3];
   if(threadIdx.x < 3) cnt[threadIdx.x] = 0;
@@ -39,12 +40,11 @@ __global__ void __launch_bounds__(1024) k_rows_inertia(const double* __restrict_
   for(int e = threadIdx.x; e < nloc * DB; e += blockDim.x) {
     const int q = e / DB, t = e % DB, k0 = (q * P + rank) * DB;
     if(k0 + t >= N) continue;
-    const double d = A[(size_t)e * ld + k0 + t];
-    if(d < -1e-14) neg++; else if(d < 1e-14) nul++; else pos++;
+    hb_inertia_count(A[(size_t)e * ld + k0 + t], neg, nul, pos);
   }
   atomicAdd(&cnt[0], neg); atomicAdd(&cnt[1], nul); atomicAdd(&cnt[2], pos);
   __syncthreads();
-  if(threadIdx.x < 3) out3[threadIdx.x] = (double)cnt[threadIdx.x];
+  if(threadIdx.x < 3) out3[threadIdx.x] = (T)cnt[threadIdx.x];
 }
 
 // the nb x nb diagonal block of block column k0 into shared memory: S[j * DLD + i] = L(k0 + i, k0 + j), i >= j
@@ -145,13 +145,6 @@ int hb_rows::create()
   return HB_OK;
 }
 
-int hb_rows::finish(const double* counts, int info)
-{
-  n_neg = (int)counts[0]; n_null = (int)counts[1]; n_pos = (int)counts[2];
-  factored = info == 0; // a zero pivot / not SPD returns -1 and leaves no factorization, as hb_symdense_matrix_changed
-  return info != 0 || n_null > 0 ? -1 : n_neg;
-}
-
 int hb_rows_factor(hb_ctx* c, hb_rows& r, int N, double* A, long long ld, int P, int rank, int q0, int nsteps, bool ldl, double* inv16, int* info,
                    const std::function<int(int k, bool local, hb_rows_panel& b)>& at,
                    const std::function<int(int k, bool local, const hb_rows_panel& b)>& move, hb_event* prof)
@@ -217,6 +210,13 @@ int hb_rows_factor(hb_ctx* c, hb_rows& r, int N, double* A, long long ld, int P,
 int hb_rows_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st)
 {
   k_rows_inertia<<<1, 1024, 0, st>>>(A, ld, N, P, rank, nloc, out3);
+  HB_LAUNCHED();
+  return HB_OK;
+}
+
+int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev)
+{
+  k_rows_inertia<<<1, 1024, 0, c->stream>>>(F, ldf, N, 1, 0, (N + DB - 1) / DB, out3_dev);
   HB_LAUNCHED();
   return HB_OK;
 }

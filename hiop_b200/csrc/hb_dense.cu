@@ -876,9 +876,7 @@ k_inertia(const double* __restrict__ A, int lda, int N, const int* __restrict__ 
         t = 0.0;
       }
     }
-    if(d < -1e-14) neg++;
-    else if(d < 1e-14) nul++;
-    else pos++;
+    hb_inertia_count(d, neg, nul, pos);
   }
   out[0] = neg; out[1] = nul; out[2] = pos;
 }

@@ -47,7 +47,70 @@ __device__ inline ArgMax cta_argmax(ArgMax a, ArgMax* sm)
   return r;
 }
 
+// The inertia rule of the reference's dsidi sweep (hiopLinSolverSymDenseLapack.hpp:127-167) for one diagonal value of a factor: negative
+// below -1e-14, null up to 1e-14, positive otherwise (NaN included)
+__device__ __forceinline__ void hb_inertia_count(double d, int& neg, int& nul, int& pos)
+{
+  if(d < -1e-14) neg++; else if(d < 1e-14) nul++; else pos++;
+}
+
 struct hb_big;
+
+// ---- the outcome of a factorization, as hb_symdense, hb_symdense_dist and hb_symdense_host report it ----
+// The mode and result of the last matrix_changed with its inertia counts, and the statistics of the safe mode (HB_FACT_RBT_NOPIV):
+// ||A'||_inf and the transform time of the last factorization, the corrections and the backward error of the last solve.
+struct hb_dense_result
+{
+  int mode = -1;
+  bool factored = false;
+  int n_neg = 0, n_null = 0, n_pos = 0;
+  double rbt_anorm = 0.0, rbt_berr = 0.0;
+  int rbt_corr = 0;
+  float rbt_ms = 0.f;
+  // the end of matrix_changed, from the counts {neg, null, pos}: -1 after a breakdown (info != 0), which leaves no factorization
+  // ("matrix is singular", hiopLinSolverSymDenseLapack.hpp:109-116); else factored, and -1 with a null pivot (:166) or n_neg
+  template <typename T> int finish(const T* counts, int info)
+  {
+    n_neg = (int)counts[0]; n_null = (int)counts[1]; n_pos = (int)counts[2];
+    factored = info == 0;
+    return info != 0 || n_null > 0 ? -1 : n_neg;
+  }
+  // the *_inertia and *_rbt_stats getters; every output may be NULL
+  int inertia(int* neg, int* null, int* pos) const
+  {
+    if(neg) *neg = n_neg;
+    if(null) *null = n_null;
+    if(pos) *pos = n_pos;
+    return HB_OK;
+  }
+  int rbt_stats(int* corrections, double* backward_error, float* transform_ms) const
+  {
+    if(corrections) *corrections = rbt_corr;
+    if(backward_error) *backward_error = rbt_berr;
+    if(transform_ms) *transform_ms = rbt_ms;
+    return HB_OK;
+  }
+  // the precondition of <who>_solve: 1 when there is nothing to solve, HB_OK to go on, else the error
+  int solve_ready(int N, const void* x, int nrhs, const char* who) const
+  {
+    if(N == 0 || nrhs == 0) return 1;
+    if(!x) {
+      snprintf(g_hb_err, sizeof(g_hb_err), "%s_solve: null rhs (%s:%d)", who, __FILE__, __LINE__);
+      return HB_ERR_INVALID;
+    }
+    if(!factored) {
+      snprintf(g_hb_err, sizeof(g_hb_err), "%s_solve: no valid factorization (call %s_matrix_changed)", who, who);
+      return HB_ERR_STATE;
+    }
+    return HB_OK;
+  }
+  // a solve in groups of right-hand sides reports the most corrections and the largest omega of its groups (a NaN wins)
+  void merge_rbt(int corr, double berr)
+  {
+    rbt_corr = corr > rbt_corr ? corr : rbt_corr;
+    if(rbt_berr == rbt_berr && (berr != berr || berr > rbt_berr)) rbt_berr = berr;
+  }
+};
 
 // ---- dispatch by caller (hb_symdense.cu; the hb_symdense_* C-ABI is the fourth caller) ----
 // The 2l x 2l matrices of the compact BFGS inverse (V, Mdir): Bunch-Kaufman
@@ -139,10 +202,9 @@ int hb_bkc_dsolve(hb_ctx* c, int N, const double* F, long long ldf, const int* i
 int hb_bkc_profile(hb_ctx* c, int on, long long* prof_host8);
 #define HB_BKC_SWAPLOG_INTS(N) ((size_t)((N) / 7 + 4) * 132)
 #define HB_BKC_W_DOUBLES(ldw) ((size_t)(ldw) * (64 + 128)) /* W = L*D of a panel (<= 64 columns) + staging rows of the interchange kernel */
-// inertia {neg, null, pos} from the diagonal with the dsidi thresholds, all rows in parallel: of a cluster Bunch-Kaufman factor
-// (1x1 / 2x2 blocks marked by ipiv, off-diagonal in dsub), or of a Cholesky / no-pivot LDL^T factor (signs of the diagonal)
+// inertia {neg, null, pos} of a cluster Bunch-Kaufman factor with the dsidi rule, all rows in parallel (1x1 / 2x2 blocks marked by
+// ipiv, off-diagonal in dsub)
 int hb_dense_inertia_blockdiag(hb_ctx* c, int N, const double* F, long long ldf, const int* ipiv_dev, const double* dsub_dev, int* out3_dev);
-int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev);
 
 // ---- random butterfly transform (HB_FACT_RBT_NOPIV, hb_rbt.cu): A' = U^T A U, U = B2 B1, shared by hb_symdense and hb_symdense_dist ----
 // oracle/rbt_model.py states every expression; both handles produce the same bits of A', b' and x for a given N.
@@ -197,17 +259,12 @@ constexpr int HB_ROWS_HDR = 136; // step header: 1/d (128 doubles), the breakdow
 enum { HB_ROWS_PH_PANEL = 0, HB_ROWS_PH_MOVE, HB_ROWS_PH_UPDATE, HB_ROWS_PH_COUNT }; // profiled: panel chain, transport + fold, update
 int hb_rows_init_attrs();
 
-// What a block-row handle owns for the loop, and the outcome of its last factorization. The update stream is the context's.
-struct hb_rows
+// What a block-row handle owns for the loop, besides the outcome of its last factorization. The update stream is the context's.
+struct hb_rows : hb_dense_result
 {
   hb_stream sp;                                     // panel stream (high priority)
   hb_event ev_bc[2], ev_free[2], ev_ahead, ev_join; // per step parity: panel ready, operands free; look-ahead done; panel stream joined
-  int mode = -1;
-  bool factored = false;
-  int n_neg = 0, n_null = 0, n_pos = 0;
   int create();
-  // the end of matrix_changed: the counts {neg, null, pos}; -1 after a breakdown (info != 0); else factored, -1 with a null pivot, n_neg
-  int finish(const double* counts, int info);
 };
 
 // Where step k's panel lives on this rank: its header, and its rows from `sub` on (pan[p * ldp + i - sub]: row i of column k0 + p). A
@@ -227,8 +284,11 @@ struct hb_rows_panel { double* hdr; double* pan; long long ldp; int sub; double*
 int hb_rows_factor(hb_ctx* c, hb_rows& r, int N, double* A, long long ld, int P, int rank, int q0, int nsteps, bool ldl, double* inv16, int* info,
                    const std::function<int(int k, bool local, hb_rows_panel& b)>& at,
                    const std::function<int(int k, bool local, const hb_rows_panel& b)>& move, hb_event* prof = nullptr);
-// out3 = {neg, null, pos} of the diagonal entries A[e * ld + k0 + t] (e = q * 128 + t of the nloc owned blocks) with the +-1e-14 rule
+// out3 = {neg, null, pos} of the diagonal entries A[e * ld + k0 + t] (e = q * 128 + t of the nloc owned blocks) with hb_inertia_count,
+// as doubles (the counts the distributed handle all-reduces)
 int hb_rows_inertia(const double* A, long long ld, int N, int P, int rank, int nloc, double* out3, cudaStream_t st);
+// the same for the whole diagonal of a Cholesky / no-pivot LDL^T factor F (P = 1, A = F, ld = ldf, nloc = ceil(N / 128)), as ints
+int hb_dense_inertia_diag(hb_ctx* c, int N, const double* F, long long ldf, int* out3_dev);
 // The forward steps on the row-major N x nrhs xw (y_k = L_kk^-1 b_k, b_>k -= L_>k,k y_k, LDL^T: z_k = y_k / d_k) in ascending block order,
 // then the backward steps (x_k = L_kk^-T (z_k - L_>k,k^T x_>k)) in descending order. rows(k, &Ak): block row k addressed like the factor
 // (Ak[(k0 + p) * ld + i] = L(i, k0 + p)), or null when another rank computes it; after(k, forward) runs after each. ybuf, tdot: 128 nrhs.
@@ -288,8 +348,11 @@ struct hb_rbt_trace
 int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, double* xw, double* bp, double* rw, double* nrm_host,
                  const std::function<int(double*)>& sweeps, const std::function<int(const double*, const double*, double*)>& residual, int* corr,
                  double* berr, hb_rbt_trace* trace = nullptr);
-// copies a trace into the host buffers of hb_debug_symdense_rbt_solve / hb_debug_symdense_dist_rbt_solve (every one may be NULL)
-void hb_rbt_trace_out(const hb_rbt_trace& t, int* passes, double* anorm, double* norms, double* xp, double* bp);
+// The traced solve of the debug entries hb_debug_symdense_rbt_solve / hb_debug_symdense_dist_rbt_solve (who): HB_ERR_STATE without an
+// RBT factorization in r; else solve(trace), its return value into *ret_host and what the trace read into the host buffers (every one
+// may be NULL)
+int hb_rbt_traced_solve(const hb_dense_result& r, const char* who, const std::function<int(hb_rbt_trace*)>& solve, int* ret_host, int* passes,
+                        double* anorm, double* norms, double* xp, double* bp);
 // One GPU: A' from the upper triangle of A (ld lda; the other triangle is not read) in one pass (k_rbt_fused): the upper triangle of A'
 // into F (ldf; may be A itself when hb_rbt_in_place(N), NULL for none), the full A' into Ak (ldk), ||A'||_inf into nrm_dev[0].
 // part: hb_rbt_part_doubles(N) doubles of row-sum scratch.

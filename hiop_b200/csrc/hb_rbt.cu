@@ -512,13 +512,20 @@ int hb_rbt_solve(hb_ctx* c, int N, int nrhs, const double* f, double anorm, doub
   return std::isfinite(om) ? 1 : 0;
 }
 
-void hb_rbt_trace_out(const hb_rbt_trace& t, int* passes, double* anorm, double* norms, double* xp, double* bp)
+int hb_rbt_traced_solve(const hb_dense_result& r, const char* who, const std::function<int(hb_rbt_trace*)>& solve, int* ret_host, int* passes,
+                        double* anorm, double* norms, double* xp, double* bp)
 {
+  if(!r.factored || r.mode != HB_FACT_RBT_NOPIV) return hb_fail(HB_ERR_STATE, "%s: no valid RBT factorization", who);
+  hb_rbt_trace t;
+  const int ok = solve(&t);
+  if(ok < 0) return ok;
+  if(ret_host) *ret_host = ok;
   if(passes) *passes = (int)(t.b.empty() ? 0 : t.x.size() / t.b.size());
   if(anorm) *anorm = t.anorm;
   if(norms) std::copy(t.norms.begin(), t.norms.end(), norms);
   if(xp) std::copy(t.x.begin(), t.x.end(), xp);
   if(bp) std::copy(t.b.begin(), t.b.end(), bp);
+  return HB_OK;
 }
 
 bool hb_rbt_in_place(int N) { return rbt_quarters_of(N).closed; }

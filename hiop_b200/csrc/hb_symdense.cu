@@ -152,7 +152,7 @@ int hb_dense_lsq_factor(hb_ctx* c, int N, double* A, int lda, int* info_dev)
 }
 int hb_dense_lsq_solve(hb_ctx* c, int N, const double* F, int ldf, double* x) { return hb_dense_tri_solve(c, N, F, ldf, false, x); }
 
-struct hb_symdense
+struct hb_symdense : hb_dense_result // mode, factored, the inertia counts and the safe mode's statistics
 {
   hb_ctx* ctx = nullptr;
   int N = 0;
@@ -173,18 +173,12 @@ struct hb_symdense
   hb_dev<int> ipiv;
   hb_dev<int> info;         // device: [0] info, [1..3] inertia
   hb_pinned<int> info_host;
-  int mode = -1;
   int bk_widths = 0;        // cluster Bunch-Kaufman: OR of the panel widths (8 / 16 / 32 / 64) the last factorization launched (no order)
-  bool factored = false;
-  int n_neg = 0, n_null = 0, n_pos = 0;
   // HB_FACT_RBT_NOPIV, allocated by the first RBT factorization: A' (N x N, full), the butterfly diagonals (2 N), row-sum scratch and
   // ||A'||_inf; the solve adds the rows of x and b', the residual and per-rhs norms
   hb_dev<double> Ak, rbt_f, rbt_part, rbt_nrm, rbt_xw, rbt_b, rbt_r, rbt_col;
   hb_pinned<double> rbt_nrm_host;
   hb_event ev_rbt[2];
-  double rbt_anorm = 0.0, rbt_berr = 0.0;
-  int rbt_corr = 0;
-  float rbt_ms = 0.f;
 };
 
 extern "C" int hb_symdense_create(hb_ctx* c, int N, hb_symdense** out)
@@ -277,7 +271,7 @@ extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
   const bool rbt = mode == HB_FACT_RBT_NOPIV;
   s->mode = mode;
   s->factored = false;
-  if(N == 0) { s->factored = true; s->n_neg = s->n_null = s->n_pos = 0; return 0; }
+  if(N == 0) { const int none[3] = {0, 0, 0}; return s->finish(none, 0); }
   HB_CUDA(cudaMemsetAsync(s->info, 0, sizeof(int) * 4, c->stream));
   s->big.inv_valid = false;
   const Plan p = symdense_plan(c, rbt ? HB_FACT_NOPIV : mode, N);
@@ -320,20 +314,13 @@ extern "C" int hb_symdense_matrix_changed(hb_symdense* s, int mode)
   }
   HB_CUDA(cudaMemcpyAsync(s->info_host, s->info, sizeof(int) * 4, cudaMemcpyDeviceToHost, c->stream));
   HB_CUDA(cudaStreamSynchronize(c->stream));
-  s->n_neg = s->info_host[1]; s->n_null = s->info_host[2]; s->n_pos = s->info_host[3];
-  if(s->info_host[0] != 0) return -1; // zero pivot / not SPD: "matrix is singular" (hiopLinSolverSymDenseLapack.hpp:109-116)
-  s->factored = true;
-  if(s->n_null > 0) return -1;        // :166
-  return s->n_neg;
+  return s->finish(s->info_host + 1, s->info_host[0]);
 }
 
 extern "C" int hb_symdense_inertia(hb_symdense* s, int* n_neg, int* n_null, int* n_pos)
 {
   HB_REQUIRE(s, "null handle");
-  if(n_neg) *n_neg = s->n_neg;
-  if(n_null) *n_null = s->n_null;
-  if(n_pos) *n_pos = s->n_pos;
-  return HB_OK;
+  return s->inertia(n_neg, n_null, n_pos);
 }
 
 // the sweeps of the current factor on nrhs right-hand sides stored one after the other, in place
@@ -387,9 +374,7 @@ static int rbt_solve(hb_symdense* s, double* x, int nrhs, hb_rbt_trace* trace = 
 extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
 {
   HB_REQUIRE(s && nrhs >= 0, "hb_symdense_solve: bad arguments");
-  if(s->N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_solve: no valid factorization (call hb_symdense_matrix_changed)%s", "");
+  if(const int rc = s->solve_ready(s->N, x, nrhs, "hb_symdense"); rc != HB_OK) return rc;
   if(s->mode == HB_FACT_RBT_NOPIV) return rbt_solve(s, x, nrhs);
   HB_CHECK(plan_sweeps(s, x, nrhs));
   return 1;
@@ -398,10 +383,7 @@ extern "C" int hb_symdense_solve(hb_symdense* s, double* x, int nrhs)
 extern "C" int hb_symdense_rbt_stats(hb_symdense* s, int* corrections, double* backward_error, float* transform_ms)
 {
   HB_REQUIRE(s, "null handle");
-  if(corrections) *corrections = s->rbt_corr;
-  if(backward_error) *backward_error = s->rbt_berr;
-  if(transform_ms) *transform_ms = s->rbt_ms;
-  return HB_OK;
+  return s->rbt_stats(corrections, backward_error, transform_ms);
 }
 
 // diagnostics (tests): the RBT transform of the upper triangle of M without factoring; A' (full) and the factor buffer's upper triangle
@@ -430,15 +412,11 @@ extern "C" int hb_debug_symdense_rbt_solve(hb_symdense* s, double* x, int nrhs, 
                                            double* anorm_host, double* norms_host, double* xp_host, double* bp_host)
 {
   HB_REQUIRE(s && x && nrhs > 0 && s->N > 0, "hb_debug_symdense_rbt_solve: bad arguments");
-  if(!s->factored || s->mode != HB_FACT_RBT_NOPIV)
-    return hb_fail(HB_ERR_STATE, "hb_debug_symdense_rbt_solve: no valid RBT factorization%s", "");
-  HB_CUDA(cudaSetDevice(s->ctx->device));
-  hb_rbt_trace t;
-  const int ok = rbt_solve(s, x, nrhs, &t, Aref, anorm);
-  if(ok < 0) return ok;
-  if(ret_host) *ret_host = ok;
-  hb_rbt_trace_out(t, passes_host, anorm_host, norms_host, xp_host, bp_host);
-  return HB_OK;
+  auto solve = [&](hb_rbt_trace* t) -> int {
+    HB_CUDA(cudaSetDevice(s->ctx->device));
+    return rbt_solve(s, x, nrhs, t, Aref, anorm);
+  };
+  return hb_rbt_traced_solve(*s, "hb_debug_symdense_rbt_solve", solve, ret_host, passes_host, anorm_host, norms_host, xp_host, bp_host);
 }
 
 extern "C" int hb_symdense_matrix_changed_host(hb_symdense* s, const double* M_host, int mode)

@@ -42,7 +42,7 @@ int agree(hb_ctx* c, int rc)
 
 } // namespace
 
-struct hb_symdense_dist : hb_rows // the panel stream, the step loop's events, mode, factored and the inertia counts
+struct hb_symdense_dist : hb_rows // the panel stream, the step loop's events and the outcome record
 {
   hb_ctx* ctx = nullptr;
   int N = 0, P = 1, rank = 0, nblk = 0, nloc = 0;
@@ -66,9 +66,6 @@ struct hb_symdense_dist : hb_rows // the panel stream, the step loop's events, m
   hb_dev<double> Ak, rbt_f, rbt_rows, rbt_nrm, rbt_b, rbt_r;
   hb_pinned<double> rbt_nrm_host;
   hb_event ev_rbt[2];
-  double rbt_anorm = 0.0, rbt_berr = 0.0;
-  int rbt_corr = 0;
-  float rbt_ms = 0.f;
   ~hb_symdense_dist()
   {
     if(sp) cudaStreamSynchronize(sp);
@@ -259,10 +256,7 @@ extern "C" int hb_debug_symdense_dist_rbt(hb_symdense_dist* s, int stages)
 extern "C" int hb_symdense_dist_rbt_stats(hb_symdense_dist* s, int* corrections, double* backward_error, float* transform_ms)
 {
   HB_REQUIRE(s, "null handle");
-  if(corrections) *corrections = s->rbt_corr;
-  if(backward_error) *backward_error = s->rbt_berr;
-  if(transform_ms) *transform_ms = s->rbt_ms;
-  return HB_OK;
+  return s->rbt_stats(corrections, backward_error, transform_ms);
 }
 
 extern "C" int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode)
@@ -308,16 +302,13 @@ extern "C" int hb_symdense_dist_matrix_changed(hb_symdense_dist* s, int mode)
         s->phase_ms[ph] += ms;
       }
   }
-  return s->finish(s->red_host, s->info_host[0]);
+  return s->finish(s->red_host.get(), s->info_host[0]);
 }
 
 extern "C" int hb_symdense_dist_inertia(hb_symdense_dist* s, int* n_neg, int* n_null, int* n_pos)
 {
   HB_REQUIRE(s, "null handle");
-  if(n_neg) *n_neg = s->n_neg;
-  if(n_null) *n_null = s->n_null;
-  if(n_pos) *n_pos = s->n_pos;
-  return HB_OK;
+  return s->inertia(n_neg, n_null, n_pos);
 }
 
 // the forward and backward sweeps of the factor on the replicated row-major N x nrhs vectors xw, in place: the owner of block k computes
@@ -389,9 +380,7 @@ static int dist_solve(hb_symdense_dist* s, double* x, int nrhs, hb_rbt_trace* tr
 extern "C" int hb_symdense_dist_solve(hb_symdense_dist* s, double* x, int nrhs)
 {
   HB_REQUIRE(s && nrhs >= 0, "hb_symdense_dist_solve: bad arguments");
-  if(s->N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_dist_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_dist_solve: no valid factorization (call hb_symdense_dist_matrix_changed)%s", "");
+  if(const int rc = s->solve_ready(s->N, x, nrhs, "hb_symdense_dist"); rc != HB_OK) return rc;
   return dist_solve(s, x, nrhs, nullptr);
 }
 
@@ -400,12 +389,6 @@ extern "C" int hb_debug_symdense_dist_rbt_solve(hb_symdense_dist* s, double* x, 
                                                 double* norms_host, double* xp_host, double* bp_host)
 {
   HB_REQUIRE(s && x && nrhs > 0 && s->N > 0, "hb_debug_symdense_dist_rbt_solve: bad arguments");
-  if(!s->factored || s->mode != HB_FACT_RBT_NOPIV)
-    return hb_fail(HB_ERR_STATE, "hb_debug_symdense_dist_rbt_solve: no valid RBT factorization%s", "");
-  hb_rbt_trace t;
-  const int ok = dist_solve(s, x, nrhs, &t);
-  if(ok < 0) return ok;
-  if(ret_host) *ret_host = ok;
-  hb_rbt_trace_out(t, passes_host, anorm_host, norms_host, xp_host, bp_host);
-  return HB_OK;
+  auto solve = [&](hb_rbt_trace* t) { return dist_solve(s, x, nrhs, t); };
+  return hb_rbt_traced_solve(*s, "hb_debug_symdense_dist_rbt_solve", solve, ret_host, passes_host, anorm_host, norms_host, xp_host, bp_host);
 }

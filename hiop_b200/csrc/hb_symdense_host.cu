@@ -210,7 +210,7 @@ __global__ void k_keep_lower(int nb, const double* __restrict__ T, long long ld,
 
 } // namespace
 
-struct hb_symdense_host : hb_rows // the panel stream, the step loop's events, mode, factored and the inertia counts
+struct hb_symdense_host : hb_rows // the panel stream, the step loop's events and the outcome record
 {
   hb_ctx* ctx = nullptr;
   plan_t p;
@@ -226,9 +226,6 @@ struct hb_symdense_host : hb_rows // the panel stream, the step loop's events, m
   hb_stream sc;                // copy stream
   hb_event ev_in[2], ev_read[2], ev_out[2], ev_a, ev_b, ev_panel, ev_t[2];
   bool resident = false;
-  double rbt_anorm = 0.0, rbt_berr = 0.0;
-  int rbt_corr = 0;
-  float rbt_ms = 0.f;
   double* at(size_t off) const { return mem.get() + off; }
   double* slot(int j) const { return mem.get() + p.ring + (size_t)j * 2 * DB * p.ld; } // W or L rows; the formed L follows at + 128 ld
   double* half(int j) const { return slot(j) + (size_t)DB * p.ld; }                    // that second half
@@ -560,16 +557,13 @@ extern "C" int hb_symdense_host_matrix_changed(hb_symdense_host* s, int mode)
   if(rbt) HB_CHECK(rbt_transform(s));
   HB_CHECK(factor(s, ldl));
   s->resident = p.nslab == 1;
-  return s->finish(s->host, *reinterpret_cast<const int*>(s->host.get() + 3));
+  return s->finish(s->host.get(), *reinterpret_cast<const int*>(s->host.get() + 3));
 }
 
 extern "C" int hb_symdense_host_inertia(hb_symdense_host* s, int* n_neg, int* n_null, int* n_pos)
 {
   HB_REQUIRE(s, "null handle");
-  if(n_neg) *n_neg = s->n_neg;
-  if(n_null) *n_null = s->n_null;
-  if(n_pos) *n_pos = s->n_pos;
-  return HB_OK;
+  return s->inertia(n_neg, n_null, n_pos);
 }
 
 extern "C" int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs)
@@ -577,9 +571,7 @@ extern "C" int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs)
   HB_REQUIRE(s && nrhs >= 0, "hb_symdense_host_solve: bad arguments");
   const plan_t& p = s->p;
   const int N = p.N;
-  if(N == 0 || nrhs == 0) return 1;
-  HB_REQUIRE(x, "hb_symdense_host_solve: null rhs");
-  if(!s->factored) return hb_fail(HB_ERR_STATE, "hb_symdense_host_solve: no valid factorization (call hb_symdense_host_matrix_changed)%s", "");
+  if(const int rc = s->solve_ready(N, x, nrhs, "hb_symdense_host"); rc != HB_OK) return rc;
   hb_ctx* c = s->ctx;
   HB_CUDA(cudaSetDevice(c->device));
   cudaStream_t su = c->stream;
@@ -636,8 +628,7 @@ extern "C" int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs)
       const int rc = hb_rbt_solve(c, N, ng, r.f, s->rbt_anorm, xw, r.bp, r.rw, s->host.get() + 8, sweeps, residual, &corr, &berr);
       if(rc < 0) return rc;
       ok &= rc;
-      s->rbt_corr = std::max(s->rbt_corr, corr);
-      if(s->rbt_berr == s->rbt_berr && (berr != berr || berr > s->rbt_berr)) s->rbt_berr = berr; // a NaN wins
+      s->merge_rbt(corr, berr);
     }
     HB_CHECK(hb_rbt_to_rows(c, N, ng, xg, xw, true));
   }
@@ -648,10 +639,7 @@ extern "C" int hb_symdense_host_solve(hb_symdense_host* s, double* x, int nrhs)
 extern "C" int hb_symdense_host_rbt_stats(hb_symdense_host* s, int* corrections, double* backward_error, float* transform_ms)
 {
   HB_REQUIRE(s, "null handle");
-  if(corrections) *corrections = s->rbt_corr;
-  if(backward_error) *backward_error = s->rbt_berr;
-  if(transform_ms) *transform_ms = s->rbt_ms;
-  return HB_OK;
+  return s->rbt_stats(corrections, backward_error, transform_ms);
 }
 
 extern "C" int hb_symdense_host_rbt_plan_view(int N, size_t device_bytes, int* dims, int* strip_first_slot_host, long long* bytes_host)

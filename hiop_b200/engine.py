@@ -160,11 +160,59 @@ class Context:
         check(self.L.hb_mat_trans_times_vec(self.h, m, n, _ptr(A), n, beta, _ptr(y), alpha, _ptr(x)), "hb_mat_trans_times_vec")
 
 
-class LinSolverSymDense:
+class _DenseSolver:
+    """What the three dense symmetric solvers share, on the C-ABI functions <_C>_destroy, _matrix_changed, _inertia, _solve and
+    _rbt_stats of the handle h"""
+
+    _C = ""
+    _HELD = ()      # attributes that view or lend memory to the handle: dropped with it
+
+    def _fn(self, name):
+        return getattr(self.ctx.L, self._C + name)
+
+    def close(self):
+        if self.h:
+            self._fn("_destroy")(self.h)
+            self.h = None
+            for a in self._HELD:
+                setattr(self, a, None)
+
+    @staticmethod
+    def _factored(rc: int, name: str) -> int:
+        if rc < -1:     # -1 is a breakdown or a null pivot, not an error
+            check(rc, name)
+        return rc
+
+    def _matrix_changed(self, mode: int) -> int:
+        return self._factored(self._fn("_matrix_changed")(self.h, mode), self._C + "_matrix_changed")
+
+    def inertia(self):
+        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        check(self._fn("_inertia")(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), self._C + "_inertia")
+        return a.value, b.value, c.value
+
+    def solve(self, x: torch.Tensor) -> bool:
+        nrhs = x.numel() // max(self.n, 1) if self.n else 0
+        rc = self._fn("_solve")(self.h, _ptr(x), nrhs)
+        if rc < 0:
+            check(rc, self._C + "_solve")
+        return rc == 1
+
+    def rbt_stats(self):
+        """(corrections, backward error) of the last RBT_NOPIV solve and the transform time (ms) of the last RBT_NOPIV factorization.
+        LinSolverSymDenseDist reports a transform time of 0 unless profiling; LinSolverSymDenseHost reports the largest corrections and
+        backward error over the groups of right-hand sides of the solve."""
+        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
+        check(self._fn("_rbt_stats")(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), self._C + "_rbt_stats")
+        return n.value, be.value, float(ms.value)
+
+
+class LinSolverSymDense(_DenseSolver):
     """hiopLinSolverSymDense: owns the N x N row-major system matrix (upper triangle valid), `matrixChanged()` returns
     the number of negative eigenvalues or -1, `solve(x)` overwrites the rhs (src/LinAlg/hiopLinSolver.hpp:78-128)."""
 
     BUNCH_KAUFMAN, NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_BUNCH_KAUFMAN, _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
+    _C = "hb_symdense"
 
     def __init__(self, ctx: Context, n: int, mode: int = _lib.HB_FACT_BUNCH_KAUFMAN):
         self.ctx, self.n, self.mode = ctx, n, mode
@@ -172,40 +220,18 @@ class LinSolverSymDense:
         check(ctx.L.hb_symdense_create(ctx.h, n, ctypes.byref(self.h)), "hb_symdense_create")
         self._mptr = ctx.L.hb_symdense_matrix(self.h)
 
-    def close(self):
-        if self.h:
-            self.ctx.L.hb_symdense_destroy(self.h)
-            self.h = None
-
     def set_matrix(self, M: torch.Tensor):
         """Fills sysMatrix() from a device tensor (what the KKT class's build_kkt_matrix does in place)."""
         assert M.shape == (self.n, self.n)
         check(self.ctx.L.hb_memcpy_d2d(self.ctx.h, ctypes.c_void_p(self._mptr), _ptr(M.contiguous()), 8 * self.n * self.n), "memcpy")
 
     def matrixChanged(self) -> int:
-        rc = self.ctx.L.hb_symdense_matrix_changed(self.h, self.mode)
-        if rc < -1:
-            check(rc, "hb_symdense_matrix_changed")
-        return rc
+        return self._matrix_changed(self.mode)
 
     def matrixChanged_host(self, M: np.ndarray) -> int:
         M = np.ascontiguousarray(M, dtype=np.float64)
         rc = self.ctx.L.hb_symdense_matrix_changed_host(self.h, M.ctypes.data_as(ctypes.c_void_p), self.mode)
-        if rc < -1:
-            check(rc, "hb_symdense_matrix_changed_host")
-        return rc
-
-    def inertia(self):
-        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        check(self.ctx.L.hb_symdense_inertia(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "hb_symdense_inertia")
-        return a.value, b.value, c.value
-
-    def solve(self, x: torch.Tensor) -> bool:
-        nrhs = x.numel() // max(self.n, 1) if self.n else 0
-        rc = self.ctx.L.hb_symdense_solve(self.h, _ptr(x), nrhs)
-        if rc < 0:
-            check(rc, "hb_symdense_solve")
-        return rc == 1
+        return self._factored(rc, "hb_symdense_matrix_changed_host")
 
     def solve_host(self, x: np.ndarray) -> bool:
         assert x.dtype == np.float64 and x.flags["C_CONTIGUOUS"]
@@ -214,12 +240,6 @@ class LinSolverSymDense:
         if rc < 0:
             check(rc, "hb_symdense_solve_host")
         return rc == 1
-
-    def rbt_stats(self):
-        """(corrections, backward error) of the last RBT_NOPIV solve and the transform time (ms) of the last RBT_NOPIV factorization"""
-        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
-        check(self.ctx.L.hb_symdense_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_rbt_stats")
-        return n.value, be.value, float(ms.value)
 
 
 class _DeviceArray:
@@ -230,7 +250,7 @@ class _DeviceArray:
         self._owner = owner
 
 
-class LinSolverSymDenseDist:
+class LinSolverSymDenseDist(_DenseSolver):
     """The dense symmetric solver with the matrix factored across the context's ranks (hb_symdense_dist): Cholesky, no-pivot LDL^T, or
     (RBT_NOPIV, the safe mode) no-pivot LDL^T of a random butterfly transform U^T A U with refined solves, on a 1-D block-cyclic layout
     of 128-row blocks (sharding.block_rows). Every call is collective over the ranks; with one rank (no
@@ -238,6 +258,7 @@ class LinSolverSymDenseDist:
     solve(x) takes and returns x replicated on every rank."""
 
     NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
+    _C, _HELD = "hb_symdense_dist", ("_local",)
 
     def __init__(self, ctx: Context, n: int):
         self.ctx, self.n = ctx, n
@@ -250,12 +271,6 @@ class LinSolverSymDenseDist:
         assert len(self.rows) == self.n_blocks
         self._local = torch.as_tensor(_DeviceArray(ptr.value or 0, (self.n_blocks * sharding.DIST_BLOCK, self.ld), self), device=ctx.device) \
             if self.n_blocks else torch.empty((0, self.ld), dtype=torch.float64, device=ctx.device)
-
-    def close(self):
-        if self.h:
-            self._local = None
-            self.ctx.L.hb_symdense_dist_destroy(self.h)
-            self.h = None
 
     def local(self) -> torch.Tensor:
         """(n_blocks * 128) x ld view of this rank's block rows, stacked in the order of sharding.block_rows; columns >= n are padding"""
@@ -275,22 +290,7 @@ class LinSolverSymDenseDist:
         if mode not in (self.NOPIV, self.CHOLESKY, self.RBT_NOPIV):    # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
             raise EngineError("LinSolverSymDenseDist: Bunch-Kaufman is not distributed (its pivot search needs every column); use RBT_NOPIV "
                               "for the safe mode, or LinSolverSymDense")
-        rc = self.ctx.L.hb_symdense_dist_matrix_changed(self.h, mode)
-        if rc < -1:
-            check(rc, "hb_symdense_dist_matrix_changed")
-        return rc
-
-    def inertia(self):
-        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        check(self.ctx.L.hb_symdense_dist_inertia(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "hb_symdense_dist_inertia")
-        return a.value, b.value, c.value
-
-    def solve(self, x: torch.Tensor) -> bool:
-        nrhs = x.numel() // max(self.n, 1) if self.n else 0
-        rc = self.ctx.L.hb_symdense_dist_solve(self.h, _ptr(x), nrhs)
-        if rc < 0:
-            check(rc, "hb_symdense_dist_solve")
-        return rc == 1
+        return self._matrix_changed(mode)
 
     def profile(self, on: bool):
         """arm (on=True) / read (on=False -> (panel chain, broadcast, trailing update) ms of the last factorization on this rank)"""
@@ -298,14 +298,8 @@ class LinSolverSymDenseDist:
         check(self.ctx.L.hb_symdense_dist_profile(self.h, int(on), ms), "hb_symdense_dist_profile")
         return None if on else tuple(float(v) for v in ms)
 
-    def rbt_stats(self):
-        """(corrections, backward error) of the last RBT solve and the transform time (ms; 0 unless profiling) of the last RBT factorization"""
-        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
-        check(self.ctx.L.hb_symdense_dist_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_dist_rbt_stats")
-        return n.value, be.value, float(ms.value)
 
-
-class LinSolverSymDenseHost:
+class LinSolverSymDenseHost(_DenseSolver):
     """The dense symmetric solver of one GPU with the matrix in page-locked host memory (hb_symdense_host): Cholesky or no-pivot LDL^T,
     streamed through at most `device_bytes` of device memory (0: what is free, less a margin) in slabs of 128-row block rows. It owns
     a pinned n x n host tensor, matrix(); the caller fills its upper triangle, matrixChanged(mode) overwrites that triangle with the
@@ -314,6 +308,7 @@ class LinSolverSymDenseHost:
     accepts RBT_NOPIV; without it RBT_NOPIV is refused (use LinSolverSymDenseDist, or pass rbt=True)."""
 
     NOPIV, CHOLESKY, RBT_NOPIV = _lib.HB_FACT_NOPIV, _lib.HB_FACT_CHOLESKY, _lib.HB_FACT_RBT_NOPIV
+    _C, _HELD = "hb_symdense_host", ("_M", "_K")
 
     def __init__(self, ctx: Context, n: int, device_bytes: int = 0, rbt: bool = False):
         self.ctx, self.n, self.rbt = ctx, n, rbt
@@ -330,13 +325,6 @@ class LinSolverSymDenseHost:
                 self.close()
                 check(rc, "hb_symdense_host_set_rbt_copy")
 
-    def close(self):
-        if self.h:
-            self.ctx.L.hb_symdense_host_destroy(self.h)
-            self.h = None
-            self._M = None
-            self._K = None
-
     def matrix(self) -> torch.Tensor:
         """the pinned n x n row-major host matrix the handle factors in place (upper triangle)"""
         return self._M
@@ -350,22 +338,7 @@ class LinSolverSymDenseHost:
             # the C-ABI's HB_ERR_INVALID would read as the -1 of a breakdown here
             raise EngineError("LinSolverSymDenseHost: only CHOLESKY and NOPIV stream from host memory, and RBT_NOPIV with rbt=True; use "
                               "LinSolverSymDense for Bunch-Kaufman")
-        rc = self.ctx.L.hb_symdense_host_matrix_changed(self.h, mode)
-        if rc < -1:
-            check(rc, "hb_symdense_host_matrix_changed")
-        return rc
-
-    def inertia(self):
-        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        check(self.ctx.L.hb_symdense_host_inertia(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "hb_symdense_host_inertia")
-        return a.value, b.value, c.value
-
-    def solve(self, x: torch.Tensor) -> bool:
-        nrhs = x.numel() // max(self.n, 1) if self.n else 0
-        rc = self.ctx.L.hb_symdense_host_solve(self.h, _ptr(x), nrhs)
-        if rc < 0:
-            check(rc, "hb_symdense_host_solve")
-        return rc == 1
+        return self._matrix_changed(mode)
 
     @staticmethod
     def plan_view(n: int, device_bytes: int) -> dict:
@@ -379,13 +352,6 @@ class LinSolverSymDenseHost:
         check(L.hb_symdense_host_plan_view(n, device_bytes, dims, first, b), "hb_symdense_host_plan_view")
         return {"slabs": dims[0], "blocks": dims[1], "slab_blocks": dims[2], "first": [first[i] for i in range(dims[0] + 1)],
                 "peak_bytes": b[0], "h2d_bytes": b[1], "d2h_bytes_cholesky": b[2], "d2h_bytes_ldlt": b[3], "solve_h2d_bytes": b[4]}
-
-    def rbt_stats(self):
-        """(largest corrections, largest backward error) over the groups of the last RBT solve, and the transform time (ms) of the last
-        RBT factorization"""
-        n, be, ms = ctypes.c_int(), ctypes.c_double(), ctypes.c_float()
-        check(self.ctx.L.hb_symdense_host_rbt_stats(self.h, ctypes.byref(n), ctypes.byref(be), ctypes.byref(ms)), "hb_symdense_host_rbt_stats")
-        return n.value, be.value, float(ms.value)
 
     @staticmethod
     def rbt_plan_view(n: int, device_bytes: int) -> dict:

@@ -119,7 +119,7 @@ def test_dense_kkt_cluster_bunch_kaufman_order(ctx):
     """XDYcYd at N = 600 + 100 + 2 * 150 = 1000, past the cluster Bunch-Kaufman threshold: bit-identical assembly, the inertia, and the
     solve within its backward error bound for the factor read back"""
     from oracle import bounds
-    from test_gpu_symdense_paths import readback, factor_parts, theta
+    from dense_handles import readback, factor_parts, theta
     from hiop_b200.engine import KKTLinSysDense
     H, Jc, Jd, it, pat, deltas = _dominant_problem(600, 100, 150, 43, 0.05)
     Mo, _, _ = ko.dense_build_kkt_matrix(1, H, Jc, Jd, it, pat, deltas)

@@ -134,7 +134,7 @@ def check_exact(r, what):
 def check_real_solve(r, what):
     """with the real factor: [dx_d; dyc; dyd] within the solve's backward error bound for the device's M and the model's rhs (factor read
     back), dx_s = the model's unpack of the device's own dense solution, bit for bit"""
-    from test_gpu_symdense_paths import readback, factor_parts, theta
+    from dense_handles import readback, factor_parts, theta
     p = r.p
     _, Hxs, _ = mm.diagonals(p)
     dx, dyc, dyd = r.solve(identity=False)

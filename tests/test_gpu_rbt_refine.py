@@ -16,8 +16,7 @@ import torch
 from oracle import bounds
 from oracle import rbt_model as rbt
 from test_cpu_rbt_model import known_matrix, PLACED, PLACED_MIN_N, assert_corrected_x, assert_placed, placed_reference, placed_rhs
-from test_gpu_symdense_dist import upper_nan
-from test_gpu_symdense_dist_rbt import make_ctx, gpu_families  # noqa: F401 (make_ctx: a fixture)
+from dense_handles import make_ctx, gpu_families, upper_nan  # noqa: F401 (make_ctx: a fixture)
 from multirank import run_ranks
 
 pytestmark = pytest.mark.gpu

@@ -13,10 +13,11 @@ import torch
 from hiop_b200 import sharding, synth
 from oracle import bounds
 from multirank import run_ranks
+from dense_handles import K128, MDS_FIELDS, factor_dist, factor_parts_from_rows, factor_single, local_rows, matrix, rhs, same_rows
+from dense_handles import make_ctx  # noqa: F401 (a fixture)
 
 CHOL, NOPIV, BK = 2, 1, 0
 ERR_INVALID, ERR_STATE = -1, -5                              # HB_ERR_* of include/hiopb200.h
-K128 = dict(HB_DENSE_BIG_MIN=0, HB_DENSE_PAIR_MIN=1 << 30)   # hb_symdense: look-ahead factorization, blocks unpaired (K = 128)
 
 
 # ---- layout (CPU) -------------------------------------------------------------------------------------------------------------------
@@ -33,114 +34,6 @@ def test_block_rows_cover_every_row_once_block_cyclic(N, world):
 
 
 # ---- single rank -------------------------------------------------------------------------------------------------------------------------
-@pytest.fixture
-def make_ctx(monkeypatch):
-    made = []
-
-    def make(**env):
-        from hiop_b200.engine import Context
-        for k in ("HB_DENSE_PAIR_MIN", "HB_BK_CLUSTER_MIN", "HB_DENSE_BIG_MIN", "HB_CHOL_COOP"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, str(v))
-        c = Context(0)
-        made.append(c)
-        return c
-    yield make
-    for c in made:
-        c.close()
-
-
-def matrix(mode, N, seed, device):
-    """(M, inertia): SPD for Cholesky, a matrix of known inertia with eigenvalues >= 0.5 in modulus for the no-pivot LDL^T"""
-    if mode == CHOL:
-        g = torch.Generator(device="cpu").manual_seed(seed)
-        G = torch.randn((N, N // 2 + 1), generator=g, dtype=torch.float64).to(device)
-        d = torch.rand(N, generator=g, dtype=torch.float64).to(device) * 1.5 + 0.5
-        return G @ G.T / max(N, 1) + torch.diag(d), (0, 0, N)
-    return bounds.known_inertia_matrix(N, 0, N // 3, seed, device=device)
-
-
-def upper_nan(M):
-    U = M.clone()
-    U.masked_fill_(torch.ones(M.shape, dtype=torch.bool, device=M.device).tril_(-1), float("nan"))
-    return U
-
-
-def local_rows(s):
-    """{global row: this rank's stored row (length N)} of a LinSolverSymDenseDist"""
-    torch.cuda.synchronize()
-    s.ctx.sync()
-    loc = s.local()[:, :s.n].cpu().numpy()
-    out = {}
-    for q, (b, e) in enumerate(s.rows):
-        for r in range(b, e):
-            out[r] = loc[q * 128 + r - b]
-    return out
-
-
-def factor_dist(ctx, mode, M, rhs_list):
-    """factor M (device, full) with LinSolverSymDenseDist and solve each rhs (nrhs x N); returns rc, inertia, rows, solutions"""
-    from hiop_b200.engine import LinSolverSymDenseDist
-    N = M.shape[0]
-    s = LinSolverSymDenseDist(ctx, N)
-    torch.cuda.synchronize()
-    s.set_matrix(upper_nan(M))
-    rc = s.matrixChanged(mode)
-    inertia = s.inertia()
-    rows = local_rows(s)
-    sols = []
-    for b in rhs_list:
-        x = ctx.to_device(b)
-        assert s.solve(x)
-        ctx.sync()
-        sols.append(x.cpu().numpy())
-    s.close()
-    return rc, inertia, rows, sols
-
-
-def factor_single(ctx, mode, M):
-    """hb_symdense's factor (row-major, upper valid) of M, its return value and inertia; asserts the look-ahead path at K = 128"""
-    from hiop_b200.engine import LinSolverSymDense
-    from test_gpu_symdense_paths import readback
-    N = M.shape[0]
-    s = LinSolverSymDense(ctx, N, mode)
-    torch.cuda.synchronize()
-    s.set_matrix(upper_nan(M).contiguous())
-    ctx.sync()
-    rc = s.matrixChanged()
-    rb = readback(s)
-    assert rb["plan"] == ("BIG_CHOL" if mode == CHOL else "BIG_LDL", "BIG", "DIAG", False), rb["plan"]
-    inertia = s.inertia()
-    s.close()
-    return rc, inertia, rb["F"]
-
-
-def rhs(N, seed, nrhs):
-    return np.random.default_rng(seed).standard_normal((nrhs, N))
-
-
-def same_rows(rows, F, what):
-    for r, v in rows.items():
-        a, b = v[r:], F[r, r:]
-        if not np.array_equal(a.view(np.uint64), b.view(np.uint64)):
-            bad = np.nonzero(a.view(np.uint64) != b.view(np.uint64))[0]
-            pytest.fail(f"{what}: row {r}: {bad.size} entries differ, first at column {r + bad[0]}: {a[bad[0]]!r} vs {b[bad[0]]!r}")
-
-
-def factor_parts_from_rows(rows, N, mode):
-    """(L, d) on the host from the stored rows (row r of the row-major upper triangle = column r of L)"""
-    Lt = np.zeros((N, N))
-    for r, v in rows.items():
-        Lt[r, r:] = v[r:]
-    L = Lt.T.copy()
-    if mode == CHOL:
-        return L, np.ones(N)
-    d = np.diag(L).copy()
-    np.fill_diagonal(L, 1.0)
-    return L, d
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("mode", [CHOL, NOPIV], ids=["chol", "nopiv"])
 @pytest.mark.parametrize("N", [1, 127, 128, 129, 1000, 4099, 8192])
@@ -214,10 +107,6 @@ def test_failure_and_misuse(make_ctx):
 
 
 # ---- mixed dense-sparse, one rank ------------------------------------------------------------------------------------------------------
-MDS_FIELDS = ("Hd", "Hs_diag", "Jcd", "Jdd", "Jcs_vals", "Jds_vals", "vl", "sdl", "vu", "sdu", "idl", "idu", "delta_wx", "delta_wd", "delta_cc",
-              "delta_cd")
-
-
 def mds_run(ctx, p, dist):
     """build (single and distributed), factor the distributed matrix with the no-pivot LDL^T, solve; returns (M, rows, ret, dx, dyc, dyd)"""
     from hiop_b200.engine import KKTLinSysCompressedMDSXYcYd

@@ -3,9 +3,6 @@ oracle/rbt_model.py, its factor bit for bit against hb_symdense's no-pivot facto
 Bunch-Kaufman, the refined solve, failure and resources, the mixed dense-sparse step in stable mode, and P = 2, 4 against P = 1.
 
 Single-rank cases run on one GPU. Multi-rank cases spawn one process per GPU and skip when fewer GPUs are present."""
-from types import SimpleNamespace
-import pathlib
-
 import numpy as np
 import pytest
 import torch
@@ -13,70 +10,12 @@ import torch
 from hiop_b200 import sharding, synth
 from oracle import bounds
 from oracle import rbt_model as rbt
-from test_cpu_rbt_model import FAMILIES
-from test_gpu_symdense_dist import K128, local_rows, upper_nan, factor_single, same_rows, factor_parts_from_rows
 from multirank import run_ranks
+from dense_handles import (GOLDEN, K128, MDS_FIELDS, SOLVE_REL, bk_single, factor_parts_from_rows, factor_single, golden_mds, gpu_families,
+                           local_rows, orig_backward_error, rbt_dist, same_rows, upper_nan)
+from dense_handles import make_ctx  # noqa: F401 (a fixture)
 
 RBT, NOPIV, CHOL, BK = 3, 1, 2, 0
-GOLDEN = pathlib.Path(__file__).parent / "golden"
-SOLVE_REL = 1e3 * 2.0 ** -52     # |x - x_bk|_inf / |x_bk|_inf <= SOLVE_REL * cond_inf(A): both solves are backward stable
-
-
-@pytest.fixture
-def make_ctx(monkeypatch):
-    made = []
-
-    def make(**env):
-        from hiop_b200.engine import Context
-        for k in ("HB_DENSE_PAIR_MIN", "HB_BK_CLUSTER_MIN", "HB_DENSE_BIG_MIN", "HB_CHOL_COOP"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, str(v))
-        c = Context(0)
-        made.append(c)
-        return c
-    yield make
-    for c in made:
-        c.close()
-
-
-def bk_single(ctx, A):
-    """hb_symdense Bunch-Kaufman on A (numpy, full): return value and inertia"""
-    from hiop_b200.engine import LinSolverSymDense
-    N = A.shape[0]
-    s = LinSolverSymDense(ctx, N, BK)
-    torch.cuda.synchronize()
-    s.set_matrix(torch.from_numpy(np.ascontiguousarray(A)).to(ctx.device))
-    ctx.sync()
-    rc = s.matrixChanged()
-    inr = s.inertia()
-    s.close()
-    return rc, inr
-
-
-def rbt_dist(ctx, A, rhs=None, mode=RBT):
-    """factor A (numpy, full) on a LinSolverSymDenseDist in `mode`; solve rhs (N x nrhs) when given. Returns rc, inertia, rows, x, stats"""
-    from hiop_b200.engine import LinSolverSymDenseDist
-    N = A.shape[0]
-    s = LinSolverSymDenseDist(ctx, N)
-    torch.cuda.synchronize()
-    s.set_matrix(upper_nan(torch.from_numpy(np.ascontiguousarray(A)).to(ctx.device)))
-    rc = s.matrixChanged(mode)
-    inr = s.inertia()
-    rows = local_rows(s)
-    x = stats = None
-    if rhs is not None and rc >= 0:
-        xd = ctx.to_device(np.ascontiguousarray(rhs.T))
-        assert s.solve(xd)
-        ctx.sync()
-        x = xd.cpu().numpy().T.copy()
-        stats = s.rbt_stats()
-    s.close()
-    return rc, inr, rows, x, stats
-
-
-def orig_backward_error(A, x, b):
-    return rbt.backward_error(A, x, b)
 
 
 # ---- one rank -------------------------------------------------------------------------------------------------------------------------
@@ -113,14 +52,6 @@ def test_transform_and_factor_bit_identical_to_the_model(make_ctx, N):
     assert corr <= 3 and om <= 4 * rbt.EPS, (corr, om)
     assert orig_backward_error(A, x, b) <= 1e-14
     torch.cuda.empty_cache()
-
-
-def gpu_families():
-    for name, A in FAMILIES.items():
-        yield name, A
-    yield "known_2x2_1000", bounds.known_inertia_matrix(1000, 200, 250, seed=9)[0].numpy()
-    from test_cpu_rbt_model import saddle
-    yield "saddle_1500_500", saddle(1500, 500, 11, 300)
 
 
 @pytest.mark.gpu
@@ -177,10 +108,6 @@ def test_zero_row_fails_and_the_handle_stays_usable(make_ctx):
 
 
 # ---- mixed dense-sparse in stable mode ------------------------------------------------------------------------------------------------
-MDS_FIELDS = ("Hd", "Hs_diag", "Jcd", "Jdd", "Jcs_vals", "Jds_vals", "vl", "sdl", "vu", "sdu", "idl", "idu", "delta_wx", "delta_wd", "delta_cc",
-              "delta_cd")
-
-
 def mds_stable(ctx, p):
     """single-GPU KKTLinSysCompressedMDSXYcYd(safe_mode=True) and factorizeWithCurvCheck_dist(safe_mode=True) on the same inputs"""
     from hiop_b200.engine import KKTLinSysCompressedMDSXYcYd, LinSolverSymDenseDist
@@ -207,11 +134,6 @@ def mds_stable(ctx, p):
             d.close()
         k.close()
     return out
-
-
-def golden_mds():
-    g = dict(np.load(GOLDEN / "mds_nxs50_nxd20.npz"))
-    return SimpleNamespace(**{k: (v if v.ndim else v.item()) for k, v in g.items() if not k.startswith("ref_")})
 
 
 MDS_REL = 1e-9      # both are backward-stable solves of a system of moderate condition

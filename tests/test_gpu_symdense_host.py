@@ -11,59 +11,11 @@ import torch
 
 from hiop_b200 import synth
 from oracle import bounds
-from test_gpu_symdense_dist import K128, factor_dist, make_ctx, matrix, rhs, same_rows, upper_nan  # noqa: F401 (make_ctx: fixture)
+from dense_handles import K128, assert_lower_untouched, budget_for, budgets, dist_rows_array, factor_dist, matrix, plan, rhs, same_rows, upper_nan
+from dense_handles import make_ctx  # noqa: F401 (a fixture)
 
 CHOL, NOPIV, BK, RBT = 2, 1, 0, 3
 ERR_INVALID, ERR_STATE = -1, -5
-
-
-def plan(N, budget):
-    from hiop_b200.engine import LinSolverSymDenseHost
-    return LinSolverSymDenseHost.plan_view(N, budget)
-
-
-def budget_for(N, slabs):
-    """the smallest budget whose plan has at most `slabs` slabs (1 << 40: one slab)"""
-    lo, hi = 1, 1 << 40
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        try:
-            ok = plan(N, mid)["slabs"] <= slabs
-        except Exception:
-            ok = False
-        hi, lo = (mid, lo) if ok else (hi, mid)
-    return hi
-
-
-def budget_for_height(N, H):
-    """the smallest budget whose plan puts at least H block rows in a slab"""
-    lo, hi = 1, 1 << 40
-    while hi - lo > 1:
-        mid = (lo + hi) // 2
-        try:
-            ok = plan(N, mid)["slab_blocks"] >= H
-        except Exception:
-            ok = False
-        hi, lo = (mid, lo) if ok else (hi, mid)
-    return hi
-
-
-def budgets(N):
-    """{one slab, two slabs, one block row per slab, three slabs with a shorter last one}, each once"""
-    nblk = -(-N // 128)
-    out = {}
-    for name, n in (("one_slab", 1), ("two_slabs", 2), ("row_per_slab", nblk)):
-        b = budget_for(N, n)
-        if all(plan(N, b)["slabs"] != plan(N, v)["slabs"] for v in out.values()):
-            out[name] = b
-    # the first slab height that gives three slabs with a remainder, so that the last slab has fewer block rows
-    H = next((h for h in range(1, nblk) if -(-nblk // h) == 3 and nblk % h), None)
-    if H is not None:
-        b = budget_for_height(N, H)
-        p = plan(N, b)
-        assert p["slabs"] == 3 and p["first"][3] - p["first"][2] < p["first"][1] - p["first"][0], p
-        out["three_slabs_short_last"] = b
-    return out
 
 
 def host_factor(ctx, mode, M, budget, rhs_list):
@@ -84,20 +36,6 @@ def host_factor(ctx, mode, M, budget, rhs_list):
     F = s.matrix().numpy().copy()
     s.close()
     return rc, inertia, F, sols
-
-
-def dist_rows_array(rows, N):
-    F = np.zeros((N, N))
-    for r, v in rows.items():
-        F[r] = v[:N]
-    return F
-
-
-def assert_lower_untouched(F, M, what):
-    """the strictly lower triangle of the buffer still holds upper_nan's NaNs, bit for bit"""
-    low = np.tril(np.ones(F.shape, dtype=bool), -1)
-    want = upper_nan(M).cpu().numpy()
-    assert np.array_equal(F[low].view(np.uint64), want[low].view(np.uint64)), what
 
 
 def factor_parts(F, mode):

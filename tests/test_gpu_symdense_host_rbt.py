@@ -11,9 +11,9 @@ import torch
 
 from oracle import bounds
 from oracle import rbt_model as rbt
-from test_gpu_symdense_dist import K128, local_rows, make_ctx, matrix, rhs, same_rows, upper_nan  # noqa: F401 (make_ctx: fixture)
-from test_gpu_symdense_host import assert_lower_untouched, budget_for, budgets, dist_rows_array, plan
-from test_gpu_symdense_dist_rbt import bk_single, gpu_families, orig_backward_error
+from dense_handles import (K128, assert_lower_untouched, bk_single, budget_for, budgets, dist_rows_array, gpu_families, local_rows, matrix,
+                           orig_backward_error, plan, rhs, same_rows, upper_nan)
+from dense_handles import make_ctx  # noqa: F401 (a fixture)
 
 RBT, NOPIV = 3, 1
 ERR_INVALID, ERR_STATE = -1, -5

@@ -6,8 +6,6 @@ known by construction, and the Bunch-Kaufman pivots against LAPACK's dsytrf. Eac
 the dispatch chose, so a threshold change cannot silently move a case to another path. The branches that are not the default at these
 sizes are forced through the environment knobs hb_dense_init reads once per context (HB_DENSE_PAIR_MIN, HB_BK_CLUSTER_MIN,
 HB_DENSE_BIG_MIN, HB_CHOL_COOP)."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
@@ -17,35 +15,12 @@ from hiop_b200 import synth
 from oracle import bounds
 from oracle import kkt_oracle as ko
 from test_gpu_parity import _setup_kkt, _as_dict, _kkt_residual
+from dense_handles import DEV, factor_parts, make_ctx, readback, theta  # noqa: F401 (make_ctx: fixture)
 
 pytestmark = pytest.mark.gpu
 
-# enum order of Factor / Solve / Inertia in hb_symdense.cu
-FACTOR = ("SYTF2", "SYTRF_BLOCKED", "BK_CLUSTER", "PANEL_CHOL", "PANEL_LDL", "COOP_CHOL", "BIG_CHOL", "BIG_LDL")
-SOLVE = ("SYTRS", "ONE_CTA", "BIG")
-INERTIA = ("IPIV", "BLOCKDIAG", "DIAG")
 BK, NOPIV, CHOL = 0, 1, 2
-DEV = torch.device("cuda", 0)
 DSYTRF_MAX_N = 7001      # pivot sequence and factor compared with scipy's dsytrf up to this order
-
-
-@pytest.fixture
-def make_ctx(monkeypatch):
-    """Context(0) created under the given environment (hb_dense_init reads the knobs once per context)"""
-    made = []
-
-    def make(**env):
-        from hiop_b200.engine import Context
-        for k in ("HB_DENSE_PAIR_MIN", "HB_BK_CLUSTER_MIN", "HB_DENSE_BIG_MIN", "HB_CHOL_COOP"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, str(v))
-        c = Context(0)
-        made.append(c)
-        return c
-    yield make
-    for c in made:
-        c.close()
 
 
 # ---- matrices -------------------------------------------------------------------------------------------------------------------------
@@ -85,51 +60,9 @@ def set_matrix(s, M):
 
 
 # ---- one factorization, read back -----------------------------------------------------------------------------------------------------
-def readback(s):
-    N = s.n
-    plan = (ctypes.c_int * 4)()
-    widths = ctypes.c_int()
-    F = np.empty((N, N))
-    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    plan_only = lambda: s.ctx.L.hb_debug_symdense_factor(s.h, plan, ctypes.byref(widths), None, None, None, None)
-    from hiop_b200._lib import check
-    check(plan_only(), "hb_debug_symdense_factor")
-    bkc = FACTOR[plan[0]] == "BK_CLUSTER"
-    ipiv = np.empty(N, dtype=np.int32) if FACTOR[plan[0]] in ("SYTF2", "SYTRF_BLOCKED", "BK_CLUSTER") else None   # pivoting factors only
-    perm = np.empty(N, dtype=np.int32) if bkc else None
-    dsub = np.empty(N) if bkc else None
-    check(s.ctx.L.hb_debug_symdense_factor(s.h, None, None, p(F), p(ipiv) if ipiv is not None else None, p(perm) if bkc else None, p(dsub) if bkc else None),
-          "hb_debug_symdense_factor")
-    return dict(plan=(FACTOR[plan[0]], SOLVE[plan[1]], INERTIA[plan[2]], bool(plan[3])), widths=widths.value, F=F, ipiv=ipiv, perm=perm,
-                dsub=dsub)
-
-
 def _same(a, b):
     """bitwise equal, None (no such output for this factor) only with None"""
     return (a is None and b is None) or (a is not None and b is not None and np.array_equal(a, b))
-
-
-def factor_parts(rb):
-    """(L, d, dsub, perm) of the factor read back, on the device; P A P^T = L D L^T"""
-    f = rb["plan"][0]
-    N = rb["F"].shape[0]
-    if f in ("SYTF2", "SYTRF_BLOCKED"):                          # LAPACK's 'L' storage and pivots
-        L, d, dsub, perm = bounds.lapack_to_permuted(rb["F"].T.copy(), rb["ipiv"].astype(np.int64))
-        t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(DEV)
-        return t(L), t(d), t(dsub), perm
-    Fl = torch.from_numpy(rb["F"]).to(DEV).T.tril()
-    if f.endswith("CHOL"):
-        return Fl.contiguous(), torch.ones(N, dtype=torch.float64, device=DEV), None, np.arange(N)
-    d = torch.diagonal(Fl).clone()
-    L = Fl.tril(-1) + torch.eye(N, dtype=torch.float64, device=DEV)
-    if f == "BK_CLUSTER":
-        return L, d, torch.from_numpy(rb["dsub"]).to(DEV), rb["perm"].astype(np.int64)
-    return L, d, None, np.arange(N)
-
-
-def theta(L):
-    """explicit diagonal-block inverses: 16 x 16 (k_trsm_panel, cooperative paths) and 128 x 128 (look-ahead, blocked solves)"""
-    return max(bounds.block_theta(L, 16), bounds.block_theta(L, 128))
 
 
 def run_case(ctx, mode, N, seed, expect, widths=None, nrhs_list=(1, 7, 8)):

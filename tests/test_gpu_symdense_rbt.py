@@ -12,9 +12,8 @@ import torch
 
 from oracle import bounds
 from oracle import rbt_model as rbt
-from test_gpu_symdense_dist import K128, upper_nan
-from test_gpu_symdense_dist_rbt import make_ctx, bk_single, rbt_dist, gpu_families, golden_mds, orig_backward_error, MDS_FIELDS, SOLVE_REL  # noqa: F401
-from test_gpu_symdense_paths import readback
+from dense_handles import K128, MDS_FIELDS, SOLVE_REL, bk_single, golden_mds, gpu_families, orig_backward_error, rbt_dist, readback, upper_nan
+from dense_handles import make_ctx  # noqa: F401 (a fixture)
 from test_gpu_dropin_drivers import REF, ROW, _compare, _tables_agree
 
 pytestmark = pytest.mark.gpu
